@@ -4,7 +4,7 @@ metric : env-steps/sec over collect+update (the reference's ``train_speed``, fsr
 step   : ONE collect + update cycle (trainer.train_step + policy_update_fn)
 configs: --config c1 | c2 (default, the headline) | c3 | c4 | c5   (BASELINE.json "configs", in order)
 
-  python bench.py [--config c2] [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--config c2] [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Prints one JSON line (rank 0).  See DESIGN.md "Measurement" for how every field is derived.
 """
@@ -50,7 +50,8 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 rate -- upper bounds, not measured here
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -195,15 +196,10 @@ def ppo_rooflines(cfg, agent, col, buf, T, device, pk, how):
     fl = net_flops(D, H, A, cfg["batch"]) * n_mb
     ach = fl / (ms_rep * 1e-3) / 1e12
     peak = pk["bf16_tflops_sustained"]
-    traffic_file = os.path.join(ROOT, "profiles", "r2_ppo_persist_traffic.json")
-    # the captured DRAM traffic belongs to the persistent launch; the chain's (H != 256) is in profiles/r1_ppo_update_ncu_summary.txt
-    traffic = json.load(open(traffic_file)) if (persistent and os.path.exists(traffic_file)) else None
-    roof = {"kernel": "ppo_persist_kernel (one launch per repeat: tcgen05 kind::tf32 3-term split, TMEM accumulators, bulk-copy "
+    roof = {"kernel": "ppo_persist_kernel (one launch per repeat: wgmma kind tf32 3-term split, register accumulators, bulk-copy "
                       "operand images)" if persistent else "ppo_fwd/bwd/wgrad_adam chain (three launches per minibatch)",
             "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
-            "traffic": traffic["dram_bytes_per_launch"] if traffic else None,
-            "traffic_unit": "DRAM bytes read+written per launch (ncu --set full --cache-control none, "
-                            "profiles/r2_ppo_persist_ncu_summary.txt)" if traffic else None,
+            "traffic": None, "traffic_unit": None,
             "peak_source": how + " bf16 sustained (kernel timed inside a long step)",
             "ms_per_launch": ms_rep, "minibatch_steps_per_launch": n_mb, "us_per_minibatch_step": ms_rep * 1e3 / n_mb,
             "launches_per_repeat": launches_rep, "persistent": persistent,
@@ -281,6 +277,8 @@ def run_ours(args):
     ev1.record()
     torch.cuda.synchronize()
     launches = int(_fl.lib.fsrl_launch_count()) - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, agent, buf)
     ms = ev0.elapsed_time(ev1)
     if dist is not None:
         t = torch.tensor([ms], device=device)
@@ -376,6 +374,23 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+DUMP_ROWS = 65536      # transitions of the rollout / replay buffer written by --dump-outputs
+
+
+def dump_outputs(out_dir, agent, buf):
+    """What the timed path computed in its last collect+update cycle, as float32 .npy files for an output-for-output
+    comparison of two builds: the flat parameter vector after the update and the buffer fields the collect wrote, on a
+    fixed seeded sample of DUMP_ROWS transitions (the same rows in every run of a config)."""
+    os.makedirs(out_dir, exist_ok=True)
+    theta = agent.policy.arena.theta.detach().float().cpu().numpy()
+    np.save(os.path.join(out_dir, "theta.npy"), theta)
+    n = int(buf.obs.shape[0])
+    rows = np.sort(np.random.default_rng(0).choice(n, size=min(n, DUMP_ROWS), replace=False))
+    idx = torch.from_numpy(rows).to(buf.obs.device)
+    for name in ("obs", "obs_next", "act", "rew", "cost", "logp", "terminated", "truncated"):
+        np.save(os.path.join(out_dir, name + ".npy"), getattr(buf, name).index_select(0, idx).float().cpu().numpy())
+
+
 def other_roofline(cfg, agent, steps_per_cycle, ms_cycle, collect_s, pk, how):
     """CPO: Fisher/Hessian-vector products dominate (~ 4 x 2 N P flops each, SURVEY.md 8d); SAC: latency of a gradient step."""
     s0 = agent.policy.arena.slots[0]
@@ -402,12 +417,12 @@ def other_roofline(cfg, agent, steps_per_cycle, ms_cycle, collect_s, pk, how):
 # reference arm / cpu_baseline: the reference's own classes on the host cores (oracle/refarm.py)
 # -------------------------------------------------------------------------------------------------
 def _reference_dir():
-    d = os.path.join(ROOT, "baseline", "_ref")
+    d = os.path.join(ROOT, "oracle", "_ref")
     return d if os.path.isdir(os.path.join(d, "fsrl")) else None
 
 
 def cpu_reference(config="c2", sample_envs=32, cycles=1, threads=None, runner=None):
-    """One or more collect+update cycles of the UNMODIFIED reference (baseline/_ref): fsrl.data.FastCollector over one worker
+    """One or more collect+update cycles of the UNMODIFIED reference (oracle/_ref): fsrl.data.FastCollector over one worker
     PROCESS per env (tianshou SubprocVectorEnv protocol; the simulator inside a worker is the numpy twin of the device env
     model, pybullet / mujoco being absent), fsrl.policy.PPOLagrangian.process_fn + learn.  c1 runs verbatim (4 envs); the other
     PPO configs run their network / batch shapes on a bounded sample of `sample_envs` envs (one process per env does not
@@ -418,7 +433,8 @@ def cpu_reference(config="c2", sample_envs=32, cycles=1, threads=None, runner=No
         return cpu_port_other(cfg, sample_envs)
     ref_dir = _reference_dir()
     if ref_dir is None:
-        raise SystemExit("baseline/_ref is missing: run __graft_entry__.build() in the build container first")
+        return {"value": None, "unit": "env-steps/s", "kind": "reference",
+                "unavailable": "oracle/_ref missing (build() installs the reference there when its sources are present)"}
     from oracle import refarm
     n_env = cfg["envs"] if config == "c1" else min(sample_envs, cfg["envs"])
     threads = threads or 4                                        # the reference's default (ppol_cfg.py:11 thread = 4)
@@ -436,7 +452,7 @@ def cpu_reference(config="c2", sample_envs=32, cycles=1, threads=None, runner=No
             "torch_threads": threads, "kind": "reference", "collect_s": tc, "update_s": tu,
             "same_config": config == "c1",
             "sample": f"{n_env} envs x {runner.T} steps x {cycles} cycle(s), {cfg['hidden'][0]}-wide MLPs, batch {cfg['batch']}, "
-                      f"repeat {cfg['repeat']}: unmodified fsrl.data.FastCollector + fsrl.policy.PPOLagrangian from baseline/_ref "
+                      f"repeat {cfg['repeat']}: unmodified fsrl.data.FastCollector + fsrl.policy.PPOLagrangian from oracle/_ref "
                       f"(no fsrl_b200 import), one env worker process per env, torch.set_num_threads({threads}) (reference default); "
                       f"collect {tc:.1f} s + update {tu:.1f} s"}
 
@@ -460,7 +476,7 @@ def run_reference(args):
     from oracle import refarm
     ref_dir = _reference_dir()
     if ref_dir is None:
-        print(json.dumps({"impl": "reference", "unavailable": "baseline/_ref missing (build() installs it)"}))
+        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref missing (build() installs it)"}))
         return
     n_env = cfg["envs"] if args.config == "c1" else min(args.cpu_envs, cfg["envs"])
     threads = 4
@@ -499,6 +515,8 @@ if __name__ == "__main__":
     ap.add_argument("--cpu-envs", type=int, default=32,
                     help="envs (= worker processes) of the bounded CPU sample for configs other than c1")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the parameters and a seeded buffer sample of the last timed cycle to DIR/<name>.npy")
     a = ap.parse_args()
     if a.impl == "reference":
         run_reference(a)

@@ -1,4 +1,4 @@
-"""fsrl_b200 -- B200-native (sm_100a) hot path for safe RL behind FSRL's API surface.
+"""fsrl_b200 -- H100-native (sm_90a) hot path for safe RL behind FSRL's API surface.
 
 Only the data-parallel hot path of liuzuxin/FSRL lives here (SURVEY.md section 8): rollout
 collection + dual GAE, and the constrained policy updates, as hand-written CUDA behind the

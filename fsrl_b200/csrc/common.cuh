@@ -1,4 +1,4 @@
-// Shared device/host helpers for the fsrl_b200 kernels (sm_100a only).
+// Shared device/host helpers for the fsrl_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -46,7 +46,7 @@ extern unsigned long long g_launches;  // kernels launched by this library (host
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-int sm_count();  // cached cudaDevAttrMultiProcessorCount of the current device (148 on B200)
+int sm_count();  // cached cudaDevAttrMultiProcessorCount of the current device (132 on an H100 SXM)
 
 // ---- device helpers -------------------------------------------------------------------
 __device__ __forceinline__ double shfl_up_f64(double v, int d) {

@@ -12,8 +12,8 @@
 // split into hi = tf32(x), lo = tf32(x - hi) and the product is accumulated as
 // a_lo*b_hi + a_hi*b_lo + a_hi*b_hi in fp32 (mma.sync.m16n8k8.tf32), i.e. ~2^-21 relative
 // error per product -- indistinguishable from an fp32 FMA chain at the parity tolerances.
-// The row tiles here are 16..64 rows (a 256-row minibatch split over 16 CTAs), far below the
-// 128-row atoms of tcgen05, and the kernels are latency- not throughput-bound, so the
+// The row tiles here are 16..64 rows (a 256-row minibatch split over 16 CTAs), at or below the
+// 64-row atom of a wgmma warpgroup, and the kernels are latency- not throughput-bound, so the
 // warp-level mma path is the right tensor-core granularity for this workload.
 //
 // Thread mapping (256 threads = 8 warps): a CTA owns R rows (R = 4096/H, at least 16); warp w
@@ -68,8 +68,7 @@ struct MlpTile {
 
 // x = hi + lo with hi, lo representable in TF32 (10 explicit mantissa bits).  Round-to-nearest,
 // ties away from zero -- the result of cvt.rna.tf32.f32 -- done with integer ops: the cvt runs on
-// the quarter-rate conversion pipe and was the bound of every split-operand GEMM here
-// (measured: tools/micro/mma_rate.cu, profiles/r1_mma_rate.txt).
+// the quarter-rate conversion pipe, which would otherwise bound every split-operand GEMM here.
 __device__ __forceinline__ uint32_t round_tf32(float x) { return (__float_as_uint(x) + 0x1000u) & 0xffffe000u; }
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
     hi = round_tf32(x);

@@ -446,7 +446,7 @@ __global__ void ppo_gather_kernel(const fsrl_ppo_update_t u, long long n) {
 constexpr int WG_TPB = 256, WG_T = 64, WG_TKT = 32, WG_RC = 128, WG_NST = 2, WG_LD = WG_T + 8;   // LD = 8 mod 32: conflict-free fragments
 // shared memory of a weight-gradient role: WG_NST stages x (L chunk + G chunk), each [WG_RC][WG_LD]
 // (re-used as the cross-warp reduce buffer), then fin[80][WG_T] (layer-1 results) and 256 partials.
-// (measured: 64-row chunks x 3 stages, 132 KB, which would let a forward CTA co-reside, is 4% slower)
+// (64-row chunks x 3 stages, 132 KB, would let a forward CTA co-reside; the two have not been compared on H100)
 constexpr size_t WG_SMEM_FLOATS = 2 * WG_NST * (size_t)WG_RC * WG_LD + 80 * WG_T + 256;
 static_assert(2 * WG_NST * WG_RC * WG_LD >= 8 * 32 * (WG_T + 8), "reduce buffer must fit in the staging area");
 
@@ -1155,7 +1155,7 @@ static int ppo_launch_minibatch(const fsrl_ppo_update_t& u, int mb_off, int B, i
         // single GPU: gradients never leave the registers -- tiles -> norm -> barrier -> clip + Adam
         AdamStep ad = {(float)(1.0 - b1), (float)b2, (float)(1.0 - b2), bc2s, (float)u.adam_eps, neg_step};
         unsigned long long target = (unsigned long long)(bar_count + 1) * gB.x * gB.y;
-        // Ordinary (not cooperative) launch: measured 4.6 % faster per cycle.  The grid barrier is still
+        // Ordinary (not cooperative) launch: no cooperative-launch overhead per step.  The grid barrier is still
         // safe: fuse_ok guarantees grid <= SMs x CTAs/SM, every CTA of the grid becomes resident without
         // waiting on anything but the barrier (the preceding bwd CTAs drain unconditionally, the next fwd
         // CTAs are only scheduled after ALL of these have triggered), and grid_barrier traps after 20 s

@@ -1,39 +1,40 @@
-// Persistent PPO-Lagrangian update: ONE launch per repeat runs every minibatch step of
-// /root/reference/fsrl/policy/ppo_lag.py:223-247 (forward, clipped-surrogate + lambda * cost-advantage
-// loss and value losses :152-212, lagrangian_base.py:145-166, backward, clip_grad_norm_, Adam) on a
-// co-resident grid of 32 CTAs per network.  Blackwell-native data path: the three 256^3 GEMMs of a
-// network and step run on tcgen05 tensor cores (kind::tf32, fp32-faithful 3-term split, accumulators
-// in tensor memory), operands arrive as bulk asynchronous copies (TMA unit) of pre-split "plane
-// layout" images that the producing CTAs write straight from their epilogues, and the CTAs of a
-// step are chained by device-scope release/acquire counters instead of kernel launches.
+// Persistent PPO-Lagrangian update: ONE launch per repeat runs every minibatch step of the reference's
+// fsrl/policy/ppo_lag.py:223-247 (forward, clipped-surrogate + lambda * cost-advantage loss and value losses
+// :152-212, lagrangian_base.py:145-166, backward, clip_grad_norm_, Adam) on a co-resident grid of 32 CTAs per
+// network.  Hopper data path: the three 256^3 GEMMs of a network and step run on the warpgroup tensor cores
+// (wgmma kind tf32, fp32-faithful 3-term split, accumulators in registers), operands arrive as bulk asynchronous
+// copies (TMA unit) of pre-split "plane layout" images that the producing CTAs write straight from their epilogues,
+// and the CTAs of a step are chained by device-scope release/acquire counters instead of kernel launches.
 //
 // Work decomposition of one network (H = 256, minibatch = 256 rows = 4 row blocks of 64):
 //   CTA c = 8 a + b           a = row block (4), b = 32-wide column block (8)
 //   S   h1 tile   [64 r x 32 k]   FFMA (K = D)            -> images H1A (MN = r, K = k), H1T (MN = k, K = r)
-//   G1  h2 tile   [64 r x 32 o] = h1[r, :] W2t[:, o]      A = H1A block a, B = W2A block b      (tcgen05)
+//   G1  h2 tile   [64 r x 32 o] = h1[r, :] W2t[:, o]      A = H1A block a, B = W2A block b      (wgmma)
 //       head partial over the tile's 32 columns -> 8 partials per row block -> loss gradient dOut
 //       dz2 tile = (dOut W3^T) * relu'(h2)                -> images DZA (MN = r, K = o), DZT (MN = o, K = r)
 //   G2  (CTAs 0-15: ka = c / 4, rb = c % 4)  dh1^T tile [64 k x 64 r] = W2t[k, :] dz2[r, :]^T
 //       A = W2B block ka, B = DZA block rb;  * relu'(h1) -> partial dW1 / db1 over the 64 rows
 //   G3  (CTAs 16-31: ka, ob = c % 4)         dW2^T tile [64 o x 64 k] = dz2[:, o]^T h1[:, k]
-//       A = DZT block ob, B = H1T block ka;  the CTA owns this tile of W2: Adam state (p, m, v) lives in
-//       tensor memory for the whole launch, the updated tile is re-published as images W2A / W2B
+//       A = DZT block ob, B = H1T block ka;  the CTA owns this tile of W2: its Adam state (p, m, v) lives in the
+//       epilogue threads' registers for the whole launch, the updated tile is re-published as images W2A / W2B
 //   small parameters (W1, b1, b2, W3, b3, log sigma): every CTA keeps the slices it consumes (+ their
 //       Adam moments) in shared memory and applies the identical update to them (deterministic
 //       replicas); gradients are fixed-order sums of per-row-block partials.
 //   global-norm clip: per-CTA sums of squares -> one device-wide counter hop -> every CTA adds the
 //       96 partials in the same order.
-// All operand images are K-major SWIZZLE_NONE plane images (umma.cuh); transposed copies are written
-// by the producer (MN-major tf32 operands would need the 128B_BASE32B swizzle).
+// All operand images are K-major no-swizzle plane images (wgmma.cuh); transposed copies are written by the producer
+// (wgmma reads tf32 operands K-major only).
 //
-// CTA = 320 threads: warp 0 bulk-copy producer, warp 1 MMA issuer, warps 2-9 epilogue (two per tensor-memory
-// subpartition).  The 8 CTAs of a row block form a thread-block cluster: their head partials travel over distributed
-// shared memory (st.async + mbarrier complete_tx); all other hops are flag lines in L2.  The cross terms of the 3-term
-// split accumulate in their own tensor-memory columns (TM_C).  With world > 1 the <DP = true> instantiation exchanges
-// gradients itself over peer memory (dp_* functions below: tagged + hashed 16-byte packets pushed into the peers' buffers).
-// DESIGN.md 3a / 6 hold the measurements behind these choices.
+// CTA = 288 threads: warps 0-7 (two warpgroups) issue the MMAs and run the epilogue, warp 8 is the bulk-copy producer.
+// Warp w holds rows 16 (w % 4) .. + 15 of a 64-row tile; warpgroup w / 4 computes the 8-column groups its threads own
+// in the epilogue, so an accumulator tile goes from the wgmma fragment to the epilogue layout through a per-warp
+// region of shared memory without any barrier.  The 8 CTAs of a row block form a thread-block cluster: their head
+// partials travel over distributed shared memory (st.async + mbarrier complete_tx); all other hops are flag lines in
+// L2.  The cross terms of the 3-term split accumulate in their own registers.  With world > 1 the <DP = true>
+// instantiation exchanges gradients itself over peer memory (dp_* functions below: tagged + hashed 16-byte packets
+// pushed into the peers' buffers).
 #include "ppo_persist.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include <cstdlib>
 #include <cmath>
 #include <vector>
@@ -41,16 +42,19 @@
 namespace fsrl {
 namespace pp {
 
-using namespace umma;
+using namespace wg;
 
-constexpr int WQ = 2;                    // epilogue warps per tensor-memory subpartition (1 or 2)
-constexpr int NEPI = 128 * WQ;           // epilogue threads: warps 2 .. 2 + 4 WQ - 1
-constexpr int TPB = 64 + NEPI;           // warp 0: copy producer, warp 1: MMA issuer, then the epilogue warps
+constexpr int WQ = 2;                    // epilogue warpgroups = warps that share the rows of a 16-row slab
+constexpr int NEPI = 128 * WQ;           // epilogue (and MMA) threads: warps 0 .. 4 WQ - 1
+constexpr int TPB = NEPI + 32;           // + the bulk-copy producer warp
 constexpr int C1 = 16 / WQ;              // columns a thread owns of a 32-column tile (G1: h2 / dz2)
 constexpr int C2 = 32 / WQ;              // columns a thread owns of a 64-column tile (G2 / G3 and the W2 tile)
 constexpr int RB = 64;                   // rows per row block
 constexpr int MB = 256;                  // rows per minibatch
-constexpr int SLOT_BYTES = 65536, NSLOT = 3;
+constexpr int KC = 32, NCH = 256 / KC;   // k per operand chunk, chunks per GEMM
+constexpr int SLOT_BYTES = 32768, NSLOT = 4;   // chunk: A hi | A lo | B hi | B lo, 64 (G1: B 32) rows x KC each
+constexpr int A_CHUNK = 64 * KC * 4;     // bytes of one 64-row operand chunk
+constexpr int ACC_LD = 68;               // row stride (floats) of the staged accumulator tile [64][ACC_LD]
 constexpr int OUTP = 8;                  // padded head width
 constexpr int H_ = 256;
 constexpr int IMG = 65536;               // floats per image (256 x 256)
@@ -67,23 +71,18 @@ constexpr int SUMSQ_FLOATS = 128;                               // global tail: 
 // flag lines (32 unsigned each): per net A, C, D1, B[4]; global D2
 constexpr int FLAG_LINE = 32;
 constexpr int F_A = 0, F_C = 1, F_D1 = 2, F_B = 3, F_PER_NET = 7;
-constexpr int TM_COLS = 512, TM_P = 64, TM_M = 96, TM_V = 128;  // tensor-memory columns: [0,64) accumulators, Adam state
-// The two cross terms a_lo b_hi + a_hi b_lo accumulate in their OWN tensor-memory columns [TM_C, TM_C + 64) and meet the
-// a_hi b_hi sum only in the epilogue: the tensor core's accumulator add drops the low bits of a small addend, and the
-// cross terms are 2^-11 of the main ones (tools/micro/umma_probe.cu accuracy study, K = 256: rms error vs fp64 1.7e-6 with
-// one accumulator, 5.7e-7 with the corrections apart; an fp32 FMA chain: 1.9e-7).  Same MMA count, one more tcgen05.ld.
-constexpr int TM_C = 256;
-constexpr int TM_G = 160;                                        // reduced gradient tile (data-parallel runs)
+// The two cross terms a_lo b_hi + a_hi b_lo accumulate in their OWN registers and meet the a_hi b_hi sum only in the
+// epilogue: the cross terms are 2^-11 of the main ones, and a tensor-core accumulator add may drop low bits of a small
+// addend.  Same MMA count, 8 more accumulator registers per instruction column.
 // peer-mapped exchange buffer of one step parity (floats): one region per SOURCE rank [8] plus one for the W2 means
 // (written by the packets' owners), each holding per net 16 gradient tiles and the locally reduced small-parameter
 // slices of the 8 column blocks.  Ranks PUSH their pieces into
 // every peer's buffer as 16-byte packets {3 floats, tag}: the tag (launch sequence number | step) travels with the data,
 // so the receiver polls its own memory until every packet carries the tag -- one NVLink one-way latency per exchange,
-// no system-scope fence (measured: ~6 us each with posted peer writes outstanding), no flag round trip, no remote loads.
+// no system-scope fence (slow with posted peer writes outstanding), no flag round trip, no remote loads.
 // The tag word is XORed with a hash of the three payload words: a 16-byte vector store does NOT become visible atomically
-// to a concurrent 16-byte load on the receiving GPU (measured on 2 x B200: about one packet in 1e9 showed the new tag
-// next to a stale payload word, i.e. one diverging parameter update per ~10k optimiser steps; tools/dp_identity_check.py),
-// so the receiver accepts a packet only if tag AND payload agree and simply polls again otherwise.
+// to a concurrent 16-byte load on the receiving GPU (a torn packet would show the new tag next to a stale payload
+// word, i.e. one diverging parameter update; tools/dp_identity_check.py), so the receiver accepts a packet only if tag AND payload agree and simply polls again otherwise.
 constexpr int NSMAX = (MAXD + 1) * 32 + 32 + 32 * OUTP + 16;
 constexpr int TILE_PK = (64 * 64 / NEPI + 2) / 3;                // packets per thread of a 64 x 64 tile (16 floats -> 6)
 constexpr int TILE_FLOATS = TILE_PK * NEPI * 4;                  // [packet][thread][4]
@@ -117,7 +116,7 @@ struct AdamS { float w1, b2, w2, rbc2s, eps, neg_step; };
 // torch.optim.Adam's single-tensor update.  The moments are the exact fp32 expressions; the parameter step
 // p += step * m / (sqrt(v) / sqrt(bc2) + eps) uses the SFU reciprocal square root / reciprocal (about 2 ulp each,
 // i.e. ~1e-10 absolute on a step of <= lr) instead of IEEE sqrt and division, whose slow-path calls serialise the
-// 32 elements a lane owns (measured: 19k cycles per step for the 64 x 64 tile with IEEE arithmetic).
+// 32 elements a lane owns.
 __device__ __forceinline__ float adam_one(float p, float g, float& m, float& v, const AdamS& a) {
     m = m + a.w1 * (g - m);                 // exp_avg.lerp_(grad, 1 - beta1)
     v = v * a.b2 + (a.w2 * g) * g;          // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
@@ -151,7 +150,7 @@ __device__ __forceinline__ float4 ld_packet(const float* p) {
 
 // Wait for the packets of all ranks but `me` at src + r * stride (local memory, pushed by the peers) and add them to the
 // own piece (ox, oy, oz) in rank order.  Deliberately not inlined: the exchange code runs once per step and the kernel's
-// instruction footprint matters (measured: the step slows down by ~10 % when the exchange is unrolled into the epilogue).
+// instruction footprint matters (unrolled into the epilogue, the exchange slows the whole step down).
 __device__ __noinline__ float3 dp_gather(const float* src, long long stride, int me, int world, uint32_t tag,
                                         float ox, float oy, float oz, int* err, int code) {
     const long long t0w = clock64();
@@ -230,93 +229,85 @@ __device__ __forceinline__ bool elect_one() {
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, %0;" ::"n"(NEPI) : "memory"); }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-        "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-          "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-          "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-          "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])),
-          "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-          "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-          "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])),
-          "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-        : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-          "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-          "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-          "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-        : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// Staged accumulator tile accs[64][ACC_LD] in shared memory: the epilogue layout keeps row `row` of the tile in
+// lanes l and l + 16 of a warp, NC consecutive columns from `col` (lane l < 16: the low columns, l + 16: the high ones).
+template <int NC>
+__device__ __forceinline__ void acc_ld(const float* accs, int row, int col, float (&v)[NC]) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-// two loads in flight, one wait (NC = 8 / 16): the accumulator columns and their correction columns
-template <int NC> __device__ __forceinline__ void tmem_ld_pair(uint32_t ta, uint32_t tb, float (&x)[NC], float (&y)[NC]) {
-    static_assert(NC == 8 || NC == 16, "pair loads in use");
-    uint32_t r[NC], q[NC];
-    if constexpr (NC == 8) {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(ta));
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]), "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7]) : "r"(tb));
-    } else {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                       "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]) : "r"(ta));
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                     : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]), "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7]), "=r"(q[8]),
-                       "=r"(q[9]), "=r"(q[10]), "=r"(q[11]), "=r"(q[12]), "=r"(q[13]), "=r"(q[14]), "=r"(q[15]) : "r"(tb));
+    for (int q = 0; q < NC / 4; ++q) {
+        const float4 x = *reinterpret_cast<const float4*>(accs + row * ACC_LD + col + 4 * q);
+        v[4 * q] = x.x; v[4 * q + 1] = x.y; v[4 * q + 2] = x.z; v[4 * q + 3] = x.w;
     }
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+}
+template <int NC>
+__device__ __forceinline__ void acc_st(float* accs, int row, int col, const float (&v)[NC]) {
 #pragma unroll
-    for (int i = 0; i < NC; ++i) { x[i] = __uint_as_float(r[i]); y[i] = __uint_as_float(q[i]); }
-}
-// NC = 8 / 16 / 32 consecutive columns of this thread's tensor-memory lane
-template <int NC> __device__ __forceinline__ void tmem_ldn(uint32_t taddr, float (&v)[NC]) {
-    if constexpr (NC == 8) tmem_ld8(taddr, v);
-    else if constexpr (NC == 16) tmem_ld16(taddr, v);
-    else tmem_ld32(taddr, v);
-}
-template <int NC> __device__ __forceinline__ void tmem_stn(uint32_t taddr, const float (&v)[NC]) {
-    static_assert(NC == 16 || NC == 32, "tensor-memory store widths in use");
-    if constexpr (NC == 16) tmem_st16(taddr, v);
-    else tmem_st32(taddr, v);
+    for (int q = 0; q < NC / 4; ++q)
+        *reinterpret_cast<float4*>(accs + row * ACC_LD + col + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
 }
 
-// The M = 64 accumulators occupy the lower 16 lanes of every tensor-memory subpartition (one MMA per k-step keeps the
-// shared-memory operand traffic down -- the A tile is re-read by every instruction).  All 32 lanes of the WQ warps that
-// share a subpartition split the columns: lane l < 16 of warp-in-subpartition wq keeps columns [col_lo, col_lo + NC), lane
-// l + 16 receives columns [col_hi, col_hi + NC) of lane l.
-template <int NC>
-__device__ __forceinline__ void acc_ld_split(uint32_t taddr, int lane, int col_lo, int col_hi, float (&v)[NC]) {
-    float w[NC];
-    {
-        float c[NC];
-        tmem_ld_pair<NC>(taddr + col_hi, taddr + TM_C + col_hi, w, c);
+// One GEMM of the step, issued by both epilogue warpgroups straight from the operand ring: NCH chunks of KC k, A = 64
+// rows, B = b_rows rows.  Instruction h of a warpgroup covers the 8-column groups bgrp[h] and bgrp[h] + gstep (B core
+// matrices at SBO = 128 gstep bytes), i.e. exactly the columns its threads own in the epilogue.  Each warp releases a
+// slot once its MMAs have read it (bar_empty counts the NEPI / 32 warps); one group stays in flight.
+template <int NI>
+__device__ __forceinline__ void gemm_phase(const unsigned char* ring, unsigned& qq, uint64_t* bar_full, uint64_t* bar_empty,
+                                           uint32_t b_rows, const int (&bgrp)[NI], int gstep,
+                                           float (&dm)[NI][8], float (&dc)[NI][8], int* err, int code, int lane) {
 #pragma unroll
-        for (int j = 0; j < NC; ++j) w[j] += c[j];
-        tmem_ld_pair<NC>(taddr + col_lo, taddr + TM_C + col_lo, v, c);
+    for (int h = 0; h < NI; ++h)
 #pragma unroll
-        for (int j = 0; j < NC; ++j) v[j] += c[j];
+        for (int e = 0; e < 8; ++e) dm[h][e] = dc[h][e] = 0.f;
+    const uint32_t ring_a = smem_u32(ring);
+    const uint32_t b_lbo = 16 * b_rows, b_chunk = b_rows * KC * 4, b_sbo = 128 * gstep;
+    for (int j = 0; j < NCH; ++j, ++qq) {
+        const int s = qq % NSLOT;
+        if (!mbar_wait(&bar_full[s], (qq / NSLOT) & 1, WAIT_CYCLES)) fail(err, code);
+        __syncwarp();
+        wgmma_fence();
+        const uint32_t base = ring_a + (uint32_t)s * SLOT_BYTES;
+#pragma unroll
+        for (int ks = 0; ks < KC / 8; ++ks) {
+            const uint64_t ah = smem_desc(base + ks * 2048, 1024, 128);
+            const uint64_t al = smem_desc(base + A_CHUNK + ks * 2048, 1024, 128);
+#pragma unroll
+            for (int h = 0; h < NI; ++h) {
+                const uint32_t bo = 2 * A_CHUNK + ks * 2 * b_lbo + 128 * bgrp[h];
+                const uint64_t bh = smem_desc(base + bo, b_lbo, b_sbo);
+                const uint64_t bl = smem_desc(base + bo + b_chunk, b_lbo, b_sbo);
+                mma_m64n16k8_tf32(dc[h], al, bh);
+                mma_m64n16k8_tf32(dc[h], ah, bl);
+                mma_m64n16k8_tf32(dm[h], ah, bh);
+            }
+        }
+        wgmma_commit();
+        if (j > 0) {
+            wgmma_wait<1>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&bar_empty[(qq - 1) % NSLOT]);
+        }
     }
+    wgmma_wait<0>();
 #pragma unroll
-    for (int j = 0; j < NC; ++j) {
-        const float x = __shfl_sync(0xffffffffu, w[j], lane & 15);
-        v[j] = (lane & 16) ? x : v[j];
-    }
+    for (int h = 0; h < NI; ++h) { reg_fence(dm[h]); reg_fence(dc[h]); }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bar_empty[(qq - 1) % NSLOT]);
+}
+// fragment (wgmma.cuh) -> accs, main + cross terms; warp w % 4 writes rows 16 (w % 4) .. + 15 of its column groups
+template <int NI>
+__device__ __forceinline__ void stage_acc(float* accs, const float (&dm)[NI][8], const float (&dc)[NI][8], const int (&bgrp)[NI],
+                                          int gstep, int sp, int lane) {
+    const int r = 16 * sp + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < NI; ++h)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int col = 8 * (bgrp[h] + gstep * i) + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(accs + r * ACC_LD + col) = make_float2(dm[h][4 * i] + dc[h][4 * i], dm[h][4 * i + 1] + dc[h][4 * i + 1]);
+            *reinterpret_cast<float2*>(accs + (r + 8) * ACC_LD + col) =
+                make_float2(dm[h][4 * i + 2] + dc[h][4 * i + 2], dm[h][4 * i + 3] + dc[h][4 * i + 3]);
+        }
+    __syncwarp();
 }
 
 // Transposed K-major image of a 64-row tile through shared memory.  Every epilogue thread holds NC consecutive
@@ -373,9 +364,9 @@ struct SliceMap {
 };
 
 // ---- data-parallel exchange, out of line ---------------------------------------------------------------------------------
-// All of it lives in functions the kernel CALLS: inlined into the epilogue, the mere presence of this code slowed every
-// phase of the step down by ~9 % (measured with the exchange compiled in but world = 1) -- register allocation and the
-// instruction footprint of the ~7k-instruction epilogue are that tight.
+// All of it lives in functions the kernel CALLS: inlined into the epilogue, the mere presence of this code slows every
+// phase of the step down even with world = 1 -- register allocation and the instruction footprint of the long epilogue
+// are that tight.
 struct DpCtx {
     const float* const* xg;   // [rank] exchange buffers of this step's parity (shared-memory table)
     long long region;         // floats per source-rank region
@@ -387,10 +378,10 @@ struct DpCtx {
 };
 __device__ __forceinline__ int dp_owner(int et, int q, int world) { return (int)((unsigned)((et >> 5) * TILE_PK + q) % (unsigned)world); }
 
-// hop 1 of a W2 gradient tile: every packet of the local tile (tensor-memory accumulators) to its owner
-__device__ __noinline__ void dp_tile_send(DpCtx d, size_t off, uint32_t tm_lane, int lane, int wq, int et) {
+// hop 1 of a W2 gradient tile: every packet of the local tile (staged accumulators) to its owner
+__device__ __noinline__ void dp_tile_send(DpCtx d, size_t off, const float* accs, int trow, int cb2, int et) {
     float g[C2];
-    acc_ld_split<C2>(tm_lane, lane, C2 * wq, 32 + C2 * wq, g);
+    acc_ld<C2>(accs, trow, cb2, g);
 #pragma unroll
     for (int q = 0; q < TILE_PK; ++q) {
         const size_t o_q = (size_t)d.me * d.region + off + (size_t)q * NEPI * 4;
@@ -404,10 +395,10 @@ __device__ __noinline__ void dp_tile_send(DpCtx d, size_t off, uint32_t tm_lane,
     }
 }
 // hop 2: owned packets -- rank-ordered mean of the ranks' contributions, pushed into everybody's result region; the tile
-// (owned entries final, the others still local) goes to tensor-memory columns TM_G
-__device__ __noinline__ void dp_tile_reduce(DpCtx d, size_t off, uint32_t tm_lane, int lane, int wq, int et) {
+// (owned entries final, the others still local) replaces the staged accumulators
+__device__ __noinline__ void dp_tile_reduce(DpCtx d, size_t off, float* accs, int trow, int cb2, int et) {
     float g[C2];
-    acc_ld_split<C2>(tm_lane, lane, C2 * wq, 32 + C2 * wq, g);
+    acc_ld<C2>(accs, trow, cb2, g);
     const float inv_world = 1.0f / (float)d.world;
     const float* loc = d.xg[d.me];
 #pragma unroll
@@ -421,17 +412,16 @@ __device__ __noinline__ void dp_tile_reduce(DpCtx d, size_t off, uint32_t tm_lan
         if (3 * q + 1 < C2) g[3 * q + 1] = ay;
         if (3 * q + 2 < C2) g[3 * q + 2] = az;
     }
-    __syncwarp();      // the lanes left their poll loops at different times: tcgen05.st is .sync.aligned
-    tmem_stn<C2>(tm_lane + TM_G + C2 * wq, g);
+    acc_st<C2>(accs, trow, cb2, g);
 }
-// the other owners' means: wait for them in the local result region, complete the tile in TM_G, return its sum of squares
-__device__ __noinline__ float dp_tile_finish(DpCtx d, size_t off, uint32_t tm_lane, int lane, int wq, int et) {
+// the other owners' means: wait for them in the local result region, complete the staged tile, return its sum of squares
+__device__ __noinline__ float dp_tile_finish(DpCtx d, size_t off, float* accs, int trow, int cb2, int et) {
     float g[C2];
     const long long t0w = clock64();
     if (d.direct) {
         // one hop: all ranks' tiles are (or will be) in the local contribution regions -- rank-ordered mean, rank by rank
         float own[C2];
-        acc_ld_split<C2>(tm_lane, lane, C2 * wq, 32 + C2 * wq, own);
+        acc_ld<C2>(accs, trow, cb2, own);
 #pragma unroll
         for (int jq = 0; jq < C2; ++jq) g[jq] = 0.f;
         for (int r = 0; r < d.world; ++r) {
@@ -462,12 +452,11 @@ __device__ __noinline__ float dp_tile_finish(DpCtx d, size_t off, uint32_t tm_la
         float sq = 0.f;
 #pragma unroll
         for (int jq = 0; jq < C2; ++jq) { g[jq] *= inv_world; sq = fmaf(g[jq], g[jq], sq); }
-        __syncwarp();  // the lanes left their poll loops at different times: tcgen05.st is .sync.aligned
-        tmem_stn<C2>(tm_lane + TM_G + C2 * wq, g);
+        acc_st<C2>(accs, trow, cb2, g);
         return sq;
     }
     const float* res = d.xg[d.me] + (size_t)FSRL_P2P_MAX_RANKS * d.region + off;
-    tmem_ldn<C2>(tm_lane + TM_G + C2 * wq, g);
+    acc_ld<C2>(accs, trow, cb2, g);
     float4 v[TILE_PK];
     bool ok;
     do {
@@ -490,8 +479,7 @@ __device__ __noinline__ float dp_tile_finish(DpCtx d, size_t off, uint32_t tm_la
     }
 #pragma unroll
     for (int jq = 0; jq < C2; ++jq) sq = fmaf(g[jq], g[jq], sq);
-    __syncwarp();
-    tmem_stn<C2>(tm_lane + TM_G + C2 * wq, g);
+    acc_st<C2>(accs, trow, cb2, g);
     return sq;
 }
 // small-parameter slices of one column block (n floats in shared memory): row block 0 pushes them to every rank, every
@@ -517,8 +505,7 @@ __device__ __noinline__ void dp_slices(DpCtx d, size_t off_s, float* sp_g, int n
 template <bool DP>
 __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    __shared__ __align__(8) uint64_t bar_full[NSLOT], bar_empty[NSLOT], bar_acc, bar_b;
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t bar_full[NSLOT], bar_empty[NSLOT], bar_b;
     __shared__ float s_red[4][320];          // cross-subpartition partial sums
     __shared__ float s_misc[32];
     __shared__ AdamS s_adam;
@@ -536,7 +523,8 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     unsigned* fl_net = P.flags + (size_t)net * F_PER_NET * FLAG_LINE;
     unsigned* fl_d2 = P.flags + (size_t)u.n_nets * F_PER_NET * FLAG_LINE;
     unsigned char* ring = smem_raw;
-    float* small = reinterpret_cast<float*>(smem_raw + NSLOT * SLOT_BYTES);
+    float* accs = reinterpret_cast<float*>(smem_raw + NSLOT * SLOT_BYTES);     // staged accumulator tile [64][ACC_LD]
+    float* small = accs + 64 * ACC_LD;
     const SliceMap sm(D);
     float* sp_p = small;                 // parameters
     float* sp_m = small + sm.n;          // Adam first moment
@@ -545,16 +533,11 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     float* land = small + 4 * sm.n;      // cluster mode: head partials pushed by the 8 CTAs of this row block [b][64][OUTP]
 
     if (tid == 0) {
-        for (int i = 0; i < NSLOT; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 1); }
-        mbar_init(&bar_acc, 1);
+        for (int i = 0; i < NSLOT; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], NEPI / 32); }
         mbar_init(&bar_b, 1);                // per step: one local expect_tx arrival + 16 KB of remote st.async bytes
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc<TM_COLS>(&s_tmem);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = s_tmem;
     if (DP && threadIdx.x < 2 * FSRL_P2P_MAX_RANKS) s_xg[threadIdx.x / FSRL_P2P_MAX_RANKS][threadIdx.x % FSRL_P2P_MAX_RANKS] = P.u.p2p_xg[threadIdx.x / FSRL_P2P_MAX_RANKS][threadIdx.x % FSRL_P2P_MAX_RANKS];
     if (DP) __syncthreads();
     if (P.cluster) cluster_sync_all();       // every CTA's barriers exist before a peer may arrive on them
@@ -564,7 +547,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     const long long o_w1 = pbase, o_b1 = o_w1 + (long long)D * H, o_w2 = o_b1 + H, o_b2 = o_w2 + (long long)H * H,
                     o_w3 = o_b2 + H, o_b3 = o_w3 + (long long)H * out, o_ls = o_b3 + out;
 
-    if (warp == 0) {
+    if (warp == NEPI / 32) {
         // ============================ bulk-copy producer ==========================================
         if (elect_one()) {
             unsigned qq = 0;
@@ -572,16 +555,16 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 if (!flag_wait_ge<true>(fl_net + F_A * FLAG_LINE, 32u * (t + 1), WAIT_CYCLES)) fail(P.err, 10);
                 STAMP(12);
                 fence_proxy_async();
-                for (int j = 0; j < 4; ++j, ++qq) {               // G1: K = k in chunks of 64
+                for (int j = 0; j < NCH; ++j, ++qq) {             // G1: K = k in chunks of KC
                     const int s = qq % NSLOT;
                     if (!mbar_wait(&bar_empty[s], ((qq / NSLOT) & 1) ^ 1, WAIT_CYCLES)) fail(P.err, 11);
                     unsigned char* dst = ring + (size_t)s * SLOT_BYTES;
-                    mbar_expect_tx(&bar_full[s], 49152);
-                    const size_t ao = (size_t)a * 16384 + (size_t)j * 4096, bo = (size_t)b * 8192 + (size_t)j * 2048;
-                    bulk_g2s(dst, wsn + (size_t)I_H1A_HI * IMG + ao, 16384, &bar_full[s]);
-                    bulk_g2s(dst + 16384, wsn + (size_t)I_H1A_LO * IMG + ao, 16384, &bar_full[s]);
-                    bulk_g2s(dst + 32768, wsn + (size_t)I_W2A_HI * IMG + bo, 8192, &bar_full[s]);
-                    bulk_g2s(dst + 40960, wsn + (size_t)I_W2A_LO * IMG + bo, 8192, &bar_full[s]);
+                    mbar_expect_tx(&bar_full[s], 3 * A_CHUNK);
+                    const size_t ao = (size_t)a * 16384 + (size_t)j * 64 * KC, bo = (size_t)b * 8192 + (size_t)j * 32 * KC;
+                    bulk_g2s(dst, wsn + (size_t)I_H1A_HI * IMG + ao, A_CHUNK, &bar_full[s]);
+                    bulk_g2s(dst + A_CHUNK, wsn + (size_t)I_H1A_LO * IMG + ao, A_CHUNK, &bar_full[s]);
+                    bulk_g2s(dst + 2 * A_CHUNK, wsn + (size_t)I_W2A_HI * IMG + bo, A_CHUNK / 2, &bar_full[s]);
+                    bulk_g2s(dst + 2 * A_CHUNK + A_CHUNK / 2, wsn + (size_t)I_W2A_LO * IMG + bo, A_CHUNK / 2, &bar_full[s]);
                 }
                 STAMP(13);
                 if (!flag_wait_ge<true>(fl_net + F_C * FLAG_LINE, 32u * (t + 1), WAIT_CYCLES)) fail(P.err, 12);
@@ -589,80 +572,31 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 fence_proxy_async();
                 const int ia = is_g2 ? I_W2B_HI : I_DZT_HI, ib = is_g2 ? I_DZA_HI : I_H1T_HI;
                 const int blk_a = is_g2 ? ka : q4, blk_b = is_g2 ? q4 : ka;
-                for (int j = 0; j < 4; ++j, ++qq) {               // G2: K = o ; G3: K = r ; chunks of 64
+                for (int j = 0; j < NCH; ++j, ++qq) {             // G2: K = o ; G3: K = r ; chunks of KC
                     const int s = qq % NSLOT;
                     if (!mbar_wait(&bar_empty[s], ((qq / NSLOT) & 1) ^ 1, WAIT_CYCLES)) fail(P.err, 13);
                     unsigned char* dst = ring + (size_t)s * SLOT_BYTES;
-                    mbar_expect_tx(&bar_full[s], 65536);
-                    const size_t ao = (size_t)blk_a * 16384 + (size_t)j * 4096, bo = (size_t)blk_b * 16384 + (size_t)j * 4096;
-                    bulk_g2s(dst, wsn + (size_t)ia * IMG + ao, 16384, &bar_full[s]);
-                    bulk_g2s(dst + 16384, wsn + (size_t)(ia + 1) * IMG + ao, 16384, &bar_full[s]);
-                    bulk_g2s(dst + 32768, wsn + (size_t)ib * IMG + bo, 16384, &bar_full[s]);
-                    bulk_g2s(dst + 49152, wsn + (size_t)(ib + 1) * IMG + bo, 16384, &bar_full[s]);
+                    mbar_expect_tx(&bar_full[s], 4 * A_CHUNK);
+                    const size_t ao = (size_t)blk_a * 16384 + (size_t)j * 64 * KC, bo = (size_t)blk_b * 16384 + (size_t)j * 64 * KC;
+                    bulk_g2s(dst, wsn + (size_t)ia * IMG + ao, A_CHUNK, &bar_full[s]);
+                    bulk_g2s(dst + A_CHUNK, wsn + (size_t)(ia + 1) * IMG + ao, A_CHUNK, &bar_full[s]);
+                    bulk_g2s(dst + 2 * A_CHUNK, wsn + (size_t)ib * IMG + bo, A_CHUNK, &bar_full[s]);
+                    bulk_g2s(dst + 3 * A_CHUNK, wsn + (size_t)(ib + 1) * IMG + bo, A_CHUNK, &bar_full[s]);
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ============================ MMA issuer ==================================================
-        if (elect_one()) {
-            unsigned qq = 0;
-            const uint32_t ring_a = smem_u32(ring);
-            const uint32_t id32 = idesc_tf32(64, 32, false, false), id64 = idesc_tf32(64, 64, false, false);
-            for (int t = 0; t < P.n_mb; ++t) {
-                for (int j = 0; j < 4; ++j, ++qq) {               // ---- G1: D[64 r][32 o], two 16-column halves
-                    const int s = qq % NSLOT;
-                    if (!mbar_wait(&bar_full[s], (qq / NSLOT) & 1, WAIT_CYCLES)) fail(P.err, 20);
-                    tc_fence_after();
-                    if (j == 0) STAMP(16);
-                    if (j == 3) STAMP(17);
-                    const uint32_t base = ring_a + (uint32_t)s * SLOT_BYTES;
-#pragma unroll 4
-                    for (int ks = 0; ks < 8; ++ks) {
-                        const uint64_t ah = smem_desc(base + ks * 2048, 1024, 128);
-                        const uint64_t al = smem_desc(base + 16384 + ks * 2048, 1024, 128);
-                        const uint64_t bh = smem_desc(base + 32768 + ks * 1024, 512, 128);
-                        const uint64_t bl = smem_desc(base + 40960 + ks * 1024, 512, 128);
-                        mma_tf32_ss(tmem + TM_C, al, bh, id32, (j | ks) != 0);
-                        mma_tf32_ss(tmem + TM_C, ah, bl, id32, true);
-                        mma_tf32_ss(tmem, ah, bh, id32, (j | ks) != 0);
-                    }
-                    mma_commit(&bar_empty[s]);
-                }
-                mma_commit(&bar_acc);
-                STAMP(18);
-                for (int j = 0; j < 4; ++j, ++qq) {               // ---- G2 / G3: D[64][64], two 32-column halves
-                    const int s = qq % NSLOT;
-                    if (!mbar_wait(&bar_full[s], (qq / NSLOT) & 1, WAIT_CYCLES)) fail(P.err, 21);
-                    tc_fence_after();
-                    if (j == 0) STAMP(19);
-                    if (j == 3) STAMP(20);
-                    const uint32_t base = ring_a + (uint32_t)s * SLOT_BYTES;
-#pragma unroll 4
-                    for (int ks = 0; ks < 8; ++ks) {
-                        const uint64_t ah = smem_desc(base + ks * 2048, 1024, 128);
-                        const uint64_t al = smem_desc(base + 16384 + ks * 2048, 1024, 128);
-                        const uint64_t bh = smem_desc(base + 32768 + ks * 2048, 1024, 128);
-                        const uint64_t bl = smem_desc(base + 49152 + ks * 2048, 1024, 128);
-                        mma_tf32_ss(tmem + TM_C, al, bh, id64, (j | ks) != 0);
-                        mma_tf32_ss(tmem + TM_C, ah, bl, id64, true);
-                        mma_tf32_ss(tmem, ah, bh, id64, (j | ks) != 0);
-                    }
-                    mma_commit(&bar_empty[s]);
-                }
-                mma_commit(&bar_acc);
-                STAMP(21);
             }
         }
     } else {
-        // ============================ epilogue warps ===============================================
-        const int et = tid - 64;                    // 0 .. NEPI - 1
-        const int sp = warp & 3;                    // tensor-memory subpartition of this warp
-        const int wq = (warp - 2) >> 2;             // which of the WQ warps of that subpartition
+        // ============================ MMA + epilogue warps ========================================
+        const int et = tid;                         // 0 .. NEPI - 1
+        const int sp = warp & 3;                    // 16-row slab of this warp (its rank in the warpgroup)
+        const int wq = warp >> 2;                   // warpgroup: which of the WQ warps of that slab
         const int r16 = lane & 15, half = lane >> 4;
         const int trow = 16 * sp + r16;             // row of the 64-row tile held by this lane
         const int cb1 = 16 * half + C1 * wq;        // first of this thread's C1 columns of a 32-column tile
         const int cb2 = 32 * half + C2 * wq;        // first of this thread's C2 columns of a 64-column tile
-        const uint32_t tm_lane = tmem + ((uint32_t)(32 * sp) << 16);
+        const int bg1[1] = {wq}, bg2[2] = {2 * wq, 2 * wq + 4};   // column groups of the warpgroup's MMAs: G1, G2 / G3
+        unsigned qq = 0;                            // operand ring position
+        float w2p[C2], w2m[C2], w2v[C2];            // owned W2 tile (G3 CTAs): parameters and Adam moments
         float* stat_base = u.stats;
         // ---- data-parallel exchange over peer memory (NVLink): every CTA pushes its local gradient piece into its
         // rank's region of EVERY rank's exchange buffer, one thread fences and release-stores the step id into the same
@@ -670,7 +604,6 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
         // memory in rank order -- point-to-point between equal CTAs, one NVLink one-way latency, no remote loads,
         // bit-identical sums on every rank.
         const int world = (DP && u.world > 1) ? u.world : 1;
-        const float inv_world = 1.0f / (float)world;
         // W2 tiles travel in two hops (reduce-scatter + all-gather, 2 (W - 1) / W tile volumes per rank instead of W - 1):
         // packet q of epilogue warp w is OWNED by rank (6 w + q) mod W -- every rank sends it there, the owner sums the
         // ranks' packets in rank order and pushes the mean into everybody's result region (region 8).  Both hops are
@@ -687,7 +620,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             return d;
         };
 
-        // ---- initial state: small slices from the arena, the W2 tile (p, m, v) into tensor memory ----
+        // ---- initial state: small slices from the arena, the W2 tile (p, m, v) into registers ----
         for (int i = et; i < sm.n; i += NEPI) {
             long long src = -1;
             if (i < sm.b2) { const int d = i / 32, kk = i % 32; src = (d < D) ? o_w1 + (long long)d * H + 32 * b + kk : o_b1 + 32 * b + kk; }
@@ -701,17 +634,17 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
         }
         if (!is_g2) {
             const int o = 64 * q4 + trow;
-            float pv[C2], mv[C2], vv[C2];
 #pragma unroll
             for (int j = 0; j < C2; ++j) {
                 const long long idx = o_w2 + (long long)(64 * ka + cb2 + j) * H + o;
-                pv[j] = u.theta[idx]; mv[j] = u.adam_m[idx]; vv[j] = u.adam_v[idx];
+                w2p[j] = u.theta[idx]; w2m[j] = u.adam_m[idx]; w2v[j] = u.adam_v[idx];
             }
-            tmem_stn<C2>(tm_lane + TM_P + C2 * wq, pv); tmem_stn<C2>(tm_lane + TM_M + C2 * wq, mv); tmem_stn<C2>(tm_lane + TM_V + C2 * wq, vv);
+        } else {
+#pragma unroll
+            for (int j = 0; j < C2; ++j) w2p[j] = w2m[j] = w2v[j] = 0.f;
         }
         epi_bar();
 
-        unsigned acc_phase = 0;
         for (int t = 0; t < P.n_mb; ++t) {
             const long long row0 = (long long)t * MB;                 // first row of the minibatch in the gathered arrays
             const int slot = P.slot0 + t;
@@ -735,11 +668,11 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 if (net == 0) { prefetch_l2(u.act + r * A); prefetch_l2(u.logp_old + r); prefetch_l2(u.adv + r); if (C > 1) prefetch_l2(u.adv + u.ld + r); }
                 else { prefetch_l2(u.ret + (long long)(net - 1) * u.ld + r); if (u.value_clip) prefetch_l2(u.values + (long long)(net - 1) * u.ld + r); }
             }
-            // ---- S(a): publish the images of the owned W2 tile (from tensor memory) ------------------
+            // ---- S(a): publish the images of the owned W2 tile (from registers) ------------------------
             float* scratch = reinterpret_cast<float*>(ring);       // the operand ring is idle outside the GEMM phases
             if (!is_g2) {
-                float pv[C2], phi[C2], plo[C2];
-                tmem_ldn<C2>(tm_lane + TM_P + C2 * wq, pv);
+                const float (&pv)[C2] = w2p;
+                float phi[C2], plo[C2];
                 const int o = 64 * q4 + trow;                   // output unit of this lane
                 float* w2a_hi = wsn + (size_t)I_W2A_HI * IMG + (size_t)(o >> 5) * 8192 + (size_t)(o & 31) * 4;
                 float* w2a_lo = w2a_hi + IMG;
@@ -796,6 +729,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 for (int rep = 0; rep < 2; ++rep)
                     transposed_flush<32>(scratch + rep * TSCR, et, wsn + (size_t)I_H1T_HI * IMG + (size_t)(b >> 1) * 16384, 64 * (a + 2 * rep), 32 * (b & 1));
             }
+            fence_proxy_async_smem();                                // scratch stores before the next bulk copies into the ring
             epi_bar();
             if (et == 0) { STAMP(1); flag_add_release(fl_net + F_A * FLAG_LINE); }
 
@@ -825,14 +759,15 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 p_rsg[j] = 1.0f / expf(p_ls[j]);
             }
 
-            // ---- G1 epilogue: h2 = relu(acc + b2), head partial over this tile's 32 columns -------------
-            if (!mbar_wait(&bar_acc, acc_phase & 1, WAIT_CYCLES)) fail(P.err, 30);
-            __syncwarp();      // every thread polled on its own: reconverge before the .sync.aligned tensor-memory loads
-            ++acc_phase;
-            tc_fence_after();
+            // ---- G1 (wgmma), then its epilogue: h2 = relu(acc + b2), head partial over this tile's 32 columns ----
+            {
+                float dm[1][8], dc[1][8];
+                gemm_phase<1>(ring, qq, bar_full, bar_empty, 32, bg1, 2, dm, dc, P.err, 30, lane);
+                stage_acc<1>(accs, dm, dc, bg1, 2, sp, lane);
+            }
             if (et == 0) STAMP(2);
             float h2[C1];
-            acc_ld_split<C1>(tm_lane, lane, C1 * wq, 16 + C1 * wq, h2);
+            acc_ld<C1>(accs, trow, cb1, h2);
             float hp[OUTP];
 #pragma unroll
             for (int j = 0; j < OUTP; ++j) hp[j] = 0.f;
@@ -896,7 +831,6 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                     *reinterpret_cast<float4*>(dst) = make_float4(hp[0], hp[1], hp[2], hp[3]);
                     *reinterpret_cast<float4*>(dst + 4) = make_float4(hp[4], hp[5], hp[6], hp[7]);
                 }
-                tc_fence_before();
                 epi_bar();
                 if (et == 0) {
                     STAMP(3);
@@ -1064,6 +998,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                     stat_base[(size_t)slot * FSRL_PPO_STATS + ST_ENTROPY] = ent;
                 }
             }
+            fence_proxy_async_smem();                                // scratch stores before the next bulk copies into the ring
             epi_bar();
             if (et == 0) { STAMP(5); flag_add_release(fl_net + F_C * FLAG_LINE); }
 
@@ -1093,17 +1028,20 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                     }
                 }
             }
-            if (!mbar_wait(&bar_acc, acc_phase & 1, WAIT_CYCLES)) fail(P.err, 32);
-            __syncwarp();      // every thread polled on its own: reconverge before the .sync.aligned tensor-memory loads
-            ++acc_phase;
-            tc_fence_after();
+            {
+                float dm[2][8], dc[2][8];
+                gemm_phase<2>(ring, qq, bar_full, bar_empty, 64, bg2, 1, dm, dc, P.err, 32, lane);
+                stage_acc<2>(accs, dm, dc, bg2, 1, sp, lane);
+            }
             if (et == 0) STAMP(6);
             float sq = 0.f;
             if (is_g2) {
                 // without clusters the observation block goes to slot 0 of the operand ring, idle from here until the
-                // next step's flag A
+                // next step's flag A -- once BOTH warpgroups are past gemm_phase: each warp has only waited for its own
+                // MMAs, and the other warpgroup's may still be reading the last chunks of the ring
                 float* xs = P.cluster ? land : reinterpret_cast<float*>(ring);
                 if (!P.cluster) {
+                    epi_bar();
 #pragma unroll
                     for (int q = 0; q < (64 * MAXD + NEPI - 1) / NEPI; ++q) {
                         const int e = et + q * NEPI;
@@ -1112,7 +1050,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 }
                 // lane: k = 64 ka + trow ; rows cb2 + j of row block q4; partial set 2 q4 + wq (WQ sets per row block)
                 float v[C2];
-                acc_ld_split<C2>(tm_lane, lane, C2 * wq, 32 + C2 * wq, v);
+                acc_ld<C2>(accs, trow, cb2, v);
                 const int k = 64 * ka + trow;
 #pragma unroll
                 for (int jq = 0; jq < C2; ++jq) v[jq] = (mreg[jq] > 0.f) ? v[jq] : 0.f;
@@ -1133,14 +1071,13 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 sb1 += __shfl_xor_sync(0xffffffffu, sb1, 16);
                 if (half == 0) dst[(size_t)D * H] = sb1;          // db1
                 if (et == 0) STAMP(23);
-                tc_fence_before();
                 epi_bar();
                 if (et == 0) flag_add_release(fl_net + F_D1 * FLAG_LINE);
             } else {
                 float g[C2];
-                acc_ld_split<C2>(tm_lane, lane, C2 * wq, 32 + C2 * wq, g);
+                acc_ld<C2>(accs, trow, cb2, g);
                 if (DP && world > 1) {
-                    dp_tile_send(dp_ctx(t), (size_t)(net * 16 + (c - 16)) * TILE_FLOATS + (size_t)et * 4, tm_lane, lane, wq, et);
+                    dp_tile_send(dp_ctx(t), (size_t)(net * 16 + (c - 16)) * TILE_FLOATS + (size_t)et * 4, accs, trow, cb2, et);
                     if (et == 0) STAMP(32);
                 } else {
 #pragma unroll
@@ -1197,11 +1134,11 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 const DpCtx d = dp_ctx(t);
                 const size_t off_t = (size_t)(net * 16 + (c - 16)) * TILE_FLOATS + (size_t)et * 4;
                 epi_bar();                                    // sp_g complete
-                if (!is_g2 && !d.direct) { dp_tile_reduce(d, off_t, tm_lane, lane, wq, et); if (et == 0) STAMP(33); }
+                if (!is_g2 && !d.direct) { dp_tile_reduce(d, off_t, accs, trow, cb2, et); if (et == 0) STAMP(33); }
                 dp_slices(d, (size_t)u.n_nets * 16 * TILE_FLOATS + (size_t)(net * 8 + b) * SLICE_PK * 4, sp_g, sm.n, et, a == 0);
                 __syncwarp();
                 if (et == 0) STAMP(38);
-                if (!is_g2) { sq += dp_tile_finish(d, off_t, tm_lane, lane, wq, et); if (et == 0) STAMP(41); }
+                if (!is_g2) { sq += dp_tile_finish(d, off_t, accs, trow, cb2, et); if (et == 0) STAMP(41); }
                 epi_bar();                                    // sp_g holds the global mean before the norm / Adam read it
             }
             // every small parameter is counted once in the norm: W1/b1/b2/W3 slices by row block 0, b3 / log sigma by CTA 0.
@@ -1216,7 +1153,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             }
             // ---- global gradient norm: per-CTA partial -> device-wide hop -> same summation order everywhere --
             sq = warp_sum(sq);
-            if (lane == 0) s_misc[warp - 2] = sq;
+            if (lane == 0) s_misc[warp] = sq;
             epi_bar();
             if (et == 0) {
                 float tot = 0.f;
@@ -1239,7 +1176,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             if (blockIdx.x == 0 && et == 0 && stat_base) stat_base[(size_t)slot * FSRL_PPO_STATS + ST_GRADNORM] = sqrtf(nsq);
             const AdamS ad = s_adam;
             if (et == 0) STAMP(24);
-            // ---- clip + Adam: replicated small slices, then the owned W2 tile (tensor memory) --------------------
+            // ---- clip + Adam: replicated small slices, then the owned W2 tile (registers) ------------------------
             for (int i = et; i < sm.n; i += NEPI) {
                 float m = sp_m[i], v = sp_v[i];
                 sp_p[i] = adam_one(sp_p[i], sp_g[i] * gscale, m, v, ad);
@@ -1247,15 +1184,11 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             }
             if (et == 0) STAMP(25);
             if (!is_g2) {
-                float g[C2], pv[C2], mv[C2], vv[C2];
-                if (DP && world > 1) tmem_ldn<C2>(tm_lane + TM_G + C2 * wq, g);
-                else acc_ld_split<C2>(tm_lane, lane, C2 * wq, 32 + C2 * wq, g);
-                tmem_ldn<C2>(tm_lane + TM_P + C2 * wq, pv); tmem_ldn<C2>(tm_lane + TM_M + C2 * wq, mv); tmem_ldn<C2>(tm_lane + TM_V + C2 * wq, vv);
+                float g[C2];
+                acc_ld<C2>(accs, trow, cb2, g);            // data-parallel runs: the ranks' mean (dp_tile_*)
 #pragma unroll
-                for (int j = 0; j < C2; ++j) pv[j] = adam_one(pv[j], g[j] * gscale, mv[j], vv[j], ad);
-                tmem_stn<C2>(tm_lane + TM_P + C2 * wq, pv); tmem_stn<C2>(tm_lane + TM_M + C2 * wq, mv); tmem_stn<C2>(tm_lane + TM_V + C2 * wq, vv);
+                for (int j = 0; j < C2; ++j) w2p[j] = adam_one(w2p[j], g[j] * gscale, w2m[j], w2v[j], ad);
             }
-            tc_fence_before();
             epi_bar();     // slices final before the next h1 tile / head reads them; s_adam may be rewritten
             if (et == 0) STAMP(11);
         }
@@ -1272,24 +1205,21 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             }
         }
         if (!is_g2) {
-            float pv[C2], mv[C2], vv[C2];
-            tmem_ldn<C2>(tm_lane + TM_P + C2 * wq, pv); tmem_ldn<C2>(tm_lane + TM_M + C2 * wq, mv); tmem_ldn<C2>(tm_lane + TM_V + C2 * wq, vv);
             const int o = 64 * q4 + trow;
 #pragma unroll
             for (int j = 0; j < C2; ++j) {
                 const long long idx = o_w2 + (long long)(64 * ka + cb2 + j) * H + o;
-                u.theta[idx] = pv[j]; u.adam_m[idx] = mv[j]; u.adam_v[idx] = vv[j];
+                u.theta[idx] = w2p[j]; u.adam_m[idx] = w2m[j]; u.adam_v[idx] = w2v[j];
             }
         }
-        tc_fence_before();
     }
     __syncthreads();
     if (P.cluster) cluster_sync_all();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc<TM_COLS>(tmem); }
 }
 
 static size_t smem_bytes(int D, bool cluster = false) {
-    return (size_t)NSLOT * SLOT_BYTES + 4 * sizeof(float) * SliceMap(D).n + (cluster ? sizeof(float) * 8 * 64 * OUTP : 0);
+    return (size_t)NSLOT * SLOT_BYTES + sizeof(float) * 64 * ACC_LD + 4 * sizeof(float) * SliceMap(D).n +
+           (cluster ? sizeof(float) * 8 * 64 * OUTP : 0);
 }
 
 }  // namespace pp

@@ -1,4 +1,4 @@
-// Persistent tcgen05 PPO-Lagrangian update (csrc/ppo_persist.cu): one launch per repeat.
+// Persistent wgmma PPO-Lagrangian update (csrc/ppo_persist.cu): one launch per repeat.
 #pragma once
 #include "common.cuh"
 #include "fsrl_b200.h"

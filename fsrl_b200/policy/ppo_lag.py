@@ -132,7 +132,7 @@ class PPOLagrangian(LagrangianPolicy):
         u.mb_stats = self._mb_stats.data_ptr()
         u.batch_size = int(getattr(self, '_dp_batch', 0))
         u.barrier = self._norm_sq.data_ptr() + 8
-        # persistent tcgen05 path (csrc/ppo_persist.cu): operand images, partial buffers and flags
+        # persistent wgmma path (csrc/ppo_persist.cu): operand images, partial buffers and flags
         nws = int(_lib.lib.fsrl_ppo_persist_ws_floats(len(ar.slots), s0.D, s0.H))
         if getattr(self, "_persist_ws", None) is None or self._persist_ws.numel() < nws:
             self._persist_ws = torch.zeros(nws, dtype=torch.float32, device=ar.device)

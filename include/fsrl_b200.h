@@ -1,4 +1,4 @@
-/* fsrl_b200 -- C-ABI of the B200-native FSRL hot path.
+/* fsrl_b200 -- C-ABI of the H100-native (sm_90a) FSRL hot path.
  *
  * The reference (liuzuxin/FSRL) is pure Python and has NO FFI layer of its own
  * (SURVEY.md F1, 8b): its boundary is the Python class API (fsrl.policy / fsrl.data).  This
@@ -189,7 +189,7 @@ typedef struct fsrl_ppo_update {
     float* p2p_part;               /* local [FSRL_P2P_PARTIALS]: per-CTA sums of g^2 (summed in a fixed
                                     * order by the Adam kernel: atomics would break rank lock-step) */
     int p2p_rank, p2p_on;
-    /* persistent tcgen05 path (csrc/ppo_persist.cu; H = 256, batch 256): workspace of
+    /* persistent wgmma path (csrc/ppo_persist.cu; H = 256, batch 256): workspace of
      * fsrl_ppo_persist_ws_floats() floats for the operand images / partials / flags; NULL or
      * persist_off != 0 selects the three-launch chain.  With world > 1 the launch exchanges gradients
      * itself: it treats every p2p_xg[b][r] as fsrl_ppo_persist_p2p_floats() floats of packet regions

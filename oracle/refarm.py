@@ -1,4 +1,4 @@
-"""The CPU arm of bench.py (test / baseline infrastructure): the UNMODIFIED reference classes from ``baseline/_ref``
+"""The CPU arm of bench.py (test / baseline infrastructure): the UNMODIFIED reference classes from ``oracle/_ref``
 (``pip install --no-deps --target``; ``/root/reference`` in the build container) run the whole collect + update
 cycle on the host cores --
 

@@ -7,8 +7,8 @@ code is involved), puts ``ref_dir`` first on ``sys.path`` so that ``import fsrl`
 and adds the one missing tianshou method the learners call, ``Batch.split`` (restated in
 oracle/ppo.py::split_indices, SURVEY.md 2.3 [UNVERIFIED]).
 
-ref_dir is ``/root/reference`` in the build container (golden-vector generation) or
-``baseline/_ref`` (``pip install --no-deps --target``, travels to the GPU box) for
+ref_dir is the reference source tree (golden-vector generation) or ``oracle/_ref``
+(``pip install --no-deps --target``, made by ``__graft_entry__.build()``) for
 ``bench.py --impl reference`` / ``cpu_baseline``.
 """
 from __future__ import annotations

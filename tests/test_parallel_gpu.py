@@ -70,7 +70,7 @@ def test_two_rank_update_keeps_parameters_identical():
 
 
 def _persistent_update(rank, dist):
-    """c2-shaped networks (2x256, batch 256) so that the persistent tcgen05 launch runs the update: its in-kernel
+    """c2-shaped networks (2x256, batch 256) so that the persistent wgmma launch runs the update: its in-kernel
     peer-memory exchange (csrc/ppo_persist.cu) against the three-launch chain's exchange kernel on the same data."""
     import ctypes
     from helpers import build_ppo

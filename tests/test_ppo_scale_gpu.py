@@ -133,7 +133,7 @@ def test_c2_shape_first_steps_and_epoch_parameters():
 
 
 def test_persistent_path_small_epoch_matches_oracle():
-    """64 envs x 300 steps = 75 minibatches of 256 rows through the persistent tcgen05 launch
+    """64 envs x 300 steps = 75 minibatches of 256 rows through the persistent wgmma launch
     (csrc/ppo_persist.cu): the gate must select it, and the first 8 steps / the parameters after a complete
     8-step epoch must match the fp32 oracle like the three-launch chain does."""
     import ctypes
@@ -167,6 +167,14 @@ def test_persistent_path_small_epoch_matches_oracle():
     np.random.seed(32)
     policy.learn(sub, batch_size=256, repeat=1)
     _assert_params_within_fp32_noise(policy, [a2] + c2, actor, critics, osub, lag, 32)
+
+
+def test_persistent_path_without_clusters_matches_oracle(monkeypatch):
+    """The same epochs with hop B through global memory instead of a thread-block cluster (FSRL_PPO_NO_CLUSTER=1; also
+    the launch used when 12 clusters of 8 cannot be co-resident): the G2 epilogue then stages its observation block in
+    the operand ring the GEMM has just read."""
+    monkeypatch.setenv("FSRL_PPO_NO_CLUSTER", "1")
+    test_persistent_path_small_epoch_matches_oracle()
 
 
 def _group_names(policy):
@@ -245,11 +253,11 @@ def test_gradients_against_fp64_autograd(hidden, task, lag):
     for r in rows:
         print("%-18s %12.3e %12.3e" % r)
     for name, e_dev, e_32 in rows:
-        # Measured (B200): the fp32 autograd reference sits 1e-7..6e-7 from fp64.  The persistent tcgen05 launch
-        # (H = 256 case; 3xTF32 with the cross terms in their own tensor-memory accumulator, DESIGN.md 3a) sits at
-        # 4e-7..1e-6; the three-launch chain (H = 512 cases, mma.sync 3xTF32, one accumulator) at 4e-7..4e-6 and up
-        # to 1e-5 where the value loss gradient 2 (v - ret) cancels (|v - ret| << |v| amplifies the forward error of
-        # v into every group of that critic alike).  A wrong term in a kernel shows up at 1e-2 and above.
+        # The fp32 autograd reference sits near 1e-7 from fp64 (printed above).  The persistent wgmma launch (H = 256
+        # case; 3xTF32 with the cross terms in their own accumulator, DESIGN.md 3a) and the three-launch chain (H = 512
+        # cases, mma.sync 3xTF32, one accumulator) stay a few times above it; the chain reaches 1e-5 where the value loss
+        # gradient 2 (v - ret) cancels (|v - ret| << |v| amplifies the forward error of v into every group of that critic
+        # alike).  A wrong term in a kernel shows up at 1e-2 and above.
         assert e_dev <= (3e-6 if hidden == (256, 256) else 2e-5), (name, e_dev, e_32)
 
 

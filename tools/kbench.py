@@ -45,7 +45,7 @@ def bench_gae(envs, T):
     end = dev((d["terminated"] | d["truncated"]).astype(np.uint8))
     term = dev(d["terminated"].astype(np.uint8))
     adv = torch.empty_like(v); ret = torch.empty_like(v)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
     fn = lambda: ops.gae_dual(v, vn, r, c, end, term, 0.99, 0.95, out=(adv, ret))
     mean_ms, min_ms = time_kernel(fn, flush=flush)
     alg_bytes = N * (16 * 2 + 10)   # SURVEY.md 8(d): 16*C + 10 B / transition (+1 B terminated)

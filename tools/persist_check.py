@@ -1,4 +1,4 @@
-"""Bring-up / regression check of the persistent tcgen05 PPO path (csrc/ppo_persist.cu) on a B200:
+"""Bring-up / regression check of the persistent wgmma PPO path (csrc/ppo_persist.cu) on an H100:
 
 1. ONE minibatch step: decode the operand images the kernel leaves in its workspace (h1 in both
    orientations, the W2 images) and the small-parameter gradient partials, compare them with a torch
@@ -145,9 +145,8 @@ def main():
         names = {1: "S done (h1 tile + W2 images)", 2: "G1 accumulators ready", 3: "head partial written", 4: "flag B passed",
                  5: "dz2 + partials written", 6: "G2/G3 accumulators ready", 7: "G2/G3 epilogue done", 8: "flag D1 passed",
                  9: "slices reduced, sumsq out", 10: "flag D2 passed", 11: "Adam done (step end)", 12: "[producer] flag A passed",
-                 13: "[producer] G1 copies issued", 14: "[producer] flag C passed", 16: "[mma] G1 first chunk landed",
-                 17: "[mma] G1 last chunk landed", 18: "[mma] G1 issued", 19: "[mma] G2/3 first chunk landed",
-                 20: "[mma] G2/3 last chunk landed", 21: "[mma] G2/3 issued", 22: "G2: mask applied", 23: "G2: dW1 partial stored",
+                 13: "[producer] G1 copies issued", 14: "[producer] flag C passed", 22: "G2: mask applied",
+                 23: "G2: dW1 partial stored",
                  24: "norm known", 25: "small slices stepped", 26: "head gathered, loss gradient", 27: "dz2 images stored",
                  28: "partial sums exchanged"}
         rel = dbg - dbg[:, :1]
