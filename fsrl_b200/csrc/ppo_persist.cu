@@ -26,13 +26,14 @@
 // (wgmma reads tf32 operands K-major only).
 //
 // CTA = 288 threads: warps 0-7 (two warpgroups) issue the MMAs and run the epilogue, warp 8 is the bulk-copy producer.
-// Warp w holds rows 16 (w % 4) .. + 15 of a 64-row tile; warpgroup w / 4 computes the 8-column groups its threads own
-// in the epilogue, so an accumulator tile goes from the wgmma fragment to the epilogue layout through a per-warp
-// region of shared memory without any barrier.  The 8 CTAs of a row block form a thread-block cluster: their head
-// partials travel over distributed shared memory (st.async + mbarrier complete_tx); all other hops are flag lines in
-// L2.  The cross terms of the 3-term split accumulate in their own registers.  With world > 1 the <DP = true>
-// instantiation exchanges gradients itself over peer memory (dp_* functions below: tagged + hashed 16-byte packets
-// pushed into the peers' buffers).
+// Warp w holds rows 16 (w % 4) .. + 15 of a 64-row tile.  Warpgroup 0 issues every GEMM alone with full-width
+// m64n32k8 / m64n64k8 MMAs (each reads the A tile once for all columns), and warps w and w + 4 exchange the finished
+// rows through shared memory behind one 64-thread barrier per warp pair (stage_acc).
+// The 8 CTAs of a row block form a thread-block cluster: operand chunks that several of them need are multicast
+// from L2 once into all of them (copy_operand), their head partials travel over distributed shared memory
+// (st.async + mbarrier complete_tx); all other hops are flag lines in L2.  The cross terms of the 3-term split
+// accumulate in their own registers.  With world > 1 the <DP = true> instantiation exchanges gradients itself over peer
+// memory (dp_* functions below: tagged + hashed 16-byte packets pushed into the peers' buffers).
 #include "ppo_persist.cuh"
 #include "wgmma.cuh"
 #include <cstdlib>
@@ -246,20 +247,18 @@ __device__ __forceinline__ void acc_st(float* accs, int row, int col, const floa
         *reinterpret_cast<float4*>(accs + row * ACC_LD + col + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
 }
 
-// One GEMM of the step, issued by both epilogue warpgroups straight from the operand ring: NCH chunks of KC k, A = 64
-// rows, B = b_rows rows.  Instruction h of a warpgroup covers the 8-column groups bgrp[h] and bgrp[h] + gstep (B core
-// matrices at SBO = 128 gstep bytes), i.e. exactly the columns its threads own in the epilogue.  Each warp releases a
-// slot once its MMAs have read it (bar_empty counts the NEPI / 32 warps); one group stays in flight.
-template <int NI>
-__device__ __forceinline__ void gemm_phase(const unsigned char* ring, unsigned& qq, uint64_t* bar_full, uint64_t* bar_empty,
-                                           uint32_t b_rows, const int (&bgrp)[NI], int gstep,
-                                           float (&dm)[NI][8], float (&dc)[NI][8], int* err, int code, int lane) {
+// One GEMM of the step, issued by warpgroup 0 alone straight from the operand ring: NCH chunks of KC k, A = 64 rows,
+// B = N rows, full-width m64nNk8 MMAs.  Every output element accumulates over all of K in one register chain, in the
+// same order as with narrower MMAs: the result does not depend on how the columns are cut into instructions.  Each warp
+// releases a slot once its MMAs have read it: lane r < n_dst arrives on the bar_empty of cluster rank r (bar_empty
+// counts the 4 MMA warps of each of the n_dst CTAs whose bulk copies write into the slot).  One group stays in flight.
+template <int N>
+__device__ __forceinline__ void gemm_phase(const unsigned char* ring, unsigned& qq, uint64_t* bar_full, uint32_t empty_r,
+                                           int n_dst, float (&dm)[N / 2], float (&dc)[N / 2], int* err, int code, int lane) {
 #pragma unroll
-    for (int h = 0; h < NI; ++h)
-#pragma unroll
-        for (int e = 0; e < 8; ++e) dm[h][e] = dc[h][e] = 0.f;
+    for (int e = 0; e < N / 2; ++e) dm[e] = dc[e] = 0.f;
     const uint32_t ring_a = smem_u32(ring);
-    const uint32_t b_lbo = 16 * b_rows, b_chunk = b_rows * KC * 4, b_sbo = 128 * gstep;
+    constexpr uint32_t b_lbo = 16 * N, b_chunk = N * KC * 4;
     for (int j = 0; j < NCH; ++j, ++qq) {
         const int s = qq % NSLOT;
         if (!mbar_wait(&bar_full[s], (qq / NSLOT) & 1, WAIT_CYCLES)) fail(err, code);
@@ -270,44 +269,64 @@ __device__ __forceinline__ void gemm_phase(const unsigned char* ring, unsigned& 
         for (int ks = 0; ks < KC / 8; ++ks) {
             const uint64_t ah = smem_desc(base + ks * 2048, 1024, 128);
             const uint64_t al = smem_desc(base + A_CHUNK + ks * 2048, 1024, 128);
-#pragma unroll
-            for (int h = 0; h < NI; ++h) {
-                const uint32_t bo = 2 * A_CHUNK + ks * 2 * b_lbo + 128 * bgrp[h];
-                const uint64_t bh = smem_desc(base + bo, b_lbo, b_sbo);
-                const uint64_t bl = smem_desc(base + bo + b_chunk, b_lbo, b_sbo);
-                mma_m64n16k8_tf32(dc[h], al, bh);
-                mma_m64n16k8_tf32(dc[h], ah, bl);
-                mma_m64n16k8_tf32(dm[h], ah, bh);
+            const uint64_t bh = smem_desc(base + 2 * A_CHUNK + ks * 2 * b_lbo, b_lbo, 128);
+            const uint64_t bl = smem_desc(base + 2 * A_CHUNK + ks * 2 * b_lbo + b_chunk, b_lbo, 128);
+            if constexpr (N == 32) {
+                mma_m64n32k8_tf32(dc, al, bh);
+                mma_m64n32k8_tf32(dc, ah, bl);
+                mma_m64n32k8_tf32(dm, ah, bh);
+            } else {
+                mma_m64n64k8_tf32(dc, al, bh);
+                mma_m64n64k8_tf32(dc, ah, bl);
+                mma_m64n64k8_tf32(dm, ah, bh);
             }
         }
         wgmma_commit();
         if (j > 0) {
             wgmma_wait<1>();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&bar_empty[(qq - 1) % NSLOT]);
+            if (lane < n_dst) mbar_arrive_cluster(empty_r + 8 * ((qq - 1) % NSLOT));
         }
     }
     wgmma_wait<0>();
-#pragma unroll
-    for (int h = 0; h < NI; ++h) { reg_fence(dm[h]); reg_fence(dc[h]); }
+    reg_fence(dm); reg_fence(dc);
     __syncwarp();
-    if (lane == 0) mbar_arrive(&bar_empty[(qq - 1) % NSLOT]);
+    if (lane < n_dst) mbar_arrive_cluster(empty_r + 8 * ((qq - 1) % NSLOT));
 }
-// fragment (wgmma.cuh) -> accs, main + cross terms; warp w % 4 writes rows 16 (w % 4) .. + 15 of its column groups
-template <int NI>
-__device__ __forceinline__ void stage_acc(float* accs, const float (&dm)[NI][8], const float (&dc)[NI][8], const int (&bgrp)[NI],
-                                          int gstep, int sp, int lane) {
-    const int r = 16 * sp + (lane >> 2);
+// Warp w of warpgroup 0 stages its fragment (main + cross terms, rows 16 w .. + 15, all N columns) into accs; warps w
+// and w + 4 read those rows back in the epilogue, so one 64-thread barrier per warp pair (ids 2 .. 5) orders them.
+template <int N>
+__device__ __forceinline__ void stage_acc(float* accs, const float (&dm)[N / 2], const float (&dc)[N / 2], int wq, int sp,
+                                          int lane) {
+    if (wq == 0) {
+        const int r = 16 * sp + (lane >> 2);
 #pragma unroll
-    for (int h = 0; h < NI; ++h)
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const int col = 8 * (bgrp[h] + gstep * i) + 2 * (lane & 3);
-            *reinterpret_cast<float2*>(accs + r * ACC_LD + col) = make_float2(dm[h][4 * i] + dc[h][4 * i], dm[h][4 * i + 1] + dc[h][4 * i + 1]);
-            *reinterpret_cast<float2*>(accs + (r + 8) * ACC_LD + col) =
-                make_float2(dm[h][4 * i + 2] + dc[h][4 * i + 2], dm[h][4 * i + 3] + dc[h][4 * i + 3]);
+        for (int i = 0; i < N / 8; ++i) {
+            const int c = 8 * i + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(accs + r * ACC_LD + c) = make_float2(dm[4 * i] + dc[4 * i], dm[4 * i + 1] + dc[4 * i + 1]);
+            *reinterpret_cast<float2*>(accs + (r + 8) * ACC_LD + c) =
+                make_float2(dm[4 * i + 2] + dc[4 * i + 2], dm[4 * i + 3] + dc[4 * i + 3]);
         }
-    __syncwarp();
+    }
+    asm volatile("bar.sync %0, 64;" ::"r"(2 + sp) : "memory");
+}
+
+// One operand of a ring chunk: its hi part (`bytes` from src) and lo part (`bytes` from src + IMG) go to dst and
+// dst + bytes.  g == 1: this CTA copies both for itself.  Otherwise the g CTAs of cta_mask (cluster ranks) need the same
+// operand: member i of the group copies the i-th of g equal pieces of [hi | lo] into all of them, so the cluster reads it
+// from L2 once.  Every destination expects the bytes of the whole slot on its own bar_full, and a slot is written again
+// only after the consumers of every destination CTA have released it (gemm_phase arrives on all 8 CTAs' bar_empty).
+// A peer writes into this CTA's ring only after flag A or flag C, and both count this CTA's own arrival, which follows
+// its fence.proxy.async.shared::cta: the epilogue's scratch use of the ring is over by then.
+__device__ __forceinline__ void copy_operand(unsigned char* dst, const float* src, uint32_t bytes, uint64_t* bar, int g, int i,
+                                             uint16_t cta_mask) {
+    if (g == 1) {
+        bulk_g2s(dst, src, bytes, bar);
+        bulk_g2s(dst + bytes, src + IMG, bytes, bar);
+        return;
+    }
+    const uint32_t piece = 2 * bytes / g, off = i * piece, part = off / bytes, in = off % bytes;
+    bulk_g2s_multicast(dst + off, src + (size_t)part * IMG + in / 4, piece, bar, cta_mask);
 }
 
 // Transposed K-major image of a 64-row tile through shared memory.  Every epilogue thread holds NC consecutive
@@ -530,10 +549,11 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     float* sp_m = small + sm.n;          // Adam first moment
     float* sp_v = small + 2 * sm.n;      // Adam second moment
     float* sp_g = small + 3 * sm.n;      // reduced gradient of the current step
-    float* land = small + 4 * sm.n;      // cluster mode: head partials pushed by the 8 CTAs of this row block [b][64][OUTP]
+    float* land = small + 4 * sm.n;      // head partials pushed by the 8 CTAs of this row block [b][64][OUTP] (cluster
+                                         // mode), G2's observation block
 
     if (tid == 0) {
-        for (int i = 0; i < NSLOT; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], NEPI / 32); }
+        for (int i = 0; i < NSLOT; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 4 * (P.cluster ? 8 : 1)); }
         mbar_init(&bar_b, 1);                // per step: one local expect_tx arrival + 16 KB of remote st.async bytes
         fence_mbar_init();
     }
@@ -561,10 +581,9 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                     unsigned char* dst = ring + (size_t)s * SLOT_BYTES;
                     mbar_expect_tx(&bar_full[s], 3 * A_CHUNK);
                     const size_t ao = (size_t)a * 16384 + (size_t)j * 64 * KC, bo = (size_t)b * 8192 + (size_t)j * 32 * KC;
-                    bulk_g2s(dst, wsn + (size_t)I_H1A_HI * IMG + ao, A_CHUNK, &bar_full[s]);
-                    bulk_g2s(dst + A_CHUNK, wsn + (size_t)I_H1A_LO * IMG + ao, A_CHUNK, &bar_full[s]);
-                    bulk_g2s(dst + 2 * A_CHUNK, wsn + (size_t)I_W2A_HI * IMG + bo, A_CHUNK / 2, &bar_full[s]);
-                    bulk_g2s(dst + 2 * A_CHUNK + A_CHUNK / 2, wsn + (size_t)I_W2A_LO * IMG + bo, A_CHUNK / 2, &bar_full[s]);
+                    // A = H1A block a: the same for the 8 CTAs of the row block (cluster)
+                    copy_operand(dst, wsn + (size_t)I_H1A_HI * IMG + ao, A_CHUNK, &bar_full[s], P.cluster ? 8 : 1, b, 0xff);
+                    copy_operand(dst + 2 * A_CHUNK, wsn + (size_t)I_W2A_HI * IMG + bo, A_CHUNK / 2, &bar_full[s], 1, 0, 0);
                 }
                 STAMP(13);
                 if (!flag_wait_ge<true>(fl_net + F_C * FLAG_LINE, 32u * (t + 1), WAIT_CYCLES)) fail(P.err, 12);
@@ -572,16 +591,18 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 fence_proxy_async();
                 const int ia = is_g2 ? I_W2B_HI : I_DZT_HI, ib = is_g2 ? I_DZA_HI : I_H1T_HI;
                 const int blk_a = is_g2 ? ka : q4, blk_b = is_g2 ? q4 : ka;
+                // with clusters, the k block ka (G2: A = W2B, G3: B = H1T) is shared by the 4 CTAs with the same b >> 2,
+                // the block q4 (G2: B = DZA, G3: A = DZT) by the CTAs b and b ^ 4
+                const int g4 = P.cluster ? 4 : 1, g2 = P.cluster ? 2 : 1;
+                const uint16_t m4 = (uint16_t)(0xfu << (b & 4)), m2 = (uint16_t)(0x11u << (b & 3));
                 for (int j = 0; j < NCH; ++j, ++qq) {             // G2: K = o ; G3: K = r ; chunks of KC
                     const int s = qq % NSLOT;
                     if (!mbar_wait(&bar_empty[s], ((qq / NSLOT) & 1) ^ 1, WAIT_CYCLES)) fail(P.err, 13);
                     unsigned char* dst = ring + (size_t)s * SLOT_BYTES;
                     mbar_expect_tx(&bar_full[s], 4 * A_CHUNK);
                     const size_t ao = (size_t)blk_a * 16384 + (size_t)j * 64 * KC, bo = (size_t)blk_b * 16384 + (size_t)j * 64 * KC;
-                    bulk_g2s(dst, wsn + (size_t)ia * IMG + ao, A_CHUNK, &bar_full[s]);
-                    bulk_g2s(dst + A_CHUNK, wsn + (size_t)(ia + 1) * IMG + ao, A_CHUNK, &bar_full[s]);
-                    bulk_g2s(dst + 2 * A_CHUNK, wsn + (size_t)ib * IMG + bo, A_CHUNK, &bar_full[s]);
-                    bulk_g2s(dst + 3 * A_CHUNK, wsn + (size_t)(ib + 1) * IMG + bo, A_CHUNK, &bar_full[s]);
+                    copy_operand(dst, wsn + (size_t)ia * IMG + ao, A_CHUNK, &bar_full[s], is_g2 ? g4 : g2, is_g2 ? b & 3 : b >> 2, is_g2 ? m4 : m2);
+                    copy_operand(dst + 2 * A_CHUNK, wsn + (size_t)ib * IMG + bo, A_CHUNK, &bar_full[s], is_g2 ? g2 : g4, is_g2 ? b >> 2 : b & 3, is_g2 ? m2 : m4);
                 }
             }
         }
@@ -594,8 +615,10 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
         const int trow = 16 * sp + r16;             // row of the 64-row tile held by this lane
         const int cb1 = 16 * half + C1 * wq;        // first of this thread's C1 columns of a 32-column tile
         const int cb2 = 32 * half + C2 * wq;        // first of this thread's C2 columns of a 64-column tile
-        const int bg1[1] = {wq}, bg2[2] = {2 * wq, 2 * wq + 4};   // column groups of the warpgroup's MMAs: G1, G2 / G3
         unsigned qq = 0;                            // operand ring position
+        // ring releases go to every CTA whose bulk copies write into this one's slots: with clusters, all 8 (multicast)
+        const int n_dst = P.cluster ? 8 : 1;
+        const uint32_t empty_r = mapa_u32(smem_u32(bar_empty), lane < n_dst ? lane : 0);
         float w2p[C2], w2m[C2], w2v[C2];            // owned W2 tile (G3 CTAs): parameters and Adam moments
         float* stat_base = u.stats;
         // ---- data-parallel exchange over peer memory (NVLink): every CTA pushes its local gradient piece into its
@@ -761,9 +784,10 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
 
             // ---- G1 (wgmma), then its epilogue: h2 = relu(acc + b2), head partial over this tile's 32 columns ----
             {
-                float dm[1][8], dc[1][8];
-                gemm_phase<1>(ring, qq, bar_full, bar_empty, 32, bg1, 2, dm, dc, P.err, 30, lane);
-                stage_acc<1>(accs, dm, dc, bg1, 2, sp, lane);
+                float dm[16], dc[16];
+                if (wq == 0) gemm_phase<32>(ring, qq, bar_full, empty_r, n_dst, dm, dc, P.err, 30, lane);
+                else qq += NCH;
+                stage_acc<32>(accs, dm, dc, wq, sp, lane);
             }
             if (et == 0) STAMP(2);
             float h2[C1];
@@ -1005,58 +1029,48 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             // ---- G2 / G3 epilogue ---------------------------------------------------------------------------
             // G2: what does not depend on the accumulators is requested BEFORE waiting for them -- the ReLU mask of
             // this lane's h1 entries (image H1A, complete since flag A) and this thread's share of the 64 x D
-            // observation block of row block q4
-            float mreg[C2];
-            float xr[(64 * MAXD + NEPI - 1) / NEPI];
-            const int nx = (64 * D + NEPI - 1) / NEPI;
+            // observation block of row block q4.  Neither stays in registers across the GEMM, whose accumulators need
+            // them: the mask is kept as C2 bits, the block is staged in the hop-B landing zone, idle until the next step
+            // (row r at r * D + (r >> 5): the two half-warps read different banks).
+            unsigned mbits = 0;
             if (is_g2) {
                 const int k = 64 * ka + trow;
                 const float* msk = wsn + (size_t)I_H1A_HI * IMG + (size_t)q4 * 16384 + (size_t)(k >> 2) * 256 + (k & 3);
+                float mreg[C2];
 #pragma unroll
                 for (int jq = 0; jq < C2; ++jq) mreg[jq] = __ldcg(msk + (size_t)(cb2 + jq) * 4);
+                float xr[(64 * MAXD + NEPI - 1) / NEPI];
+                const int nx = (64 * D + NEPI - 1) / NEPI;
                 const float* xb = u.obs + (row0 + 64 * q4) * D;
 #pragma unroll
                 for (int q = 0; q < (64 * MAXD + NEPI - 1) / NEPI; ++q)
                     xr[q] = (q < nx && et + q * NEPI < 64 * D) ? __ldg(xb + et + q * NEPI) : 0.f;
-                // cluster launches: the hop-B landing zone is idle until the next step -- the observation block is staged
-                // there NOW, while the GEMM still runs (row r at r * D + (r >> 5): the two half-warps read different banks)
-                if (P.cluster) {
 #pragma unroll
-                    for (int q = 0; q < (64 * MAXD + NEPI - 1) / NEPI; ++q) {
-                        const int e = et + q * NEPI;
-                        if (q < nx && e < 64 * D) { const int r = e / D; land[e + (r >> 5)] = xr[q]; }
-                    }
+                for (int jq = 0; jq < C2; ++jq) mbits |= (mreg[jq] > 0.f ? 1u : 0u) << jq;
+#pragma unroll
+                for (int q = 0; q < (64 * MAXD + NEPI - 1) / NEPI; ++q) {
+                    const int e = et + q * NEPI;
+                    if (q < nx && e < 64 * D) { const int r = e / D; land[e + (r >> 5)] = xr[q]; }
                 }
             }
             {
-                float dm[2][8], dc[2][8];
-                gemm_phase<2>(ring, qq, bar_full, bar_empty, 64, bg2, 1, dm, dc, P.err, 32, lane);
-                stage_acc<2>(accs, dm, dc, bg2, 1, sp, lane);
+                float dm[32], dc[32];
+                if (wq == 0) gemm_phase<64>(ring, qq, bar_full, empty_r, n_dst, dm, dc, P.err, 32, lane);
+                else qq += NCH;
+                stage_acc<64>(accs, dm, dc, wq, sp, lane);
             }
             if (et == 0) STAMP(6);
             float sq = 0.f;
             if (is_g2) {
-                // without clusters the observation block goes to slot 0 of the operand ring, idle from here until the
-                // next step's flag A -- once BOTH warpgroups are past gemm_phase: each warp has only waited for its own
-                // MMAs, and the other warpgroup's may still be reading the last chunks of the ring
-                float* xs = P.cluster ? land : reinterpret_cast<float*>(ring);
-                if (!P.cluster) {
-                    epi_bar();
-#pragma unroll
-                    for (int q = 0; q < (64 * MAXD + NEPI - 1) / NEPI; ++q) {
-                        const int e = et + q * NEPI;
-                        if (q < nx && e < 64 * D) { const int r = e / D; xs[e + (r >> 5)] = xr[q]; }
-                    }
-                }
                 // lane: k = 64 ka + trow ; rows cb2 + j of row block q4; partial set 2 q4 + wq (WQ sets per row block)
                 float v[C2];
                 acc_ld<C2>(accs, trow, cb2, v);
                 const int k = 64 * ka + trow;
 #pragma unroll
-                for (int jq = 0; jq < C2; ++jq) v[jq] = (mreg[jq] > 0.f) ? v[jq] : 0.f;
+                for (int jq = 0; jq < C2; ++jq) v[jq] = ((mbits >> jq) & 1u) ? v[jq] : 0.f;
                 epi_bar();
                 if (et == 0) STAMP(22);
-                const float* xh = xs + (size_t)cb2 * D + half;
+                const float* xh = land + (size_t)cb2 * D + half;
                 float* dst = wsn + DW1P_OFF + (size_t)(WQ * q4 + wq) * (MAXD + 1) * H + k;
                 for (int d = 0; d < D; ++d) {
                     float sacc = 0.f;
@@ -1217,9 +1231,9 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     if (P.cluster) cluster_sync_all();
 }
 
-static size_t smem_bytes(int D, bool cluster = false) {
+static size_t smem_bytes(int D) {
     return (size_t)NSLOT * SLOT_BYTES + sizeof(float) * 64 * ACC_LD + 4 * sizeof(float) * SliceMap(D).n +
-           (cluster ? sizeof(float) * 8 * 64 * OUTP : 0);
+           sizeof(float) * 8 * 64 * OUTP;
 }
 
 }  // namespace pp
@@ -1282,16 +1296,10 @@ int ppo_persist_run(const fsrl_ppo_update_t& ug, int n_mb, int stats_slot0, long
         a.dbg = reinterpret_cast<long long*>(tab_dev + 2 * (size_t)pp::MAX_MB);
         a.dbg_step = atoi(e);
     }
-    // clusters of 8 CTAs (the column blocks of one row block) when the landing zone fits and all clusters can be
-    // co-resident; otherwise hop B goes through global memory like the other hops
-    static int smem_optin = -1;
-    if (smem_optin < 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    }
-    bool cluster = !getenv("FSRL_PPO_NO_CLUSTER") && pp::smem_bytes(ug.D, true) + 8192 <= (size_t)smem_optin;
-    size_t smem = pp::smem_bytes(ug.D, cluster);
+    // clusters of 8 CTAs (the column blocks of one row block) when all clusters can be co-resident; otherwise hop B goes
+    // through global memory like the other hops, and every CTA copies its operands itself
+    bool cluster = !getenv("FSRL_PPO_NO_CLUSTER");
+    const size_t smem = pp::smem_bytes(ug.D);
     const bool dp = ug.world > 1 || getenv("FSRL_PPO_FORCE_DP_KERNEL") != nullptr;   // (the env switch: code-generation experiments)
     void (*kern)(const pp::Args) = dp ? pp::ppo_persist_kernel<true> : pp::ppo_persist_kernel<false>;
     static size_t set[2] = {0, 0};
@@ -1310,8 +1318,6 @@ int ppo_persist_run(const fsrl_ppo_update_t& ug, int n_mb, int stats_slot0, long
         if (cudaOccupancyMaxActiveClusters(&n_clusters, kern, &cfg) != cudaSuccess || n_clusters < 4 * ug.n_nets) {
             cudaGetLastError();
             cluster = false;
-            smem = pp::smem_bytes(ug.D, false);
-            cfg.dynamicSmemBytes = smem;
         }
     }
     if (!cluster) { cfg.attrs = nullptr; cfg.numAttrs = 0; }

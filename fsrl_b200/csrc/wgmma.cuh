@@ -34,6 +34,13 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// arrival on an mbarrier of any CTA of the cluster (shared::cluster address from mapa), default semantics (release at
+// CTA scope).  Used to release a ring slot once wgmma.wait_group has retired the MMAs that read it; a cluster-scope
+// release would add a fence to every arrival (on H100 it cost an earlier version of the persistent PPO kernel about
+// 14 k cycles per minibatch step).
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -59,6 +66,13 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
         ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
+// the same copy into the same shared-memory offset of every CTA of `cta_mask` (cluster ranks), each completing its
+// bytes on the mbarrier at the same offset in that CTA
+__device__ __forceinline__ void bulk_g2s_multicast(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar, uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
+        ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask) : "memory");
+}
 // orders this thread's earlier generic-proxy operations (the acquire of a flag) before its later
 // async-proxy operations (bulk copies reading what another SM wrote with ordinary stores)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
@@ -73,14 +87,26 @@ __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes
     return (uint64_t)((saddr >> 4) & 0x3fffu) | ((uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16) |
            ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32);
 }
-// D[64 x 16] += A[64 x 8] B[16 x 8]^T for the executing warpgroup.  Fragment of thread (warp w of the warpgroup, lane l):
-// d[4 i + e] = D[16 w + l / 4 + 8 (e >> 1)][8 i + 2 (l % 4) + (e & 1)],  i = 0, 1
-__device__ __forceinline__ void mma_m64n16k8_tf32(float (&d)[8], uint64_t adesc, uint64_t bdesc) {
+// D[64 x N] += A[64 x 8] B[N x 8]^T for the executing warpgroup, N = 32 or 64.  Fragment of thread (warp w of the
+// warpgroup, lane l): d[4 i + e] = D[16 w + l / 4 + 8 (e >> 1)][8 i + 2 (l % 4) + (e & 1)],  i = 0 .. N / 8 - 1
+__device__ __forceinline__ void mma_m64n32k8_tf32(float (&d)[16], uint64_t adesc, uint64_t bdesc) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %10, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "n"(1));
+}
+__device__ __forceinline__ void mma_m64n64k8_tf32(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "l"(adesc), "l"(bdesc), "n"(1));
 }
 // before the first wgmma that reads accumulator registers written by ordinary instructions
@@ -90,9 +116,10 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accesses to accumulator registers across wgmma_wait
-__device__ __forceinline__ void reg_fence(float (&d)[8]) {
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) asm volatile("" : "+f"(d[i])::"memory");
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // ---- device-scope flag barriers between the CTAs of a co-resident grid ---------------------------
