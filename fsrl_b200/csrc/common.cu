@@ -1,5 +1,6 @@
-// C-ABI plumbing shared by every entry point: thread-local error text, version, device info.
-#include "common.cuh"
+// C-ABI plumbing shared by every entry point: thread-local error text, version, device info;
+// the W2 mirror kernel of every learner.
+#include "arena.cuh"
 #include "fsrl_b200.h"
 #include <stdarg.h>
 #include <string.h>
@@ -24,6 +25,20 @@ int sm_count() {
         cached[dev] = n;
     }
     return cached[dev];
+}
+
+__global__ void w2_mirror_kernel(const W2Mirror mr, int H) {
+    const float* src = mr.w2t[blockIdx.y];
+    const int tt = blockIdx.x;
+    w2_tile(mr.w2n[blockIdx.y], H, (tt / (H / 32)) * 32, (tt % (H / 32)) * 32,
+            [&](int k, int o) { return src[(size_t)k * H + o]; });
+}
+
+int launch_w2_mirror(const W2Mirror& mr, int n_nets, int H, cudaStream_t s) {
+    FSRL_REQUIRE(n_nets >= 1 && n_nets <= W2_MIRROR_MAX_NETS, "w2 mirror: %d nets in one launch", n_nets);
+    w2_mirror_kernel<<<dim3((H / 32) * (H / 32), n_nets), 256, 0, s>>>(mr, H);
+    FSRL_LAUNCH_CHECK();
+    return FSRL_OK;
 }
 }  // namespace fsrl
 

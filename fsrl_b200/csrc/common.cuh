@@ -63,6 +63,22 @@ __device__ __forceinline__ double warp_sum(double v) {
     return v;
 }
 
+// Sum over a block of NWARPS warps, returned to every thread: warp sums, then the warp partials
+// added in warp order.  red holds NWARPS values; the leading barrier lets a caller reuse it.
+template <int NWARPS, class T>
+__device__ __forceinline__ T block_sum(T v, T* red) {
+    v = warp_sum(v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    T t = 0;
+#pragma unroll
+    for (int i = 0; i < NWARPS; ++i) t += red[i];
+    return t;
+}
+
+constexpr float LOG_SQRT_2PI = 0.9189385332046727f;   // log(sqrt(2 pi)) of the Gaussian log-density
+
 // streaming (read-once) loads: keep them out of L1
 __device__ __forceinline__ float4 ldg_stream4(const float* p) {
     return __ldcs(reinterpret_cast<const float4*>(p));
@@ -99,6 +115,16 @@ struct Philox {
         out[0] = c[0]; out[1] = c[1]; out[2] = c[2]; out[3] = c[3];
     }
 };
+
+// Box-Muller in f64 from two Philox words (CPU twin: oracle/philox.py normal_pair)
+__device__ __forceinline__ void gauss_pair(uint32_t a, uint32_t b, float& n0, float& n1) {
+    const double u1 = ((double)a + 1.0) * (1.0 / 4294967296.0);
+    const double u2 = (double)b * (1.0 / 4294967296.0);
+    const double r = sqrt(-2.0 * log(u1));
+    const double ang = 2.0 * 3.141592653589793 * u2;
+    n0 = (float)(r * cos(ang));
+    n1 = (float)(r * sin(ang));
+}
 
 // u32 -> uniform in (0,1]: (x + 1) * 2^-32 computed in f32 via the 24 top bits
 __host__ __device__ inline float u01(uint32_t x) {

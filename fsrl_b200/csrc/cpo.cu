@@ -22,8 +22,6 @@
 
 namespace fsrl {
 
-constexpr float LOG_SQRT_2PI_C = 0.9189385332046727f;
-
 // ---- per-row head kernel --------------------------------------------------------------------------
 // mode: 0 = evaluate sums only, 1 = d objective, 2 = d(-cost_surrogate), 3 = d kl
 // sums[0..3] += objective_sum, cost_ratio_sum, kl_sum, (unused); dout rows [N][16]:
@@ -48,7 +46,7 @@ __global__ void cpo_head_kernel(const fsrl_cpo_t d, long long N, int mode, doubl
                 const float ls = d.log_sigma[j];
                 sg[j] = expf(ls);
                 z_[j] = (d.act[(size_t)r * A + j] - mu[j]) / sg[j];
-                logp += -0.5f * z_[j] * z_[j] - ls - LOG_SQRT_2PI_C;
+                logp += -0.5f * z_[j] * z_[j] - ls - LOG_SQRT_2PI;
                 // kl_divergence(Normal(mu_old, s_old), Normal(mu, s))  (torch formula)
                 const float so = d.std_old[(size_t)r * A + j], mo = d.mean_old[(size_t)r * A + j];
                 const float vr = (so / sg[j]) * (so / sg[j]);
@@ -125,7 +123,7 @@ __global__ void focops_head_kernel(const fsrl_cpo_t d, long long N, float inv_la
                 const float ls = d.log_sigma[j];
                 sg[j] = expf(ls);
                 z_[j] = (d.act[(size_t)r * A + j] - mu) / sg[j];
-                logp += -0.5f * z_[j] * z_[j] - ls - LOG_SQRT_2PI_C;
+                logp += -0.5f * z_[j] * z_[j] - ls - LOG_SQRT_2PI;
                 // kl_divergence(Normal(mu, s), Normal(mu_old, s_old))  (torch formula, p = new, q = old)
                 const float so = d.std_old[(size_t)r * A + j], mo = d.mean_old[(size_t)r * A + j];
                 const float vr = (sg[j] / so) * (sg[j] / so);
@@ -219,9 +217,9 @@ cpo_rfwd_kernel(const fsrl_engine_t e, const fsrl_netref_t np_, const fsrl_netre
     const int tid = threadIdx.x;
     const int r0 = blockIdx.x * TT::R;
     const int inp = TT::in_pad(D);
-    // tangent parameter views
-    const float* v_w1t = pv; const float* v_b1 = v_w1t + (size_t)D * H; const float* v_w2t = v_b1 + H;
-    const float* v_b2 = v_w2t + (size_t)H * H; const float* v_w3t = v_b2 + H; const float* v_b3 = v_w3t + (size_t)H * out;
+    const ArenaLayout L = arena_layout(D, H, out, 0);     // tangent parameters
+    const float *v_w1t = pv + L.w1, *v_b1 = pv + L.b1, *v_w2t = pv + L.w2, *v_b2 = pv + L.b2, *v_w3t = pv + L.w3,
+                *v_b3 = pv + L.b3;
     float* xs = smem;                                   // [R][inp]
     float* ta = xs + (size_t)TT::R * inp;               // tile A [R][LDA]  (Rh1, later h2 cache)
     float* tb = ta + (size_t)TT::R * TT::LDA;           // tile B           (h1 cache, later Rh2)
@@ -305,7 +303,7 @@ cpo_rbwd_kernel(const fsrl_engine_t e, const fsrl_netref_t np_, const fsrl_netre
     const int D = np_.D, out = np_.out;
     const int tid = threadIdx.x;
     const int r0 = blockIdx.x * TT::R;
-    const float* v_w3t = pv + (size_t)D * H + H + (size_t)H * H + H;
+    const float* v_w3t = pv + arena_layout(D, H, out, 0).w3;
     float* ta = smem;                                   // Rda2 tile
     float* tb = ta + (size_t)TT::R * TT::LDA;           // da2 (primal) tile
     float* wst = tb + (size_t)TT::R * TT::LDA;
@@ -360,10 +358,8 @@ __global__ void __launch_bounds__(1024) vec_dot_kernel(const float* a, const flo
     __shared__ double red[32];
     double s = 0.0;
     for (long long i = threadIdx.x; i < n; i += 1024) s += (double)a[i] * (double)b[i];
-    s = warp_sum(s);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) { double t = 0.0; for (int w = 0; w < 32; ++w) t += red[w]; *out = t; }
+    s = block_sum<32>(s, red);
+    if (threadIdx.x == 0) *out = s;
 }
 // y = a*x + b*y
 __global__ void vec_axpby_kernel(float a, const float* x, float b, float* y, long long n) {
@@ -375,17 +371,6 @@ __global__ void vec_add_scaled_kernel(const float* a, float s, const float* b, f
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = a[i] + s * b[i];
 }
-// mirror of the W2 block of a tangent vector: dst[o][k] = src[k][o]
-__global__ void vec_w2_mirror_kernel(const float* src_w2t, float* dst, int H) {
-    __shared__ float tile[32][33];
-    const int tt = blockIdx.x;
-    const int k0 = (tt / (H / 32)) * 32, o0 = (tt % (H / 32)) * 32;
-    const int lx = threadIdx.x % 32, ly = threadIdx.x / 32;
-    for (int q = 0; q < 4; ++q) tile[ly + 8 * q][lx] = src_w2t[(size_t)(k0 + ly + 8 * q) * H + o0 + lx];
-    __syncthreads();
-    for (int q = 0; q < 4; ++q) dst[(size_t)(o0 + ly + 8 * q) * H + k0 + lx] = tile[lx][ly + 8 * q];
-}
-
 }  // namespace fsrl
 
 using namespace fsrl;
@@ -437,11 +422,15 @@ extern "C" int fsrl_cpo_hvp(const fsrl_cpo_t* d, const float* v, float* v_w2n_sc
     const fsrl_netref_t& nr_ = d->actor_r.nets[0];
     const int H = np_.H, D = np_.D, out = np_.out;
     const int B = (int)d->N;
-    const long long P = (long long)D * H + H + (long long)H * H + H + (long long)H * out + out + np_.n_extra;
+    const ArenaLayout L = arena_layout(D, H, out, np_.n_extra);
+    const long long P = L.size;
     fsrl_eng_input_t in;
     in.xa = d->obs; in.ia = d->perm; in.xb = nullptr; in.ib = nullptr; in.Da = D; in.Db = 0;
-    vec_w2_mirror_kernel<<<(H / 32) * (H / 32), 256, 0, s>>>(v + (size_t)D * H + H, v_w2n_scratch, H);
-    FSRL_LAUNCH_CHECK();
+    W2Mirror mr;
+    mr.w2t[0] = v + L.w2;
+    mr.w2n[0] = v_w2n_scratch;
+    rc = launch_w2_mirror(mr, 1, H, s);
+    if (rc) return rc;
     ENG_DISPATCH_H(H, {
         using TT = MlpTile<HH>;
         const size_t smf = sizeof(float) * ((size_t)TT::R * TT::in_pad(D) + 2 * (size_t)TT::R * TT::LDA + TT::stage_floats() + 2 * (size_t)HH * out);
@@ -450,13 +439,12 @@ extern "C" int fsrl_cpo_hvp(const fsrl_cpo_t* d, const float* v, float* v_w2n_sc
     });
     FSRL_LAUNCH_CHECK();
     {
-        EngView Rv;   // host-side pointer arithmetic for the tangent slot's out / dout
+        // the tangent slot's out / dout
         const size_t slotf = eng_slot_floats(H, d->eng.bmax);
         float* sc = d->eng.scratch + (size_t)nr_.slot * slotf;
         float* r_out = sc + 4 * (size_t)d->eng.bmax * H;
         float* r_dout = r_out + (size_t)d->eng.bmax * 16;
-        (void)Rv;
-        cpo_rhead_kernel<<<(unsigned)((d->N + 255) / 256), 256, 0, s>>>(*d, d->N, r_out, v + (P - np_.n_extra), r_dout);
+        cpo_rhead_kernel<<<(unsigned)((d->N + 255) / 256), 256, 0, s>>>(*d, d->N, r_out, v + L.extra, r_dout);
         FSRL_LAUNCH_CHECK();
     }
     ENG_DISPATCH_H(H, {
@@ -598,33 +586,19 @@ __global__ void mse_head_kernel(const float* __restrict__ out, const float* __re
         *reinterpret_cast<float4*>(dout + (size_t)i * 16 + 12) = z;
         s = (double)td * (double)td;
     }
-    s = warp_sum(s);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) { double t = 0.0; for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w]; atomicAdd(sums, t); }
+    s = block_sum<8>(s, red);   // launched with 256 threads
+    if (threadIdx.x == 0) atomicAdd(sums, s);
 }
 
 // x <- (x - mean) / std (unbiased, no eps) over n elements: cpo.py:127-131 / trpo_lag.py:129-133
 __global__ void __launch_bounds__(1024) standardize_kernel(float* x, long long n) {
     __shared__ double red[32];
-    __shared__ double s_mean, s_rstd;
     double s = 0.0;
     for (long long i = threadIdx.x; i < n; i += 1024) s += (double)x[i];
-    s = warp_sum(s);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) { double t = 0.0; for (int w = 0; w < 32; ++w) t += red[w]; s_mean = t / (double)n; }
-    __syncthreads();
-    const float mean = (float)s_mean;
+    const float mean = (float)(block_sum<32>(s, red) / (double)n);
     double q = 0.0;
     for (long long i = threadIdx.x; i < n; i += 1024) { const float d = x[i] - mean; q += (double)(d * d); }
-    q = warp_sum(q);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = q;
-    __syncthreads();
-    if (threadIdx.x == 0) { double t = 0.0; for (int w = 0; w < 32; ++w) t += red[w]; s_rstd = 1.0 / sqrt(t / (double)(n - 1)); }
-    __syncthreads();
-    const float rstd = (float)s_rstd;
+    const float rstd = (float)(1.0 / sqrt(block_sum<32>(q, red) / (double)(n - 1)));
     for (long long i = threadIdx.x; i < n; i += 1024) x[i] = (x[i] - mean) * rstd;
 }
 }  // namespace fsrl

@@ -17,10 +17,7 @@ namespace fsrl {
 
 constexpr int EDOUT_LD = 16;
 
-struct EngView {
-    Mlp3 m;
-    const float* w2n;
-    float *g_w1t, *g_b1, *g_w2t, *g_b2, *g_w3t, *g_b3, *g_extra;
+struct EngView : ArenaNet {   // + the net's scratch slot
     float *s_h1, *s_h2, *s_dz1, *s_dz2, *s_out, *s_dout, *s_dx;
 };
 
@@ -30,19 +27,8 @@ __host__ __device__ inline size_t eng_slot_floats(int H, int bmax) {
 
 __device__ __forceinline__ EngView eng_view(const fsrl_engine_t& e, const fsrl_netref_t& n) {
     EngView v;
-    const int H = n.H, D = n.D, out = n.out;
-    const float* th = e.theta + n.off;
-    float* g = e.grad + n.off;
-    size_t o = 0;
-    v.m.w1t = th + o; v.g_w1t = g + o; o += (size_t)D * H;
-    v.m.b1 = th + o;  v.g_b1 = g + o;  o += H;
-    v.m.w2t = th + o; v.g_w2t = g + o; o += (size_t)H * H;
-    v.m.b2 = th + o;  v.g_b2 = g + o;  o += H;
-    v.m.w3t = th + o; v.g_w3t = g + o; o += (size_t)H * out;
-    v.m.b3 = th + o;  v.g_b3 = g + o;  o += out;
-    v.g_extra = g + o;
-    v.m.in = D; v.m.H = H; v.m.out = out;
-    v.w2n = e.w2n + n.w2n_off;
+    const int H = n.H;
+    arena_net(v, e.theta + n.off, e.grad + n.off, e.w2n + n.w2n_off, n.D, H, n.out);
     float* sc = e.scratch + (size_t)n.slot * eng_slot_floats(H, e.bmax);
     const size_t bh = (size_t)e.bmax * H;
     v.s_h1 = sc; v.s_h2 = sc + bh; v.s_dz1 = sc + 2 * bh; v.s_dz2 = sc + 3 * bh;

@@ -23,20 +23,10 @@
 // activations stay in shared memory between layers (row stride H+4: conflict-free A
 // fragments).
 #pragma once
-#include "common.cuh"
+#include "arena.cuh"
 #include <cuda_pipeline.h>
 
 namespace fsrl {
-
-struct Mlp3 {            // device pointers, canonical layout
-    const float* w1t;    // [in][H]
-    const float* b1;     // [H]
-    const float* w2t;    // [H][H]
-    const float* b2;     // [H]
-    const float* w3t;    // [H][out]
-    const float* b3;     // [out]
-    int in, H, out;
-};
 
 constexpr int MLP_TPB = 256;
 constexpr int MLP_KC = 16;          // k-rows of a weight matrix per pipeline stage

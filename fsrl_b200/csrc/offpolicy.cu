@@ -10,22 +10,12 @@
 //
 // One call runs `n_steps` complete gradient steps back to back (the loop of
 // OffpolicyTrainer.policy_update_fn, offpolicy.py:102-104) without returning to the host.
-#include "common.cuh"
+#include "arena.cuh"
 #include "fsrl_b200.h"
 
 namespace fsrl {
 
 constexpr int OD_LD = 16;    // row stride of the engine's out / dout scratch
-constexpr float LOG_SQRT_2PI_O = 0.9189385332046727f;
-
-__device__ __forceinline__ void gauss_pair_o(uint32_t a, uint32_t b, float& n0, float& n1) {
-    const double u1 = ((double)a + 1.0) * (1.0 / 4294967296.0);
-    const double u2 = (double)b * (1.0 / 4294967296.0);
-    const double r = sqrt(-2.0 * log(u1));
-    const double ang = 2.0 * 3.141592653589793 * u2;
-    n0 = (float)(r * cos(ang));
-    n1 = (float)(r * sin(ang));
-}
 constexpr uint32_t KEY_UPD = 0x55504454u;   // 'UPDT': noise stream of the update's rsample()
 
 // ---- n-step bookkeeping (base_policy.py:481-493, :552-566) --------------------------------------
@@ -84,8 +74,8 @@ __global__ void sac_sample_kernel(const fsrl_offpolicy_t d, const float* __restr
         if (4 * c < A) {
             uint32_t rr[4];
             Philox::gen((uint32_t)b, (uint32_t)step, (uint32_t)(step >> 32) * 8u + (uint32_t)c, stream_id, d.seed, KEY_UPD, rr);
-            gauss_pair_o(rr[0], rr[1], eps[4 * c], eps[4 * c + 1]);
-            gauss_pair_o(rr[2], rr[3], eps[4 * c + 2], eps[4 * c + 3]);
+            gauss_pair(rr[0], rr[1], eps[4 * c], eps[4 * c + 1]);
+            gauss_pair(rr[2], rr[3], eps[4 * c + 2], eps[4 * c + 3]);
         }
     }
     for (int j = 0; j < A; ++j) {
@@ -95,7 +85,7 @@ __global__ void sac_sample_kernel(const fsrl_offpolicy_t d, const float* __restr
         const float sig = expf(fminf(fmaxf(sraw, d.sigma_min), d.sigma_max));
         const float u = fmaf(sig, eps[j], mu);
         const float a = tanhf(u);
-        lp += -0.5f * eps[j] * eps[j] - logf(sig) - LOG_SQRT_2PI_O - logf(1.0f - a * a + d.tanh_eps);
+        lp += -0.5f * eps[j] * eps[j] - logf(sig) - LOG_SQRT_2PI - logf(1.0f - a * a + d.tanh_eps);
         act[(size_t)b * A + j] = a;
         if (keep) { keep[(size_t)b * 24 + j] = eps[j]; keep[(size_t)b * 24 + 8 + j] = sig; keep[(size_t)b * 24 + 16 + j] = a; }
     }
@@ -257,18 +247,12 @@ __global__ void alpha_step_kernel(const fsrl_offpolicy_t d, const float* __restr
     stat_out[FSRL_OFF_ST_ALPHA_LOSS] = -la * (mean_lp + d.target_entropy);
     float m = st[1], v = st[2];
     const float t = st[3] + 1.0f;
-    m = m + 0.1f * (g - m);
-    v = v * 0.999f + (0.001f * g) * g;
     const float bc1 = 1.0f - powf(0.9f, t), bc2 = 1.0f - powf(0.999f, t);
-    const float denom = sqrtf(v) / sqrtf(bc2) + 1e-8f;
-    const float nla = la + (-(d.alpha_lr / bc1) * m) / denom;
+    const AdamStep ad = {0.1f, 0.999f, 0.001f, sqrtf(bc2), 1e-8f, -(d.alpha_lr / bc1)};   // f32 scalars, as before
+    const float nla = adam_update(la, g, m, v, ad);
     st[0] = nla; st[1] = m; st[2] = v; st[3] = t;
     *d.alpha = expf(nla);
     stat_out[FSRL_OFF_ST_ALPHA] = expf(nla);
-}
-
-static inline long long net_params(const fsrl_netref_t& r) {
-    return (long long)r.D * r.H + r.H + (long long)r.H * r.H + r.H + (long long)r.H * r.out + r.out + r.n_extra;
 }
 
 static inline fsrl_eng_input_t mk_in(const float* xa, const int* ia, int Da, const float* xb, const int* ib, int Db) {
@@ -290,7 +274,11 @@ extern "C" int fsrl_allreduce_fused(void* comm, float* buf, long long n, void* s
 // data parallel: sum the gradient slices of a net list over the ranks (averaged by Adam's grad_scale)
 static int allreduce_grads(const fsrl_offpolicy_t* d, const fsrl_netlist_t* nl, void* stream) {
     long long offs[FSRL_ENG_MAX_NETS], counts[FSRL_ENG_MAX_NETS];
-    for (int i = 0; i < nl->n; ++i) { offs[i] = nl->nets[i].off; counts[i] = net_params(nl->nets[i]); }
+    for (int i = 0; i < nl->n; ++i) {
+        const fsrl_netref_t& r = nl->nets[i];
+        offs[i] = r.off;
+        counts[i] = arena_layout(r.D, r.H, r.out, r.n_extra).size;
+    }
     return fsrl_allreduce_ranges(d->comm, d->eng.grad, offs, counts, nl->n, stream);
 }
 

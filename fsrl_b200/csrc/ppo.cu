@@ -31,20 +31,7 @@ namespace fsrl {
 
 constexpr int ST_ACTOR_REW = 0, ST_ACTOR_SAFETY = 1, ST_KL = 2, ST_VF0 = 3, ST_VF1 = 4,
               ST_ENTROPY = 5, ST_GRADNORM = 6, ST_CLIPFRAC = 7;
-constexpr float LOG_SQRT_2PI_P = 0.9189385332046727f;
 constexpr int DOUT_LD = 16;   // scratch row stride of dOut (cols [A, 2A) carry dlog_sigma)
-
-__device__ long long g_dbg_clock[32];
-__device__ long long g_dbg_cta[512];
-#ifdef FSRL_DEBUG_CLOCKS   // per-phase clock64() stamps of CTA 0 (tools/kbench.py reads them back)
-#define DBG_T(i) do { if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0) g_dbg_clock[i] = clock64(); } while (0)
-#define DBG_W(i) do { if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) g_dbg_clock[i] = clock64(); } while (0)
-#define DBG_CTA(i, v) do { if ((i) < 512) g_dbg_cta[i] = (v); } while (0)
-#else
-#define DBG_T(i) do { } while (0)
-#define DBG_W(i) do { } while (0)
-#define DBG_CTA(i, v) do { (void)(i); } while (0)
-#endif
 
 // Programmatic dependent launch (sm_90+): a kernel launched with the programmatic-serialization
 // attribute may start while its predecessor in the stream is still running; everything it reads
@@ -57,11 +44,7 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 
 __device__ __forceinline__ int slot_mb(const fsrl_ppo_update_t& u, int mb_off) { return mb_off / u.batch_size; }
 
-struct NetView {   // resolved pointers of one network inside the flat buffers
-    Mlp3 m;
-    const float* w2n;      // mirror [out][in] of w2t
-    const float* log_sigma;
-    float *g_w1t, *g_b1, *g_w2t, *g_b2, *g_w3t, *g_b3, *g_log_sigma;
+struct NetView : ArenaNet {   // one network inside the flat buffers (extra = log_sigma), + its scratch
     float *s_h1, *s_h2, *s_dz1, *s_dz2, *s_dout;   // scratch [Bmax][H] / [Bmax][16]
 };
 
@@ -71,32 +54,11 @@ __device__ __forceinline__ NetView net_view(const fsrl_ppo_update_t& u, int n) {
     const int out = (n == 0) ? u.actor_out : 1;
     const float* th = u.theta + u.net_off[n];
     float* g = u.grad + u.net_off[n];
-    size_t o = 0;
-    v.m.w1t = th + o; v.g_w1t = g + o; o += (size_t)D * H;
-    v.m.b1 = th + o;  v.g_b1 = g + o;  o += H;
-    v.m.w2t = th + o; v.g_w2t = g + o; o += (size_t)H * H;
-    v.m.b2 = th + o;  v.g_b2 = g + o;  o += H;
-    v.m.w3t = th + o; v.g_w3t = g + o; o += (size_t)H * out;
-    v.m.b3 = th + o;  v.g_b3 = g + o;  o += out;
-    v.log_sigma = th + o; v.g_log_sigma = g + o;
-    v.m.in = D; v.m.H = H; v.m.out = out;
-    v.w2n = u.w2n + (size_t)n * H * H;
+    arena_net(v, th, g, u.w2n + (size_t)n * H * H, D, H, out);
     float* sc = u.scratch + (size_t)n * u.bmax * (4 * (size_t)H + DOUT_LD);
     v.s_h1 = sc; v.s_h2 = sc + (size_t)u.bmax * H; v.s_dz1 = sc + 2 * (size_t)u.bmax * H;
     v.s_dz2 = sc + 3 * (size_t)u.bmax * H; v.s_dout = sc + 4 * (size_t)u.bmax * H;
     return v;
-}
-
-__device__ __forceinline__ float block_sum_256(float v, float* red) {
-    v = warp_sum(v);
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    __syncthreads();
-    if (lane == 0) red[w] = v;
-    __syncthreads();
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < MLP_TPB / 32; ++i) t += red[i];
-    return t;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -126,22 +88,18 @@ ppo_fwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B) {
     float* xs = smem;                                   // [R][inp]
     float* h1 = xs + (size_t)TT::R * inp;               // [R][LDA]
     float* bs = h1 + (size_t)TT::R * TT::LDA;           // [H][SLAB_LDB]  (aliased by the reduce buffer)
-    DBG_T(16);
     // observations are constant during a repeat: loaded while the previous optimiser step drains
     for (int i = tid; i < TT::R * inp; i += MLP_TPB) {
         const int r = i / inp, k = i % inp;
         xs[i] = (r0 + r < B && k < D) ? u.obs[(size_t)row_of(u, mb_off, r0 + r) * D + k] : 0.f;
     }
-    DBG_T(17);
     pdl_wait();                                         // parameters of the previous step are final
     pdl_trigger();
     // bias of this thread's epilogue columns: requested now, consumed after the GEMM
     const float4 b2v = __ldg(reinterpret_cast<const float4*>(nv.m.b2 + c0 + (tid % (SLAB_NS / 4)) * 4));
-    DBG_T(18);
     if (net == 0 && slab == 0 && blockIdx.x == 0 && tid == 0) *u.norm_sq = 0.f;   // consumed by the previous step's Adam
     slab_load<H>(nv.m.w2t, H, c0, bs);                  // in flight during layer 1
     __syncthreads();
-    DBG_T(19);
     float c[TT::MT][TT::NT][4];
     tc_init_bias<H>(c, nv.m.b1);
     tc_gemm_direct<H>(c, xs, inp, D, nv.m.w1t);
@@ -150,17 +108,14 @@ ppo_fwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B) {
         *reinterpret_cast<float2*>(h1 + (size_t)row * TT::LDA + col) = h;
         if (slab == 0 && r0 + row < u.bmax) *reinterpret_cast<float2*>(nv.s_h1 + (size_t)(r0 + row) * H + col) = h;
     });
-    DBG_T(20);
     __pipeline_wait_prior(0);
     __syncthreads();
-    DBG_T(21);
     slab_gemm<H>(h1, TT::LDA, bs, bs, [&](int row, int c4, float4 v) {
         const float4 b = b2v;                           // c4 == (tid % 16) * 4 for every element this thread visits
         if (r0 + row < u.bmax)
             *reinterpret_cast<float4*>(nv.s_h2 + (size_t)(r0 + row) * H + c0 + c4) =
                 make_float4(fmaxf(v.x + b.x, 0.f), fmaxf(v.y + b.y, 0.f), fmaxf(v.z + b.z, 0.f), fmaxf(v.w + b.w, 0.f));
     });
-    DBG_T(22);
 }
 
 // per-row head dot product  out[j] = sum_k h2[k] * w3s[k][j]  over this lane's k subset, with the
@@ -199,7 +154,6 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
     float* w3s = bs + slab_buf_floats<H>();             // [H][out]
     float* sdout = w3s + (size_t)H * wout;              // [R][DOUT_LD]
     __shared__ float s_mean[2], s_rstd[2], s_b3[MLP_MAX_OUT], s_ls[8];
-    DBG_T(0);
     // everything that does not depend on the forward launch (weights, per-row loss inputs) is
     // requested before pdl_wait(): it overlaps the forward kernel's tail
     slab_load<H>(nv.w2n, H, c0, bs);                    // W2 in [out][in] layout: rows o, columns k-slab
@@ -223,7 +177,6 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
             if (u.value_clip) p_val = u.values[(size_t)(net - 1) * u.ld + id];
         }
     }
-    DBG_T(1);
     // per-minibatch advantage normalisation (ppo_lag.py:178-182): mean / 1/std of this minibatch
     // were computed for every minibatch of the repeat by ppo_adv_stats_kernel
     if (net == 0 && tid < u.C) {
@@ -232,7 +185,7 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
         s_rstd[tid] = ms[1];
     }
     if (tid >= 32 && tid < 32 + wout) s_b3[tid - 32] = __ldg(nv.m.b3 + tid - 32);
-    if (net == 0 && tid >= 64 && tid < 64 + u.A) s_ls[tid - 64] = nv.log_sigma[tid - 64];
+    if (net == 0 && tid >= 64 && tid < 64 + u.A) s_ls[tid - 64] = nv.extra[tid - 64];
     pdl_wait();                                          // h1 / h2 of this minibatch are complete
     pdl_trigger();
     for (int el = tid; el < TT::R * (H / 4); el += MLP_TPB) {
@@ -245,7 +198,6 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
     __pipeline_wait_prior(0);                            // slab (requested long ago) and h2 tile landed
     __syncthreads();
 
-    DBG_T(2);
     // ---- head forward (every slab CTA recomputes it: H x out MACs per row, negligible) -----------
     float out[MLP_MAX_OUT];
 #pragma unroll
@@ -268,7 +220,6 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
         }
     }
 
-    DBG_T(3);
     // ---- loss gradient at the head: one thread per row -----------------------------------------
     float st_a = 0.f, st_b = 0.f, st_c = 0.f, st_d = 0.f;     // per-thread stat partials
     if (part == 0) {
@@ -288,7 +239,7 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
                         dmu[j] = u.bounded ? u.max_action * (1.0f - t * t) : 1.0f;
                         sg[j] = expf(s_ls[j]);
                         zz[j] = (p_act[j] - mu) / sg[j];
-                        logp += -0.5f * zz[j] * zz[j] - s_ls[j] - LOG_SQRT_2PI_P;
+                        logp += -0.5f * zz[j] * zz[j] - s_ls[j] - LOG_SQRT_2PI;
                     }
                 }
                 const float lpo = p_lpo;
@@ -356,7 +307,6 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
                     make_float4(dd[j], dd[j + 1], dd[j + 2], dd[j + 3]);
         }
     }
-    DBG_T(4);
     // minibatch statistics (loss/actor_rew, actor_safety, kl, vf_i): warp-level partial sums and one
     // fire-and-forget reduction per warp -- no block barrier on the critical path
     if (slab == 0) {
@@ -369,7 +319,7 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
             }
             if (blockIdx.x == 0 && tid == 0) {
                 float ent = 0.f;
-                for (int j = 0; j < u.A; ++j) ent += 0.5f + LOG_SQRT_2PI_P + s_ls[j];
+                for (int j = 0; j < u.A; ++j) ent += 0.5f + LOG_SQRT_2PI + s_ls[j];
                 stat[ST_ENTROPY] = ent;
             }
         } else {
@@ -379,7 +329,6 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
     }
     __syncthreads();
 
-    DBG_T(5);
     // ---- backward through layer 3 and ReLU 2 (full width, redundant per slab: H x out per row) ----
     const int nout = (net == 0) ? u.A : 1;       // head columns that feed w3t (mu only)
     for (int e = tid; e < TT::R * (H / 4); e += MLP_TPB) {
@@ -396,10 +345,8 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
         *reinterpret_cast<float4*>(dz + (size_t)row * TT::LDA + k4) = g4;
         if (slab == 0 && r0 + row < u.bmax) *reinterpret_cast<float4*>(nv.s_dz2 + (size_t)(r0 + row) * H + k4) = g4;
     }
-    DBG_T(6);
     __pipeline_wait_prior(0);
     __syncthreads();
-    DBG_T(7);
     // the h2 tile is dead now: its space receives this slab's h1 columns (ReLU-1 mask of the epilogue)
     // while the GEMM runs (slab_gemm waits for outstanding async copies before its first barrier)
     for (int el = tid; el < TT::R * (SLAB_NS / 4); el += MLP_TPB) {
@@ -416,7 +363,6 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
                 make_float4(hv.x > 0.f ? v.x : 0.f, hv.y > 0.f ? v.y : 0.f, hv.z > 0.f ? v.z : 0.f, hv.w > 0.f ? v.w : 0.f);
         }
     });
-    DBG_T(8);
 }
 
 // contiguous copy of the permuted batch (one launch per repeat): minibatch k is then rows
@@ -515,18 +461,6 @@ __device__ __forceinline__ float4 wg_reduced4(const float* red, int m, int n4) {
     return s4;
 }
 
-// Adam hyper-parameters of one optimiser step (torch.optim.Adam scalars, python doubles -> f32)
-struct AdamStep {
-    float w1, b2, w2, bc2s, eps, neg_step;
-};
-
-__device__ __forceinline__ float adam_one(float p, float g, float& m, float& v, const AdamStep& a) {
-    m = m + a.w1 * (g - m);                 // exp_avg.lerp_(grad, 1 - beta1)
-    v = v * a.b2 + (a.w2 * g) * g;          // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
-    const float denom = sqrtf(v) / a.bc2s + a.eps;
-    return p + (a.neg_step * m) / denom;    // param.addcdiv_(exp_avg, denom, value=-step_size)
-}
-
 // Device-wide barrier for co-resident grids (cooperative launch): monotonically increasing ticket
 // counter, one arrival per CTA, spin on an acquire load.
 __device__ __forceinline__ void grid_barrier(unsigned long long* counter, unsigned long long target) {
@@ -599,15 +533,11 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
     pdl_wait();            // dz1 / dz2 / dout of this minibatch are complete
     pdl_trigger();
     float gscale = 1.0f;   // clip coefficient (FUSED)
-    const long long t_start = clock64();
-    (void)t_start;
     auto finish = [&]() {  // norm contribution (+ barrier and clip scale when fused)
-        if (FUSED && tid == 0) { const int c = bx + 40 * net; DBG_CTA(c, clock64() - t_start); }
-        const float tot = block_sum_256(sq, s_red);
+        const float tot = block_sum<WG_TPB / 32>(sq, s_red);
         if (tid == 0 && tot != 0.f && u.world <= 1) atomicAdd(u.norm_sq, tot);   // DP: the norm of the REDUCED gradient is taken later
         if (FUSED) {
             grid_barrier(bar, bar_target);
-            if (tid == 0) { const int c = bx + 40 * net; DBG_CTA(256 + c, clock64() - t_start); }
             const float nsq = __ldcg(u.norm_sq);
             if (u.max_grad_norm > 0.f) gscale = fminf(u.max_grad_norm / (sqrtf(nsq) + 1e-6f), 1.0f);
             if (bx == 0 && net == 0 && tid == 0 && u.stats && slot >= 0)
@@ -615,6 +545,7 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
         }
     };
     const long long pbase = u.net_off[net];
+    const ArenaLayout L = arena_layout(u.D, H, nv.m.out, 0);
     if (bx < NT) {
         // ---- dW2t[k][o] = sum_r h1[r][k] * dz2[r][o] : 32 x 64 tile, 2 x 4 per thread (FFMA issue is the
         // bound on this chip, so the tiles are sized to spread over ~all SMs) ---------------------------
@@ -627,7 +558,6 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
 #pragma unroll
             for (int nt = 0; nt < 8; ++nt) { c[mt][nt][0] = c[mt][nt][1] = c[mt][nt][2] = c[mt][nt][3] = 0.f; }
         float bpart = 0.f;                                  // db2: thread (o = tid % 64, row group tid / 64)
-        DBG_W(10);
         pipeline([&](int ch, int buf) { stage(ch, buf, nv.s_h1, H, k0, WG_TKT, nv.s_dz2, H, o0, WG_T); },
                  [&](int buf) {
                      wg_mma_chunk<2, 8>(sLp(buf), sGp(buf), c);
@@ -637,7 +567,6 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
                          for (int rr = tid / WG_T; rr < WG_RC; rr += WG_TPB / WG_T) bpart += G[(size_t)rr * WG_LD];
                      }
                  });
-        DBG_W(11);
         float* red = smem;                                  // staging is dead: cross-warp reduction buffer
         float* bred = smem + 2 * WG_NST * WG_CHUNK + 80 * WG_T;      // [4][WG_T] bias partials
         wg_store_partial<2, 8>(red, c);
@@ -654,9 +583,7 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
 #pragma unroll
         for (int i = 0; i < 2; ++i) sq += acc[i][0] * acc[i][0] + acc[i][1] * acc[i][1] + acc[i][2] * acc[i][2] + acc[i][3] * acc[i][3];
         if (do_bias && tid < WG_T) sq += bsum * bsum;
-        DBG_W(12);
         finish();
-        DBG_W(13);
         if (!FUSED) {
 #pragma unroll
             for (int i = 0; i < 2; ++i)
@@ -664,7 +591,7 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
                     make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
             if (do_bias && tid < WG_T) nv.g_b2[o0 + tid] = bsum;
         } else {
-            const long long w2s = pbase + (long long)u.D * H + H;
+            const long long w2s = pbase + L.w2;
             float np[2][4];
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
@@ -672,8 +599,8 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
                 float4 p = *reinterpret_cast<float4*>(u.theta + idx);
                 float4 m = *reinterpret_cast<float4*>(u.adam_m + idx);
                 float4 v = *reinterpret_cast<float4*>(u.adam_v + idx);
-                p.x = adam_one(p.x, acc[i][0] * gscale, m.x, v.x, ad); p.y = adam_one(p.y, acc[i][1] * gscale, m.y, v.y, ad);
-                p.z = adam_one(p.z, acc[i][2] * gscale, m.z, v.z, ad); p.w = adam_one(p.w, acc[i][3] * gscale, m.w, v.w, ad);
+                p.x = adam_update(p.x, acc[i][0] * gscale, m.x, v.x, ad); p.y = adam_update(p.y, acc[i][1] * gscale, m.y, v.y, ad);
+                p.z = adam_update(p.z, acc[i][2] * gscale, m.z, v.z, ad); p.w = adam_update(p.w, acc[i][3] * gscale, m.w, v.w, ad);
                 *reinterpret_cast<float4*>(u.theta + idx) = p;
                 *reinterpret_cast<float4*>(u.adam_m + idx) = m;
                 *reinterpret_cast<float4*>(u.adam_v + idx) = v;
@@ -684,9 +611,9 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
             for (int j = 0; j < 4; ++j)
                 *reinterpret_cast<float2*>(mir + (size_t)(o0 + 4 * to + j) * H + k0 + 2 * tk) = make_float2(np[0][j], np[1][j]);
             if (do_bias && tid < WG_T) {
-                const long long idx = w2s + (long long)H * H + o0 + tid;
+                const long long idx = pbase + L.b2 + o0 + tid;
                 float m = u.adam_m[idx], v = u.adam_v[idx];
-                u.theta[idx] = adam_one(u.theta[idx], bsum * gscale, m, v, ad);
+                u.theta[idx] = adam_update(u.theta[idx], bsum * gscale, m, v, ad);
                 u.adam_m[idx] = m; u.adam_v[idx] = v;
             }
         }
@@ -751,9 +678,9 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
             const float g = fin[(size_t)d * WG_T + o];
             if (!FUSED) nv.g_w1t[(size_t)d * H + o0 + o] = g;
             else {
-                const long long idx = pbase + (long long)d * H + o0 + o;
+                const long long idx = pbase + L.w1 + (long long)d * H + o0 + o;
                 float m = u.adam_m[idx], v = u.adam_v[idx];
-                u.theta[idx] = adam_one(u.theta[idx], g * gscale, m, v, ad);
+                u.theta[idx] = adam_update(u.theta[idx], g * gscale, m, v, ad);
                 u.adam_m[idx] = m; u.adam_v[idx] = v;
             }
         }
@@ -761,9 +688,9 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
             const float g = fin[(size_t)D * WG_T + o];
             if (!FUSED) nv.g_b1[o0 + o] = g;
             else {
-                const long long idx = pbase + (long long)D * H + o0 + o;
+                const long long idx = pbase + L.b1 + o0 + o;
                 float m = u.adam_m[idx], v = u.adam_v[idx];
-                u.theta[idx] = adam_one(u.theta[idx], g * gscale, m, v, ad);
+                u.theta[idx] = adam_update(u.theta[idx], g * gscale, m, v, ad);
                 u.adam_m[idx] = m; u.adam_v[idx] = v;
             }
         }
@@ -815,20 +742,19 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
             if (j < out) {
                 if (!FUSED) nv.g_w3t[(size_t)(k0 + k) * out + j] = acc[q];
                 else {
-                    const long long idx = pbase + (long long)u.D * H + H + (long long)H * H + H + (long long)(k0 + k) * out + j;
+                    const long long idx = pbase + L.w3 + (long long)(k0 + k) * out + j;
                     float m = u.adam_m[idx], v = u.adam_v[idx];
-                    u.theta[idx] = adam_one(u.theta[idx], acc[q] * gscale, m, v, ad);
+                    u.theta[idx] = adam_update(u.theta[idx], acc[q] * gscale, m, v, ad);
                     u.adam_m[idx] = m; u.adam_v[idx] = v;
                 }
             }
         }
         if (own_b3 || own_ls) {
-            const long long b3s = pbase + (long long)u.D * H + H + (long long)H * H + H + (long long)H * out;
-            const long long idx = own_b3 ? b3s + tid : b3s + out + (tid - A);
-            if (!FUSED) { if (own_b3) nv.g_b3[tid] = csum; else nv.g_log_sigma[tid - A] = csum; }
+            const long long idx = own_b3 ? pbase + L.b3 + tid : pbase + L.extra + (tid - A);
+            if (!FUSED) { if (own_b3) nv.g_b3[tid] = csum; else nv.g_extra[tid - A] = csum; }
             else {
                 float m = u.adam_m[idx], v = u.adam_v[idx];
-                u.theta[idx] = adam_one(u.theta[idx], csum * gscale, m, v, ad);
+                u.theta[idx] = adam_update(u.theta[idx], csum * gscale, m, v, ad);
                 u.adam_m[idx] = m; u.adam_v[idx] = v;
             }
         }
@@ -840,10 +766,7 @@ __global__ void __launch_bounds__(WG_TPB)
 ppo_wgrad_kernel(const fsrl_ppo_update_t u, int mb_off, int B) {
     extern __shared__ __align__(16) float smem[];
     AdamStep ad = {};
-    const long long t0 = clock64();
-    (void)t0;
     ppo_wgrad_role<H, false>(u, mb_off, B, blockIdx.x, blockIdx.y, smem, ad, nullptr, 0ULL, -1);
-    if (threadIdx.x == 0) DBG_CTA(blockIdx.x + gridDim.x * blockIdx.y, clock64() - t0);
 }
 
 // weight gradients + clip_grad_norm_ + Adam in one launch with a grid barrier (single-GPU path)
@@ -858,18 +781,8 @@ ppo_wgrad_adam_kernel(const fsrl_ppo_update_t u, int mb_off, int B, AdamStep ad,
 // ------------------------------------------------------------------------------------------
 // Phase C: clip_grad_norm_ + Adam (torch.optim.Adam single-tensor arithmetic order)
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ float adam_one_s(float p, float g, float& m, float& v, float w1, float b2,
-                                            float w2, float bc2s, float eps, float neg_step) {
-    m = m + w1 * (g - m);                 // exp_avg.lerp_(grad, 1 - beta1)
-    v = v * b2 + (w2 * g) * g;            // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
-    const float denom = sqrtf(v) / bc2s + eps;
-    return p + (neg_step * m) / denom;    // param.addcdiv_(exp_avg, denom, value=-step_size)
-}
-
 __global__ void __launch_bounds__(256)
-adam_kernel(const fsrl_ppo_update_t u, float w1, float b2, float w2, float bc2s, float eps,
-            float neg_step, int slot, int n_plain_blocks) {
-    __shared__ float tile[32][33];
+adam_kernel(const fsrl_ppo_update_t u, const AdamStep ad, int slot, int n_plain_blocks) {
     __shared__ float nred[8];
     pdl_wait();                        // gradients / norm partials of this step are complete
     pdl_trigger();
@@ -880,7 +793,7 @@ adam_kernel(const fsrl_ppo_update_t u, float w1, float b2, float w2, float bc2s,
         const int nblk = (int)((u.n_params + 1023) / 1024);
         float sp = 0.f;
         for (int i = threadIdx.x; i < nblk; i += 256) sp += __ldcg(u.p2p_part + i);
-        nsq_raw = block_sum_256(sp, nred);
+        nsq_raw = block_sum<8>(sp, nred);
     } else {
         nsq_raw = *u.norm_sq;
     }
@@ -898,47 +811,37 @@ adam_kernel(const fsrl_ppo_update_t u, float w1, float b2, float w2, float bc2s,
         long long cc = (long long)blockIdx.x * 256 + threadIdx.x;
         long long i = -1;
         for (int n = 0; n < u.n_nets; ++n) {
+            const ArenaLayout L = arena_layout(u.D, H, (n == 0) ? u.actor_out : 1, 0);
             const long long size = ((n + 1 < u.n_nets) ? u.net_off[n + 1] : u.n_params) - u.net_off[n];
-            const long long pre = (long long)u.D * H + H, post = size - pre - (long long)H * H;
+            const long long pre = L.w2, post = size - L.b2;
             if (cc < pre) { i = u.net_off[n] + cc; break; }
             cc -= pre;
-            if (cc < post) { i = u.net_off[n] + pre + (long long)H * H + cc; break; }
+            if (cc < post) { i = u.net_off[n] + L.b2 + cc; break; }
             cc -= post;
         }
         if (i < 0) return;
         float m = u.adam_m[i], v = u.adam_v[i];
         const float g = (u.mask && u.mask[i] == 0) ? 0.f : u.grad[i] * scale;
         if (u.mask && u.mask[i] == 0) return;
-        u.theta[i] = adam_one_s(u.theta[i], g, m, v, w1, b2, w2, bc2s, eps, neg_step);
+        u.theta[i] = adam_update(u.theta[i], g, m, v, ad);
         u.adam_m[i] = m; u.adam_v[i] = v;
     } else {
         // W2 tiles: 32 x 32, update canonical W2t[k][o] and its mirror W2n[o][k]
         const int tpn = (H / 32) * (H / 32);
         const int t = blockIdx.x - n_plain_blocks;
         const int n = t / tpn, tt = t % tpn;
-        const int k0 = (tt / (H / 32)) * 32, o0 = (tt % (H / 32)) * 32;
-        const long long base = u.net_off[n] + (long long)u.D * H + H;
-        const int lx = threadIdx.x % 32, ly = threadIdx.x / 32;
+        const long long base = u.net_off[n] + arena_layout(u.D, H, (n == 0) ? u.actor_out : 1, 0).w2;
         const bool frozen = u.mask && u.mask[base] == 0;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const int kk = ly + 8 * q;
-            const long long i = base + (long long)(k0 + kk) * H + o0 + lx;
+        w2_tile(u.w2n + (size_t)n * H * H, H, (tt / (H / 32)) * 32, (tt % (H / 32)) * 32, [&](int k, int o) {
+            const long long i = base + (long long)k * H + o;
             float p = u.theta[i];
             if (!frozen) {
                 float m = u.adam_m[i], v = u.adam_v[i];
-                p = adam_one_s(p, u.grad[i] * scale, m, v, w1, b2, w2, bc2s, eps, neg_step);
+                p = adam_update(p, u.grad[i] * scale, m, v, ad);
                 u.theta[i] = p; u.adam_m[i] = m; u.adam_v[i] = v;
             }
-            tile[kk][lx] = p;
-        }
-        __syncthreads();
-        float* mir = u.w2n + (size_t)n * H * H;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const int oo = ly + 8 * q;
-            mir[(size_t)(o0 + oo) * H + k0 + lx] = tile[lx][oo];
-        }
+            return p;
+        });
     }
 }
 
@@ -998,7 +901,7 @@ __global__ void __launch_bounds__(256) ppo_dp_reduce_kernel(const fsrl_ppo_updat
             for (int q = 0; q < 4 && i4 + q < u.n_params; ++q) { u.grad[i4 + q] = a[q]; sq += a[q] * a[q]; }
         }
     }
-    const float tot = block_sum_256(sq, red);
+    const float tot = block_sum<8>(sq, red);
     if (tid == 0) u.p2p_part[blockIdx.x] = tot;     // no atomics: the Adam kernel sums these in a fixed order
 }
 
@@ -1007,10 +910,8 @@ __global__ void __launch_bounds__(1024) grad_norm_kernel(const fsrl_ppo_update_t
     __shared__ float red[32];
     float s = 0.f;
     for (long long i = threadIdx.x; i < u.n_params; i += 1024) { const float g = u.grad[i]; s += g * g; }
-    s = warp_sum(s);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) { float t = 0.f; for (int w = 0; w < 32; ++w) t += red[w]; *u.norm_sq = t; }
+    s = block_sum<32>(s, red);
+    if (threadIdx.x == 0) *u.norm_sq = s;
 }
 
 // per-minibatch sum and sum of squares of the advantages (block b = minibatch b of the repeat)
@@ -1026,13 +927,8 @@ __global__ void __launch_bounds__(256) ppo_adv_moments_kernel(const fsrl_ppo_upd
             const double a = (double)u.adv[(size_t)c * u.ld + (u.perm ? (long long)u.perm[off + i] : off + i)];
             s += a; q += a * a;
         }
-        s = warp_sum(s); q = warp_sum(q);
-        __syncthreads();
-        if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = s; red[1][threadIdx.x >> 5] = q; }
-        __syncthreads();
+        const double ts = block_sum<8>(s, red[0]), tq = block_sum<8>(q, red[1]);
         if (threadIdx.x == 0) {
-            double ts = 0.0, tq = 0.0;
-            for (int w = 0; w < 8; ++w) { ts += red[0][w]; tq += red[1][w]; }
             u.moments_w[((size_t)mb * 2 + c) * 2] = ts;
             u.moments_w[((size_t)mb * 2 + c) * 2 + 1] = tq;
         }
@@ -1043,7 +939,6 @@ __global__ void __launch_bounds__(256) ppo_adv_moments_kernel(const fsrl_ppo_upd
 // the repeat: block b = minibatch b.  In a data-parallel run the sums were all-reduced first.
 __global__ void __launch_bounds__(256) ppo_adv_stats_kernel(const fsrl_ppo_update_t u, long long n_total, int n_mb) {
     __shared__ double red[8];
-    __shared__ double s_m;
     const int mb = blockIdx.x;
     const long long off = (long long)mb * u.batch_size;
     long long B = u.batch_size;
@@ -1065,26 +960,14 @@ __global__ void __launch_bounds__(256) ppo_adv_stats_kernel(const fsrl_ppo_updat
         double sacc = 0.0;
         for (long long i = threadIdx.x; i < B; i += 256)
             sacc += (double)u.adv[(size_t)c * u.ld + (u.perm ? (long long)u.perm[off + i] : off + i)];
-        sacc = warp_sum(sacc);
-        __syncthreads();
-        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sacc;
-        __syncthreads();
-        if (threadIdx.x == 0) { double t = 0.0; for (int w = 0; w < 8; ++w) t += red[w]; s_m = t / (double)B; }
-        __syncthreads();
-        const float mean = (float)s_m;
+        const float mean = (float)(block_sum<8>(sacc, red) / (double)B);
         double q = 0.0;
         for (long long i = threadIdx.x; i < B; i += 256) {
             const float d = u.adv[(size_t)c * u.ld + (u.perm ? (long long)u.perm[off + i] : off + i)] - mean;
             q += (double)(d * d);
         }
-        q = warp_sum(q);
-        __syncthreads();
-        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = q;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            double t = 0.0; for (int w = 0; w < 8; ++w) t += red[w];
-            out[0] = mean; out[1] = 1.0f / sqrtf((float)(t / (double)(B - 1)));
-        }
+        q = block_sum<8>(q, red);
+        if (threadIdx.x == 0) { out[0] = mean; out[1] = 1.0f / sqrtf((float)(q / (double)(B - 1))); }
     }
 }
 
@@ -1146,14 +1029,9 @@ static int ppo_launch_minibatch(const fsrl_ppo_update_t& u, int mb_off, int B, i
         fuse_ok = (per_sm * sm_count() >= (int)(gB.x * 3)) ? 1 : 0;     // whole grid co-resident?
         attr_w = true;
     }
-    // torch.optim.Adam scalars (python doubles -> f32 at the op)
-    const double b1 = u.beta1, b2 = u.beta2;
-    const double bc1 = 1.0 - pow(b1, (double)adam_t), bc2 = 1.0 - pow(b2, (double)adam_t);
-    const float neg_step = (float)(-(u.lr / bc1));
-    const float bc2s = (float)sqrt(bc2);
+    const AdamStep ad = adam_step_scalars(u.lr, u.beta1, u.beta2, u.adam_eps, adam_t);
     if (u.world <= 1 && fuse_ok == 1 && u.barrier != nullptr && u.mask == nullptr) {
         // single GPU: gradients never leave the registers -- tiles -> norm -> barrier -> clip + Adam
-        AdamStep ad = {(float)(1.0 - b1), (float)b2, (float)(1.0 - b2), bc2s, (float)u.adam_eps, neg_step};
         unsigned long long target = (unsigned long long)(bar_count + 1) * gB.x * gB.y;
         // Ordinary (not cooperative) launch: no cooperative-launch overhead per step.  The grid barrier is still
         // safe: fuse_ok guarantees grid <= SMs x CTAs/SM, every CTA of the grid becomes resident without
@@ -1185,24 +1063,18 @@ static int ppo_launch_minibatch(const fsrl_ppo_update_t& u, int mb_off, int B, i
     }
     const int n_plain = adam_plain_blocks(u, H);
     const int n_tiles = u.n_nets * (H / 32) * (H / 32);
-    FSRL_CUDA(launch_chain(adam_kernel, dim3(n_plain + n_tiles), dim3(256), (size_t)0, s, false, u, (float)(1.0 - b1),
-                           (float)b2, (float)(1.0 - b2), bc2s, (float)u.adam_eps, neg_step, slot, n_plain));
+    FSRL_CUDA(launch_chain(adam_kernel, dim3(n_plain + n_tiles), dim3(256), (size_t)0, s, false, u, ad, slot, n_plain));
     return FSRL_OK;
 }
 
-__global__ void mirror_w2_kernel(const fsrl_ppo_update_t u) {
-    // w2n[n][o][k] = w2t[n][k][o]  (initial sync of the mirror, 32x32 tiles)
-    __shared__ float tile[32][33];
-    const int H = u.H;
-    const int tpn = (H / 32) * (H / 32);
-    const int n = blockIdx.x / tpn, tt = blockIdx.x % tpn;
-    const int k0 = (tt / (H / 32)) * 32, o0 = (tt % (H / 32)) * 32;
-    const float* src = u.theta + u.net_off[n] + (long long)u.D * H + H;
-    const int lx = threadIdx.x % 32, ly = threadIdx.x / 32;
-    for (int q = 0; q < 4; ++q) tile[ly + 8 * q][lx] = src[(size_t)(k0 + ly + 8 * q) * H + o0 + lx];
-    __syncthreads();
-    float* mir = u.w2n + (size_t)n * H * H;
-    for (int q = 0; q < 4; ++q) mir[(size_t)(o0 + ly + 8 * q) * H + k0 + lx] = tile[lx][ly + 8 * q];
+// w2n[n] = w2t[n]^T for every network of the descriptor
+static int ppo_sync_mirror(const fsrl_ppo_update_t& u, cudaStream_t s) {
+    W2Mirror mr;
+    for (int n = 0; n < u.n_nets; ++n) {
+        mr.w2t[n] = u.theta + u.net_off[n] + arena_layout(u.D, u.H, (n == 0) ? u.actor_out : 1, 0).w2;
+        mr.w2n[n] = u.w2n + (size_t)n * u.H * u.H;
+    }
+    return launch_w2_mirror(mr, u.n_nets, u.H, s);
 }
 
 }  // namespace fsrl
@@ -1240,10 +1112,7 @@ extern "C" int fsrl_ppo_persist_active(const fsrl_ppo_update_t* u, long long n_t
 extern "C" int fsrl_ppo_sync_mirror(const fsrl_ppo_update_t* u, void* stream) {
     int rc = check_update(u);
     if (rc) return rc;
-    const int H = u->H;
-    mirror_w2_kernel<<<u->n_nets * (H / 32) * (H / 32), 256, 0, static_cast<cudaStream_t>(stream)>>>(*u);
-    FSRL_LAUNCH_CHECK();
-    return FSRL_OK;
+    return ppo_sync_mirror(*u, static_cast<cudaStream_t>(stream));
 }
 
 // One repeat of PPOLagrangian.learn's inner loop (ppo_lag.py:223-247): every minibatch of
@@ -1303,8 +1172,8 @@ extern "C" int fsrl_ppo_lag_epoch(const fsrl_ppo_update_t* u, long long n_total,
         const int n_mb = (int)(n_total / batch_size);
         int rcp = ppo_persist_run(*u, n_mb, stats_slot0, adam_t0, s);
         if (rcp) return rcp;
-        mirror_w2_kernel<<<u->n_nets * (u->H / 32) * (u->H / 32), 256, 0, s>>>(*u);
-        FSRL_LAUNCH_CHECK();
+        rcp = ppo_sync_mirror(*u, s);
+        if (rcp) return rcp;
         if (n_minibatches) *n_minibatches = n_mb;
         return FSRL_OK;
     }
@@ -1326,68 +1195,5 @@ extern "C" int fsrl_ppo_lag_epoch(const fsrl_ppo_update_t* u, long long n_total,
         if (last) break;
     }
     if (n_minibatches) *n_minibatches = count;
-    return FSRL_OK;
-}
-
-// Measurement aid for bench.py's roofline object: average duration of each phase kernel over
-// `iters` back-to-back launches on one minibatch of u->perm (CUDA events on `stream`).  The
-// Adam phase is launched with lr = 0 so that the weights are not disturbed.
-template <int H>
-static int ppo_time_phases(const fsrl_ppo_update_t& u0, int B, int iters, float* ms, cudaStream_t s) {
-    using TT = MlpTile<H>;
-    fsrl_ppo_update_t u = u0;
-    const size_t smemF = sizeof(float) * ((size_t)TT::R * TT::in_pad(u.D) + (size_t)TT::R * TT::LDA + slab_buf_floats<H>());
-    const size_t smemB = sizeof(float) * (2 * (size_t)TT::R * TT::LDA + slab_buf_floats<H>() + (size_t)H * (u.actor_out > 1 ? u.actor_out : 1) + (size_t)TT::R * DOUT_LD);
-    FSRL_CUDA(cudaFuncSetAttribute(ppo_fwd_kernel<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemF));
-    FSRL_CUDA(cudaFuncSetAttribute(ppo_bwd_kernel<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemB));
-    cudaEvent_t e[5];
-    for (int i = 0; i < 5; ++i) FSRL_CUDA(cudaEventCreate(&e[i]));
-    const dim3 gA((B + TT::R - 1) / TT::R, H / SLAB_NS, u.n_nets);
-    constexpr int NTT = H / WG_T;
-    const dim3 gB((H / WG_TKT) * NTT + 2 * NTT, u.n_nets);
-    const size_t smemW = sizeof(float) * WG_SMEM_FLOATS;
-    FSRL_CUDA(cudaFuncSetAttribute(ppo_wgrad_kernel<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemW));
-    const int n_plain = adam_plain_blocks(u, H);
-    const int n_tiles = u.n_nets * (H / 32) * (H / 32);
-    FSRL_CUDA(cudaEventRecord(e[0], s));
-    for (int i = 0; i < iters; ++i) ppo_fwd_kernel<H><<<gA, MLP_TPB, smemF, s>>>(u, 0, B);
-    FSRL_CUDA(cudaEventRecord(e[1], s));
-    for (int i = 0; i < iters; ++i) ppo_bwd_kernel<H><<<gA, MLP_TPB, smemB, s>>>(u, 0, B, 0);
-    FSRL_CUDA(cudaEventRecord(e[2], s));
-    for (int i = 0; i < iters; ++i) ppo_wgrad_kernel<H><<<gB, WG_TPB, smemW, s>>>(u, 0, B);
-    FSRL_CUDA(cudaEventRecord(e[3], s));
-    for (int i = 0; i < iters; ++i)
-        adam_kernel<<<n_plain + n_tiles, 256, 0, s>>>(u, 0.1f, 0.999f, 0.001f, 1.0f, 1e-8f, 0.0f, -1, n_plain);
-    FSRL_CUDA(cudaEventRecord(e[4], s));
-    FSRL_CUDA(cudaEventSynchronize(e[4]));
-    for (int i = 0; i < 4; ++i) {
-        float t = 0.f;
-        FSRL_CUDA(cudaEventElapsedTime(&t, e[i], e[i + 1]));
-        ms[i] = t / (float)iters;
-    }
-    for (int i = 0; i < 5; ++i) cudaEventDestroy(e[i]);
-    FSRL_LAUNCH_CHECK();
-    return FSRL_OK;
-}
-
-extern "C" int fsrl_ppo_phase_times(const fsrl_ppo_update_t* u, int B, int iters, float* ms_out, void* stream) {
-    int rc = check_update(u);
-    if (rc) return rc;
-    FSRL_REQUIRE(ms_out && iters > 0 && B > 1 && B <= u->bmax, "fsrl_ppo_phase_times: bad arguments");
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    switch (u->H) {
-        case 64: return ppo_time_phases<64>(*u, B, iters, ms_out, s);
-        case 128: return ppo_time_phases<128>(*u, B, iters, ms_out, s);
-        case 256: return ppo_time_phases<256>(*u, B, iters, ms_out, s);
-        default: return ppo_time_phases<512>(*u, B, iters, ms_out, s);
-    }
-}
-
-extern "C" int fsrl_debug_clocks(long long* out32) {
-    FSRL_CUDA(cudaMemcpyFromSymbol(out32, fsrl::g_dbg_clock, sizeof(long long) * 32));
-    return FSRL_OK;
-}
-extern "C" int fsrl_debug_cta_cycles(long long* out512) {
-    FSRL_CUDA(cudaMemcpyFromSymbol(out512, fsrl::g_dbg_cta, sizeof(long long) * 512));
     return FSRL_OK;
 }

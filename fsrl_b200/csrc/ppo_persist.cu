@@ -35,6 +35,7 @@
 // accumulate in their own registers.  With world > 1 the <DP = true> instantiation exchanges gradients itself over peer
 // memory (dp_* functions below: tagged + hashed 16-byte packets pushed into the peers' buffers).
 #include "ppo_persist.cuh"
+#include "arena.cuh"
 #include "wgmma.cuh"
 #include <cstdlib>
 #include <cmath>
@@ -94,7 +95,6 @@ constexpr int MAX_MB = 16384;                                    // minibatches 
 constexpr long long WAIT_CYCLES = 6000000000LL;                  // ~3 s: a lost partner must not hang the GPU
 
 constexpr int ST_ACTOR_REW = 0, ST_ACTOR_SAFETY = 1, ST_KL = 2, ST_VF0 = 3, ST_ENTROPY = 5, ST_GRADNORM = 6;
-constexpr float LOG_SQRT_2PI = 0.9189385332046727f;
 
 struct Args {
     fsrl_ppo_update_t u;     // batch pointers already gathered (contiguous rows, u.perm == nullptr)
@@ -564,8 +564,9 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
 
     // parameter offsets of this network inside the flat arena
     const long long pbase = u.net_off[net];
-    const long long o_w1 = pbase, o_b1 = o_w1 + (long long)D * H, o_w2 = o_b1 + H, o_b2 = o_w2 + (long long)H * H,
-                    o_w3 = o_b2 + H, o_b3 = o_w3 + (long long)H * out, o_ls = o_b3 + out;
+    const ArenaLayout L = arena_layout(D, H, out, 0);
+    const long long o_w1 = pbase + L.w1, o_b1 = pbase + L.b1, o_w2 = pbase + L.w2, o_b2 = pbase + L.b2,
+                    o_w3 = pbase + L.w3, o_b3 = pbase + L.b3, o_ls = pbase + L.extra;
 
     if (warp == NEPI / 32) {
         // ============================ bulk-copy producer ==========================================

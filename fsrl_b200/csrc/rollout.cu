@@ -17,18 +17,6 @@ namespace fsrl {
 
 static_assert(sizeof(fsrl_mlp3_t) == sizeof(Mlp3), "ABI struct mismatch");
 
-__device__ __forceinline__ void gauss_pair(uint32_t a, uint32_t b, float& n0, float& n1) {
-    // Box-Muller in f64 (oracle/philox.py normal_pair)
-    const double u1 = ((double)a + 1.0) * (1.0 / 4294967296.0);
-    const double u2 = (double)b * (1.0 / 4294967296.0);
-    const double r = sqrt(-2.0 * log(u1));
-    const double ang = 2.0 * 3.141592653589793 * u2;
-    n0 = (float)(r * cos(ang));
-    n1 = (float)(r * sin(ang));
-}
-
-constexpr float LOG_SQRT_2PI = 0.9189385332046727f;
-
 template <int KIND, int H>
 __global__ void __launch_bounds__(MLP_TPB)
 rollout_step_kernel(const fsrl_rollout_t a) {

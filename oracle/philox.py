@@ -39,7 +39,7 @@ def usym(x):
 
 
 def normal_pair(xa, xb):
-    """Box-Muller in f64 from two u32 words (rollout.cu gauss_pair): u1 = (a+1)*2^-32 in
+    """Box-Muller in f64 from two u32 words (common.cuh gauss_pair): u1 = (a+1)*2^-32 in
     (0,1], u2 = b*2^-32; returns two f32 normals."""
     u1 = (xa.astype(np.float64) + 1.0) * (1.0 / 4294967296.0)
     u2 = xb.astype(np.float64) * (1.0 / 4294967296.0)
