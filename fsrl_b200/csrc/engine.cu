@@ -488,13 +488,27 @@ __global__ void eng_zero_grad_kernel(const fsrl_engine_t e, const fsrl_netlist_t
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) g[i] = 0.f;
 }
 
+// *norm_sq += sum of squares of the listed nets' gradient ranges (one CTA per net).  With split rows
+// the gradient is complete only after every split has added its partial tiles, so the norm of the
+// final gradient needs this pass of its own.
+__global__ void __launch_bounds__(1024) eng_grad_sumsq_kernel(const fsrl_engine_t e, const fsrl_netlist_t nl,
+                                                              const float* dst_override, float* norm_sq) {
+    __shared__ float red[32];
+    const fsrl_netref_t nr = nl.nets[blockIdx.y];
+    const long long n = arena_layout(nr.D, nr.H, nr.out, nr.n_extra).size;
+    const float* g = dst_override ? dst_override : e.grad + nr.off;
+    float s = 0.f;
+    for (long long i = threadIdx.x; i < n; i += 1024) s += g[i] * g[i];
+    s = block_sum<32>(s, red);
+    if (threadIdx.x == 0) atomicAdd(norm_sq, s);
+}
+
 int eng_wgrad_roles(const fsrl_engine_t* e, const fsrl_netlist_t* nl, const fsrl_eng_input_t* in, long long B,
                     int accumulate, float* norm_sq, const WgradRoles& roles, cudaStream_t s) {
     // split the rows so that every CTA streams <= 4096 rows (keeps all SMs busy on big batches)
     int nsplit = (int)((B + 4095) / 4096);
     if (nsplit < 1) nsplit = 1;
     if (nsplit > 65535) nsplit = 65535;
-    if (nsplit > 1) FSRL_REQUIRE(norm_sq == nullptr, "engine_wgrad: norm_sq is not available with split rows");
     const bool partial = roles.parts != 7 || !roles.bias2 || !roles.bias3;
     if (!accumulate && (nsplit > 1 || partial)) {
         // start from zero and let every part accumulate (atomically when the rows are split)
@@ -505,9 +519,14 @@ int eng_wgrad_roles(const fsrl_engine_t* e, const fsrl_netlist_t* nl, const fsrl
     }
     ENG_DISPATCH_H(nl->nets[0].H, {
         const dim3 g((HH / EWG_TK) * (HH / EWG_TO) + 2 * (HH / EWG_TO), nl->n, nsplit);
-        eng_wgrad_kernel<HH><<<g, EWG_TPB, 0, s>>>(*e, *nl, *in, (int)B, accumulate, norm_sq, roles);
+        eng_wgrad_kernel<HH><<<g, EWG_TPB, 0, s>>>(*e, *nl, *in, (int)B, accumulate, nsplit > 1 ? nullptr : norm_sq, roles);
     });
     FSRL_LAUNCH_CHECK();
+    if (nsplit > 1 && norm_sq) {
+        eng_grad_sumsq_kernel<<<dim3(1, nl->n), 1024, 0, s>>>(*e, *nl, roles.dst, norm_sq);
+        ++g_launches;
+        FSRL_LAUNCH_CHECK();
+    }
     return FSRL_OK;
 }
 }  // namespace fsrl
@@ -548,7 +567,8 @@ extern "C" int fsrl_engine_polyak(const fsrl_engine_t* e, const fsrl_netlist_t* 
     const int H = dst->nets[0].H;
     for (int i = 0; i < dst->n; ++i) {
         const fsrl_netref_t& n = dst->nets[i];
-        FSRL_REQUIRE(n.D == src->nets[i].D && n.H == src->nets[i].H && n.out == src->nets[i].out, "polyak: shape mismatch");
+        FSRL_REQUIRE(n.D == src->nets[i].D && n.H == src->nets[i].H && n.out == src->nets[i].out &&
+                         n.n_extra == src->nets[i].n_extra, "polyak: shape mismatch");
     }
     const int blocks = (int)((max_net_size(dst) + 255) / 256) + (H / 32) * (H / 32);
     eng_polyak_kernel<<<dim3(blocks, dst->n), 256, 0, static_cast<cudaStream_t>(stream)>>>(*e, *dst, *src, (float)tau);

@@ -258,6 +258,8 @@ size_t fsrl_engine_slot_floats(int H, int bmax);
 int fsrl_engine_forward(const fsrl_engine_t* e, const fsrl_netlist_t* nets, const fsrl_eng_input_t* in,
                         int B, int save, void* stream);
 int fsrl_engine_backward(const fsrl_engine_t* e, const fsrl_netlist_t* nets, int B, int want_dx, void* stream);
+/* grad (+)= the weight gradients of B rows; when norm_sq != NULL, *norm_sq += the squared norm of the
+ * listed nets' final gradients (above 4096 rows the rows are split and a separate pass sums it) */
 int fsrl_engine_wgrad(const fsrl_engine_t* e, const fsrl_netlist_t* nets, const fsrl_eng_input_t* in, int B,
                       int accumulate, float* norm_sq, void* stream);
 /* torch.optim.Adam step `step` (1-based) on the listed nets; grad <- grad*grad_scale + 2*l2_reg*p

@@ -47,6 +47,46 @@ def oracle_nets(policy, hidden):
     return actor, critics
 
 
+def adam64(p, g, m, v, t, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
+    """One torch.optim.Adam step (single-tensor form) in float64; returns (p, m, v)."""
+    b1, b2 = betas
+    p, g, m, v = (torch.as_tensor(a, dtype=torch.float64) for a in (p, g, m, v))
+    g = g + weight_decay * p
+    m = m + (1.0 - b1) * (g - m)
+    v = v * b2 + (1.0 - b2) * g * g
+    denom = v.sqrt() / np.sqrt(1.0 - b2 ** t) + eps
+    return p - (lr / (1.0 - b1 ** t)) * m / denom, m, v
+
+
+def cg64(mvp, b, nsteps=10, tol=1e-8):
+    """Conjugate gradients in float64 with the trust-region learners' early exit (stop once
+    r.r < tol, after x and r have been updated).  Returns x and r.r after every iteration run."""
+    b = torch.as_tensor(b, dtype=torch.float64)
+    x, r, p = torch.zeros_like(b), b.clone(), b.clone()
+    rs_old = float(r @ r)
+    res = []
+    for _ in range(nsteps):
+        z = mvp(p)
+        alpha = rs_old / float(p @ z)
+        x = x + alpha * p
+        r = r - alpha * z
+        rs_new = float(r @ r)
+        res.append(rs_new)
+        if rs_new < tol:
+            break
+        p = r + (rs_new / rs_old) * p
+        rs_old = rs_new
+    return x, res
+
+
+def cg_stop_tol(res, lo=2, hi=7):
+    """A residual_tol that stops cg64 right after iteration k (0-based) of a run whose r.r were
+    `res`: the geometric mean of min(res[:k]) and res[k], for the k in [lo, hi) with the widest
+    gap between the two.  Returns (k, tol)."""
+    k = max(range(lo, min(hi, len(res))), key=lambda j: min(res[:j]) / res[j])
+    return k, (min(res[:k]) * res[k]) ** 0.5
+
+
 def buffer_to_numpy(buf):
     g = lambda t: t.detach().cpu().numpy()
     return dict(obs=g(buf.obs), obs_next=g(buf.obs_next), act=g(buf.act), rew=g(buf.rew),

@@ -12,15 +12,15 @@ from helpers import buffer_to_numpy
 pytestmark = pytest.mark.gpu
 
 
-def _setup(hidden=(64, 64), task="SafetyCarCircle-v0", **kw):
+def _setup(hidden=(64, 64), task="SafetyCarCircle-v0", n_env=4, **kw):
     from fsrl_b200 import envs
     from fsrl_b200.agent import FOCOPSAgent
     from fsrl_b200.data import FastCollector, VectorReplayBuffer
     env = envs.make(task)
     agent = FOCOPSAgent(env, seed=10, hidden_sizes=hidden, **kw)
     policy = agent.policy
-    venv = envs.DeviceVectorEnv(task, 4, seed=12)
-    buf = VectorReplayBuffer(4 * env.spec.max_episode_steps, 4)
+    venv = envs.DeviceVectorEnv(task, n_env, seed=12)
+    buf = VectorReplayBuffer(n_env * env.spec.max_episode_steps, n_env)
     col = FastCollector(policy, venv, buf, exploration_noise=True)
     return policy, venv, buf, col
 
@@ -39,12 +39,17 @@ def test_nu_update_matches_reference_arithmetic():
         assert got == pytest.approx(want, abs=1e-7)
 
 
-@pytest.mark.parametrize("eta", [0.02, 1e-4])
-def test_focops_learn_matches_oracle(eta):
+@pytest.mark.parametrize("eta,hidden,n_env,batch_size", [
+    pytest.param(0.02, (64, 64), 4, 256, id="0.02"),
+    pytest.param(1e-4, (64, 64), 4, 256, id="0.0001"),
+    # one minibatch of ~4800 rows (merge_last): the actor's wgrad splits the rows and the default
+    # max_grad_norm clips with the norm of the combined gradient
+    pytest.param(0.02, (128, 128), 16, 99999, id="h128-16env-whole-batch"),
+])
+def test_focops_learn_matches_oracle(eta, hidden, n_env, batch_size):
     from oracle import focops as ofoc, nets as onets
-    hidden = (64, 64)
-    policy, venv, buf, col = _setup(hidden, eta=eta, delta=1e9)
-    stats = col.collect(n_episode=4)
+    policy, venv, buf, col = _setup(hidden, n_env=n_env, eta=eta, delta=1e9)
+    stats = col.collect(n_episode=n_env)
     policy.pre_update_fn(stats_train=stats)
     sd = policy.state_dict()
     D, A = venv.D, venv.A
@@ -64,12 +69,15 @@ def test_focops_learn_matches_oracle(eta):
     aopt = torch.optim.Adam(actor.parameters(), lr=5e-4)
     copt = torch.optim.Adam([p for c in critics for p in c.parameters()], lr=1e-3)
     nu, _ = ofoc.nu_step(0.0, 1e-2, 2.0, 10.0, stats["cost"])
+    whole = batch_size >= batch.n
+    if whole:
+        assert batch.n > 4096 and policy._grad_norm == 0.5
     np.random.seed(4)
-    ostats = ofoc.learn(actor, critics, aopt, copt, ob, 256, 2, nu, eta=eta, delta=1e9)
+    ostats = ofoc.learn(actor, critics, aopt, copt, ob, batch_size, 2, nu, eta=eta, delta=1e9)
     np.random.seed(4)
-    policy.learn(batch, batch_size=256, repeat=2)
+    policy.learn(batch, batch_size=batch_size, repeat=2)
     st = policy.last_stats
-    assert len(st["loss/kl"]) == len(ostats) >= 8
+    assert len(st["loss/kl"]) == len(ostats) >= (2 if whole else 8)
     assert st["loss/nu_value"][0] == pytest.approx(nu, abs=1e-7)
     for key in ("loss/actor_loss", "loss/kl", "loss/entropy", "loss/vf0", "loss/vf1", "loss/vf_total"):
         want = np.array([s[key] for s in ostats]); got = np.array(st[key])
