@@ -9,7 +9,7 @@ import numpy as np
 import torch
 
 from .envs import OracleVecEnv
-from .philox import action_noise, philox4x32, usym, KEY_ACT
+from .philox import action_noise, action_uniform
 
 LOG_SQRT_2PI = np.float32(0.9189385332046727)
 
@@ -72,9 +72,12 @@ def collect(env: OracleVecEnv, actor, n_episode, seed_act, act_ctr, buffer=None,
         n = len(ready)
         with torch.no_grad():
             if mode == "random":
-                r = philox4x32(ready.astype(np.uint32), act_ctr[ready], 0, 0, seed_act, KEY_ACT)
-                eps = np.stack([usym(r[j]) for j in range(env.A)], 1) if env.A <= 4 else None
-                act = eps.astype(np.float32); logp = np.zeros(n, np.float32)
+                # action_space.sample() + map_action_inverse (fast_collector.py:258-264)
+                act = action_uniform(seed_act, ready, act_ctr[ready], env.A)
+                if action_bound == "tanh":
+                    with np.errstate(divide="ignore"):
+                        act = (np.float32(0.5) * (np.log1p(act) - np.log1p(-act))).astype(np.float32)
+                logp = np.zeros(n, np.float32)
                 act_ctr[ready] += np.uint32(1)
             else:
                 out = actor(torch.from_numpy(obs))

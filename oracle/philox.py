@@ -48,6 +48,19 @@ def normal_pair(xa, xb):
     return (r * np.cos(ang)).astype(np.float32), (r * np.sin(ang)).astype(np.float32)
 
 
+def action_uniform(seed, env_ids, act_ctr, A):
+    """u[e, a] in [-1, 1) of a random-mode action with per-env counter act_ctr[e] (rollout.cu):
+    actions 4c .. 4c + 3 come from the draw with counter word 2 = c"""
+    env_ids = np.asarray(env_ids, dtype=np.uint32)
+    act_ctr = np.asarray(act_ctr, dtype=np.uint32)
+    out = np.zeros((env_ids.shape[0], A), dtype=np.float32)
+    for call in range((A + 3) // 4):
+        r = philox4x32(env_ids, act_ctr, np.uint32(call), np.uint32(0), seed, KEY_ACT)
+        for j in range(min(4, A - 4 * call)):
+            out[:, 4 * call + j] = usym(r[j])
+    return out
+
+
 def action_noise(seed, env_ids, act_ctr, A):
     """eps[e, a] for the action sampled with per-env counter act_ctr[e] (rollout.cu)."""
     env_ids = np.asarray(env_ids, dtype=np.uint32)
