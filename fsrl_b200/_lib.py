@@ -79,10 +79,10 @@ class Rollout(ctypes.Structure):
 class PpoUpdate(ctypes.Structure):
     _fields_ = [("theta", c_vp), ("grad", c_vp), ("adam_m", c_vp), ("adam_v", c_vp),
                 ("w2n", c_vp), ("scratch", c_vp), ("norm_sq", c_vp), ("stats", c_vp),
-                ("mask", c_vp), ("net_off", ctypes.c_longlong * 3),
+                ("net_off", ctypes.c_longlong * 3),
                 ("n_params", ctypes.c_longlong),
                 ("n_nets", c_int), ("D", c_int), ("H", c_int), ("A", c_int), ("C", c_int),
-                ("actor_out", c_int), ("bmax", c_int), ("head_indep", c_int),
+                ("actor_out", c_int), ("bmax", c_int), ("pad2", c_int),
                 ("obs", c_vp), ("act", c_vp), ("logp_old", c_vp), ("adv", c_vp), ("ret", c_vp),
                 ("values", c_vp), ("ld", ctypes.c_longlong), ("perm", c_vp),
                 ("eps_clip", c_f32), ("dual_clip", c_f32), ("vf_coef", c_f32),

@@ -43,7 +43,7 @@ int launch_w2_mirror(const W2Mirror& mr, int n_nets, int H, cudaStream_t s) {
 }  // namespace fsrl
 
 extern "C" const char* fsrl_last_error(void) { return fsrl::g_err; }
-extern "C" int fsrl_abi_version(void) { return 1; }
+extern "C" int fsrl_abi_version(void) { return 2; }
 namespace fsrl { unsigned long long g_launches = 0; }
 extern "C" unsigned long long fsrl_launch_count(void) { return fsrl::g_launches; }
 extern "C" int fsrl_sm_count(void) { return fsrl::sm_count(); }

@@ -24,13 +24,12 @@
 //   out-major mirror (needed by the backward GEMM) are written coalesced.
 #include "mlp.cuh"
 #include "fsrl_b200.h"
+#include "ppo_loss.cuh"
 #include "ppo_persist.cuh"
 #include <cstdlib>
 
 namespace fsrl {
 
-constexpr int ST_ACTOR_REW = 0, ST_ACTOR_SAFETY = 1, ST_KL = 2, ST_VF0 = 3, ST_VF1 = 4,
-              ST_ENTROPY = 5, ST_GRADNORM = 6, ST_CLIPFRAC = 7;
 constexpr int DOUT_LD = 16;   // scratch row stride of dOut (cols [A, 2A) carry dlog_sigma)
 
 // Programmatic dependent launch (sm_90+): a kernel launched with the programmatic-serialization
@@ -66,12 +65,9 @@ __device__ __forceinline__ NetView net_view(const fsrl_ppo_update_t& u, int n) {
 // (grid = row tiles x column slabs x nets = 192 CTAs for B = 256, H = 256):
 //   A1 ppo_fwd : x -> h1 (full, tiny K) -> h2[:, slab]           (scratch: h1, h2)
 //   A2 ppo_bwd : h2 (full) -> head -> loss gradient -> dz2 (full) -> dz1[:, slab]
-// Rows are addressed through row_of(): the epoch driver first gathers the permuted batch into
-// contiguous arrays (u.perm == nullptr afterwards), so minibatch rows are coalesced.
+// The epoch driver first gathers the permuted batch into contiguous arrays, so minibatch row i is
+// row mb_off + i of them and its loads are coalesced.
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ long long row_of(const fsrl_ppo_update_t& u, int mb_off, int i) {
-    return u.perm ? (long long)u.perm[mb_off + i] : (long long)(mb_off + i);
-}
 
 template <int H>
 __global__ void __launch_bounds__(MLP_TPB)
@@ -91,7 +87,7 @@ ppo_fwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B) {
     // observations are constant during a repeat: loaded while the previous optimiser step drains
     for (int i = tid; i < TT::R * inp; i += MLP_TPB) {
         const int r = i / inp, k = i % inp;
-        xs[i] = (r0 + r < B && k < D) ? u.obs[(size_t)row_of(u, mb_off, r0 + r) * D + k] : 0.f;
+        xs[i] = (r0 + r < B && k < D) ? u.obs[(size_t)(mb_off + r0 + r) * D + k] : 0.f;
     }
     pdl_wait();                                         // parameters of the previous step are final
     pdl_trigger();
@@ -153,7 +149,7 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
     float* bs = dz + (size_t)TT::R * TT::LDA;           // [H][SLAB_LDB]
     float* w3s = bs + slab_buf_floats<H>();             // [H][out]
     float* sdout = w3s + (size_t)H * wout;              // [R][DOUT_LD]
-    __shared__ float s_mean[2], s_rstd[2], s_b3[MLP_MAX_OUT], s_ls[8];
+    __shared__ float s_mean[2], s_rstd[2], s_b3[MLP_MAX_OUT], s_ls[8], s_rsg[8];
     // everything that does not depend on the forward launch (weights, per-row loss inputs) is
     // requested before pdl_wait(): it overlaps the forward kernel's tail
     slab_load<H>(nv.w2n, H, c0, bs);                    // W2 in [out][in] layout: rows o, columns k-slab
@@ -161,7 +157,7 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
     // per-row scalars of the loss: issued now, consumed after the head
     const int r = tid / TT::PARTS, part = tid % TT::PARTS;
     const bool row_ok = (part == 0) && (r0 + r < B);
-    const long long id = row_ok ? row_of(u, mb_off, r0 + r) : 0;
+    const long long id = row_ok ? (long long)(mb_off + r0 + r) : 0;
     float p_act[8], p_lpo = 0.f, p_adv0 = 0.f, p_adv1 = 0.f, p_ret = 0.f, p_val = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) p_act[j] = 0.f;
@@ -185,7 +181,11 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
         s_rstd[tid] = ms[1];
     }
     if (tid >= 32 && tid < 32 + wout) s_b3[tid - 32] = __ldg(nv.m.b3 + tid - 32);
-    if (net == 0 && tid >= 64 && tid < 64 + u.A) s_ls[tid - 64] = nv.extra[tid - 64];
+    if (net == 0 && tid >= 64 && tid < 64 + u.A) {          // log sigma and 1 / sigma
+        const float ls = nv.extra[tid - 64];
+        s_ls[tid - 64] = ls;
+        s_rsg[tid - 64] = 1.0f / expf(ls);
+    }
     pdl_wait();                                          // h1 / h2 of this minibatch are complete
     pdl_trigger();
     for (int el = tid; el < TT::R * (H / 4); el += MLP_TPB) {
@@ -230,72 +230,15 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
             const float invB = 1.0f / (float)B;
             if (net == 0) {
                 const int A = u.A;
-                float logp = 0.f, zz[8], sg[8], dmu[8];
+                float g_mu[8], g_ls[8];
+                ppo_actor_row(u, out, p_act, s_ls, s_rsg, p_lpo, p_adv0, p_adv1, s_mean, s_rstd, invB, g_mu, g_ls,
+                              st_a, st_b, st_c);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
-                    if (j < A) {
-                        const float t = tanhf(out[j]);
-                        const float mu = u.bounded ? u.max_action * t : out[j];
-                        dmu[j] = u.bounded ? u.max_action * (1.0f - t * t) : 1.0f;
-                        sg[j] = expf(s_ls[j]);
-                        zz[j] = (p_act[j] - mu) / sg[j];
-                        logp += -0.5f * zz[j] * zz[j] - s_ls[j] - LOG_SQRT_2PI;
-                    }
+                    if (j < A) { dd[j] = g_mu[j]; dd[A + j] = g_ls[j]; }     // log sigma columns follow the A mean columns
                 }
-                const float lpo = p_lpo;
-                const float ratio = expf(logp - lpo);
-                const float ar = (p_adv0 - s_mean[0]) * s_rstd[0];
-                const float surr1 = ratio * ar;
-                const float rc = fminf(fmaxf(ratio, 1.0f - u.eps_clip), 1.0f + u.eps_clip);
-                const float surr2 = rc * ar;
-                // d(-min(surr1, surr2))/d ratio ; ties split evenly like torch.min's backward
-                const bool inside = (ratio >= 1.0f - u.eps_clip) && (ratio <= 1.0f + u.eps_clip);
-                float g_ratio;   // d loss_rew_i / d ratio  (before the 1/B of the mean)
-                float lrew;
-                if (surr1 < surr2) { g_ratio = -ar; lrew = -surr1; }
-                else if (surr1 > surr2) { g_ratio = inside ? -ar : 0.f; lrew = -surr2; }
-                else { g_ratio = inside ? -ar : -0.5f * ar; lrew = -surr1; }
-                if (u.dual_clip > 0.f && ar < 0.f) {
-                    // clip2 = max(min(s1,s2), dual_clip*adv) for negative advantages (:188-191)
-                    const float c1 = fminf(surr1, surr2), c2 = u.dual_clip * ar;
-                    if (c2 > c1) { g_ratio = 0.f; lrew = -c2; }
-                    else if (c2 == c1) { g_ratio *= 0.5f; }
-                }
-                float g_saf = 0.f, lsaf = 0.f;
-                if (u.use_lagrangian && u.C > 1) {
-                    const float ac = (p_adv1 - s_mean[1]) * s_rstd[1];
-                    g_saf = ac * u.lagrangian;          // d mean(ratio*adv_c*lambda) / d ratio
-                    lsaf = ratio * ac * u.lagrangian;
-                }
-                // d loss / d logp = rescaling * (g_ratio + g_saf) * ratio / B
-                const float gl = u.rescaling * (g_ratio + g_saf) * ratio * invB;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    if (j < A) {
-                        dd[j] = gl * (zz[j] / sg[j]) * dmu[j];        // via mu
-                        dd[A + j] = gl * (zz[j] * zz[j] - 1.0f);       // via log_sigma
-                    }
-                }
-                st_a = lrew * invB; st_b = lsaf * invB; st_c = (lpo - logp) * invB;
             } else {
-                const float v = out[0];
-                const float ret = p_ret;
-                float lv, gv;
-                if (u.value_clip) {
-                    const float vt = p_val;
-                    const float dv = fminf(fmaxf(v - vt, -u.eps_clip), u.eps_clip);
-                    const float vc = vt + dv;
-                    const float vf1 = (ret - v) * (ret - v), vf2 = (ret - vc) * (ret - vc);
-                    const bool in_clip = (v - vt > -u.eps_clip) && (v - vt < u.eps_clip);
-                    if (vf1 > vf2) { lv = vf1; gv = 2.0f * (v - ret); }
-                    else if (vf1 < vf2) { lv = vf2; gv = in_clip ? 2.0f * (vc - ret) : 0.f; }
-                    else { lv = vf1; gv = in_clip ? 2.0f * (v - ret) : (v - ret); }
-                } else {
-                    lv = (ret - v) * (ret - v);
-                    gv = 2.0f * (v - ret);
-                }
-                dd[0] = u.vf_coef * gv * invB;
-                st_d = lv * invB;
+                dd[0] = ppo_value_row(u, out[0], p_ret, p_val, invB, st_d);
             }
         }
 #pragma unroll
@@ -317,11 +260,7 @@ ppo_bwd_kernel(const fsrl_ppo_update_t u, int mb_off, int B, int slot) {
             if (lane == 0) {
                 atomicAdd(stat + ST_ACTOR_REW, a); atomicAdd(stat + ST_ACTOR_SAFETY, b); atomicAdd(stat + ST_KL, c);
             }
-            if (blockIdx.x == 0 && tid == 0) {
-                float ent = 0.f;
-                for (int j = 0; j < u.A; ++j) ent += 0.5f + LOG_SQRT_2PI + s_ls[j];
-                stat[ST_ENTROPY] = ent;
-            }
+            if (blockIdx.x == 0 && tid == 0) stat[ST_ENTROPY] = ppo_entropy(s_ls, u.A);
         } else {
             const float d = warp_sum(st_d);
             if (lane == 0) atomicAdd(stat + ST_VF0 + (net - 1), d);
@@ -540,7 +479,7 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
             grid_barrier(bar, bar_target);
             const float nsq = __ldcg(u.norm_sq);
             if (u.max_grad_norm > 0.f) gscale = fminf(u.max_grad_norm / (sqrtf(nsq) + 1e-6f), 1.0f);
-            if (bx == 0 && net == 0 && tid == 0 && u.stats && slot >= 0)
+            if (bx == 0 && net == 0 && tid == 0 && slot >= 0)
                 u.stats[(size_t)slot * FSRL_PPO_STATS + ST_GRADNORM] = sqrtf(nsq);
         }
     };
@@ -635,14 +574,14 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
                 for (int i = tid; i < WG_RC * 4; i += WG_TPB) {
                     const int rr = i / 4, v = v0 + 4 * (i % 4);
                     float* dst = xs_ + (size_t)rr * WG_LD + 4 * (i % 4);
-                    if (rb + rr < B && v < D) __pipeline_memcpy_async(dst, u.obs + (size_t)row_of(u, mb_off, rb + rr) * D + v, 16);
+                    if (rb + rr < B && v < D) __pipeline_memcpy_async(dst, u.obs + (size_t)(mb_off + rb + rr) * D + v, 16);
                     else *reinterpret_cast<float4*>(dst) = make_float4((rb + rr < B && v == D) ? 1.0f : 0.f, 0.f, 0.f, 0.f);
                 }
             } else {
                 for (int i = tid; i < WG_RC * 16; i += WG_TPB) {
                     const int rr = i / 16, v = v0 + (i % 16);
                     float* dst = xs_ + (size_t)rr * WG_LD + (i % 16);
-                    if (rb + rr < B && v < D) __pipeline_memcpy_async(dst, u.obs + (size_t)row_of(u, mb_off, rb + rr) * D + v, 4);
+                    if (rb + rr < B && v < D) __pipeline_memcpy_async(dst, u.obs + (size_t)(mb_off + rb + rr) * D + v, 4);
                     else *dst = (rb + rr < B && v == D) ? 1.0f : 0.f;
                 }
             }
@@ -731,7 +670,7 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
             for (int q = 0; q < WG_TPB / DOUT_LD; ++q) csum += cred[q * DOUT_LD + tid];
         }
         const bool own_b3 = (k0 == 0) && tid < out;
-        const bool own_ls = (k0 == 0) && net == 0 && u.head_indep && tid >= A && tid < 2 * A && tid < DOUT_LD;
+        const bool own_ls = (k0 == 0) && net == 0 && tid >= A && tid < 2 * A && tid < DOUT_LD;
 #pragma unroll
         for (int q = 0; q < 4; ++q) if (4 * jg + q < out) sq += acc[q] * acc[q];
         if (own_b3 || own_ls) sq += csum * csum;
@@ -802,7 +741,7 @@ adam_kernel(const fsrl_ppo_update_t u, const AdamStep ad, int slot, int n_plain_
         const float coef = u.max_grad_norm / (sqrtf(nsq) + 1e-6f);
         scale = gs * fminf(coef, 1.0f);
     }
-    if (blockIdx.x == 0 && threadIdx.x == 0 && u.stats && slot >= 0)
+    if (blockIdx.x == 0 && threadIdx.x == 0 && slot >= 0)
         u.stats[(size_t)slot * FSRL_PPO_STATS + ST_GRADNORM] = sqrtf(nsq);
     const int H = u.H;
     if ((int)blockIdx.x < n_plain_blocks) {
@@ -821,9 +760,7 @@ adam_kernel(const fsrl_ppo_update_t u, const AdamStep ad, int slot, int n_plain_
         }
         if (i < 0) return;
         float m = u.adam_m[i], v = u.adam_v[i];
-        const float g = (u.mask && u.mask[i] == 0) ? 0.f : u.grad[i] * scale;
-        if (u.mask && u.mask[i] == 0) return;
-        u.theta[i] = adam_update(u.theta[i], g, m, v, ad);
+        u.theta[i] = adam_update(u.theta[i], u.grad[i] * scale, m, v, ad);
         u.adam_m[i] = m; u.adam_v[i] = v;
     } else {
         // W2 tiles: 32 x 32, update canonical W2t[k][o] and its mirror W2n[o][k]
@@ -831,15 +768,11 @@ adam_kernel(const fsrl_ppo_update_t u, const AdamStep ad, int slot, int n_plain_
         const int t = blockIdx.x - n_plain_blocks;
         const int n = t / tpn, tt = t % tpn;
         const long long base = u.net_off[n] + arena_layout(u.D, H, (n == 0) ? u.actor_out : 1, 0).w2;
-        const bool frozen = u.mask && u.mask[base] == 0;
         w2_tile(u.w2n + (size_t)n * H * H, H, (tt / (H / 32)) * 32, (tt % (H / 32)) * 32, [&](int k, int o) {
             const long long i = base + (long long)k * H + o;
-            float p = u.theta[i];
-            if (!frozen) {
-                float m = u.adam_m[i], v = u.adam_v[i];
-                p = adam_update(p, u.grad[i] * scale, m, v, ad);
-                u.theta[i] = p; u.adam_m[i] = m; u.adam_v[i] = v;
-            }
+            float m = u.adam_m[i], v = u.adam_v[i];
+            const float p = adam_update(u.theta[i], u.grad[i] * scale, m, v, ad);
+            u.theta[i] = p; u.adam_m[i] = m; u.adam_v[i] = v;
             return p;
         });
     }
@@ -924,7 +857,7 @@ __global__ void __launch_bounds__(256) ppo_adv_moments_kernel(const fsrl_ppo_upd
     for (int c = 0; c < u.C; ++c) {
         double s = 0.0, q = 0.0;
         for (long long i = threadIdx.x; i < B; i += 256) {
-            const double a = (double)u.adv[(size_t)c * u.ld + (u.perm ? (long long)u.perm[off + i] : off + i)];
+            const double a = (double)u.adv[(size_t)c * u.ld + off + i];
             s += a; q += a * a;
         }
         const double ts = block_sum<8>(s, red[0]), tq = block_sum<8>(q, red[1]);
@@ -959,11 +892,11 @@ __global__ void __launch_bounds__(256) ppo_adv_stats_kernel(const fsrl_ppo_updat
         // two-pass like torch: mean in fp32 arithmetic would differ in the last bits only; use f64 sums
         double sacc = 0.0;
         for (long long i = threadIdx.x; i < B; i += 256)
-            sacc += (double)u.adv[(size_t)c * u.ld + (u.perm ? (long long)u.perm[off + i] : off + i)];
+            sacc += (double)u.adv[(size_t)c * u.ld + off + i];
         const float mean = (float)(block_sum<8>(sacc, red) / (double)B);
         double q = 0.0;
         for (long long i = threadIdx.x; i < B; i += 256) {
-            const float d = u.adv[(size_t)c * u.ld + (u.perm ? (long long)u.perm[off + i] : off + i)] - mean;
+            const float d = u.adv[(size_t)c * u.ld + off + i] - mean;
             q += (double)(d * d);
         }
         q = block_sum<8>(q, red);
@@ -1030,7 +963,7 @@ static int ppo_launch_minibatch(const fsrl_ppo_update_t& u, int mb_off, int B, i
         attr_w = true;
     }
     const AdamStep ad = adam_step_scalars(u.lr, u.beta1, u.beta2, u.adam_eps, adam_t);
-    if (u.world <= 1 && fuse_ok == 1 && u.barrier != nullptr && u.mask == nullptr) {
+    if (u.world <= 1 && fuse_ok == 1) {
         // single GPU: gradients never leave the registers -- tiles -> norm -> barrier -> clip + Adam
         unsigned long long target = (unsigned long long)(bar_count + 1) * gB.x * gB.y;
         // Ordinary (not cooperative) launch: no cooperative-launch overhead per step.  The grid barrier is still
@@ -1123,6 +1056,7 @@ extern "C" int fsrl_ppo_lag_epoch(const fsrl_ppo_update_t* u, long long n_total,
     int rc = check_update(u);
     if (rc) return rc;
     FSRL_REQUIRE(u->obs && u->act && u->logp_old && u->adv && u->ret && u->perm && u->stats, "ppo: null batch pointer");
+    FSRL_REQUIRE(u->gather && u->barrier, "ppo: null gather or barrier buffer");
     FSRL_REQUIRE(n_total <= 2147483647LL, "ppo: batch too large for 32-bit row offsets");
     FSRL_REQUIRE(batch_size >= 2 && n_total >= 2, "ppo: batch too small");
     FSRL_REQUIRE(2 * batch_size - 1 <= u->bmax || n_total <= u->bmax, "ppo: scratch bmax %d too small for batch_size %d", u->bmax, batch_size);
@@ -1130,22 +1064,20 @@ extern "C" int fsrl_ppo_lag_epoch(const fsrl_ppo_update_t* u, long long n_total,
     int count = 0;
     const bool merge_last = (n_total % batch_size) > 0;       // tianshou Batch.split
     fsrl_ppo_update_t ug = *u;
-    if (u->barrier) FSRL_CUDA(cudaMemsetAsync(u->barrier, 0, sizeof(unsigned long long), s));
-    if (u->gather) {
-        // one coalescing pass per repeat: the permuted batch becomes contiguous, minibatch k is
-        // rows [k*bs, (k+1)*bs) and no kernel chases indices afterwards
-        ppo_gather_kernel<<<(unsigned)((n_total + 255) / 256), 256, 0, s>>>(*u, n_total);
-        FSRL_LAUNCH_CHECK();
-        float* g = u->gather;
-        ug.obs = g; g += n_total * u->D;
-        ug.act = g; g += n_total * u->A;
-        ug.logp_old = g; g += n_total;
-        ug.adv = g; g += (long long)u->C * n_total;
-        ug.ret = g; g += (long long)u->C * n_total;
-        ug.values = u->values ? g : nullptr;
-        ug.ld = n_total;
-        ug.perm = nullptr;
-    }
+    FSRL_CUDA(cudaMemsetAsync(u->barrier, 0, sizeof(unsigned long long), s));
+    // one coalescing pass per repeat: the permuted batch becomes contiguous, minibatch k is
+    // rows [k*bs, (k+1)*bs) and no kernel chases indices afterwards
+    ppo_gather_kernel<<<(unsigned)((n_total + 255) / 256), 256, 0, s>>>(*u, n_total);
+    FSRL_LAUNCH_CHECK();
+    float* g = u->gather;
+    ug.obs = g; g += n_total * u->D;
+    ug.act = g; g += n_total * u->A;
+    ug.logp_old = g; g += n_total;
+    ug.adv = g; g += (long long)u->C * n_total;
+    ug.ret = g; g += (long long)u->C * n_total;
+    ug.values = u->values ? g : nullptr;
+    ug.ld = n_total;
+    ug.perm = nullptr;
     ug.batch_size = batch_size;
     u = &ug;
     FSRL_REQUIRE(u->world <= 1 || (u->comm && u->moments_w && u->batch_size == batch_size),

@@ -36,6 +36,7 @@
 // memory (dp_* functions below: tagged + hashed 16-byte packets pushed into the peers' buffers).
 #include "ppo_persist.cuh"
 #include "arena.cuh"
+#include "ppo_loss.cuh"
 #include "wgmma.cuh"
 #include <cstdlib>
 #include <cmath>
@@ -93,8 +94,6 @@ constexpr int XG_PER_NET = 16 * TILE_FLOATS + 8 * SLICE_PK * 4;
 constexpr int XG_FLAG_FLOATS = 8 * 128 * 2;                      // (reserved: flag lines of the fenced protocol)
 constexpr int MAX_MB = 16384;                                    // minibatches per launch (Adam scalar table)
 constexpr long long WAIT_CYCLES = 6000000000LL;                  // ~3 s: a lost partner must not hang the GPU
-
-constexpr int ST_ACTOR_REW = 0, ST_ACTOR_SAFETY = 1, ST_KL = 2, ST_VF0 = 3, ST_ENTROPY = 5, ST_GRADNORM = 6;
 
 struct Args {
     fsrl_ppo_update_t u;     // batch pointers already gathered (contiguous rows, u.perm == nullptr)
@@ -621,7 +620,6 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
         const int n_dst = P.cluster ? 8 : 1;
         const uint32_t empty_r = mapa_u32(smem_u32(bar_empty), lane < n_dst ? lane : 0);
         float w2p[C2], w2m[C2], w2v[C2];            // owned W2 tile (G3 CTAs): parameters and Adam moments
-        float* stat_base = u.stats;
         // ---- data-parallel exchange over peer memory (NVLink): every CTA pushes its local gradient piece into its
         // rank's region of EVERY rank's exchange buffer, one thread fences and release-stores the step id into the same
         // slot of every rank's flag array; the receiver waits for the ranks' flags and sums their pieces from its own
@@ -650,7 +648,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             if (i < sm.b2) { const int d = i / 32, kk = i % 32; src = (d < D) ? o_w1 + (long long)d * H + 32 * b + kk : o_b1 + 32 * b + kk; }
             else if (i < sm.w3) src = o_b2 + 32 * b + (i - sm.b2);
             else if (i < sm.b3) { const int oo = (i - sm.w3) / OUTP, jj = (i - sm.w3) % OUTP; if (jj < out) src = o_w3 + (long long)(32 * b + oo) * out + jj; }
-            else { const int jj = i - sm.b3; if (jj < out) src = o_b3 + jj; else if (net == 0 && u.head_indep && jj >= 8 && jj < 8 + A) src = o_ls + (jj - 8); }
+            else { const int jj = i - sm.b3; if (jj < out) src = o_b3 + jj; else if (net == 0 && jj >= 8 && jj < 8 + A) src = o_ls + (jj - 8); }
             sp_p[i] = src >= 0 ? u.theta[src] : 0.f;
             sp_m[i] = src >= 0 ? u.adam_m[src] : 0.f;
             sp_v[i] = src >= 0 ? u.adam_v[src] : 0.f;
@@ -759,7 +757,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
 
             // per-row loss inputs (independent of the GEMM): issued now, consumed after the head
             const long long grow = row0 + 64 * a + trow;
-            float p_act[8], p_lpo = 0.f, p_adv0 = 0.f, p_adv1 = 0.f, p_ret = 0.f, p_val = 0.f, mean0 = 0.f, rstd0 = 1.f, mean1 = 0.f, rstd1 = 1.f;
+            float p_act[8], p_lpo = 0.f, p_adv0 = 0.f, p_adv1 = 0.f, p_ret = 0.f, p_val = 0.f, mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
 #pragma unroll
             for (int j = 0; j < 8; ++j) p_act[j] = 0.f;
             if (net == 0) {
@@ -769,7 +767,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 p_adv0 = __ldg(u.adv + grow);
                 if (C > 1) p_adv1 = __ldg(u.adv + u.ld + grow);
                 const float* ms = u.mb_stats + (size_t)t * 4;
-                mean0 = __ldg(ms); rstd0 = __ldg(ms + 1); mean1 = __ldg(ms + 2); rstd1 = __ldg(ms + 3);
+                mean[0] = __ldg(ms); rstd[0] = __ldg(ms + 1); mean[1] = __ldg(ms + 2); rstd[1] = __ldg(ms + 3);
             } else {
                 p_ret = __ldg(u.ret + (long long)(net - 1) * u.ld + grow);
                 if (u.value_clip) p_val = __ldg(u.values + (long long)(net - 1) * u.ld + grow);
@@ -881,66 +879,13 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             {
                 const float invB = 1.0f / (float)MB;
                 if (net == 0) {
-                    float logp = 0.f, zz[8], dmu[8];
+                    float g_mu[8], g_ls[8];
+                    ppo_actor_row(u, outv, p_act, p_ls, p_rsg, p_lpo, p_adv0, p_adv1, mean, rstd, invB, g_mu, g_ls,
+                                  st_a, st_b, st_c);
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        zz[j] = dmu[j] = 0.f;
-                        if (j < A) {
-                            const float tnh = tanhf(outv[j]);
-                            const float mu = u.bounded ? u.max_action * tnh : outv[j];
-                            dmu[j] = u.bounded ? u.max_action * (1.0f - tnh * tnh) : 1.0f;
-                            zz[j] = (p_act[j] - mu) * p_rsg[j];
-                            logp += -0.5f * zz[j] * zz[j] - p_ls[j] - LOG_SQRT_2PI;
-                        }
-                    }
-                    const float ratio = expf(logp - p_lpo);
-                    const float ar = (p_adv0 - mean0) * rstd0;
-                    const float surr1 = ratio * ar;
-                    const float rc = fminf(fmaxf(ratio, 1.0f - u.eps_clip), 1.0f + u.eps_clip);
-                    const float surr2 = rc * ar;
-                    const bool inside = (ratio >= 1.0f - u.eps_clip) && (ratio <= 1.0f + u.eps_clip);
-                    float g_ratio, lrew;
-                    if (surr1 < surr2) { g_ratio = -ar; lrew = -surr1; }
-                    else if (surr1 > surr2) { g_ratio = inside ? -ar : 0.f; lrew = -surr2; }
-                    else { g_ratio = inside ? -ar : -0.5f * ar; lrew = -surr1; }
-                    if (u.dual_clip > 0.f && ar < 0.f) {
-                        const float c1 = fminf(surr1, surr2), c2 = u.dual_clip * ar;
-                        if (c2 > c1) { g_ratio = 0.f; lrew = -c2; }
-                        else if (c2 == c1) { g_ratio *= 0.5f; }
-                    }
-                    float g_saf = 0.f, lsaf = 0.f;
-                    if (u.use_lagrangian && C > 1) {
-                        const float ac = (p_adv1 - mean1) * rstd1;
-                        g_saf = ac * u.lagrangian;
-                        lsaf = ratio * ac * u.lagrangian;
-                    }
-                    const float gl = u.rescaling * (g_ratio + g_saf) * ratio * invB;
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        if (j < A) {
-                            dd[j] = gl * (zz[j] * p_rsg[j]) * dmu[j];
-                            dd[8 + j] = gl * (zz[j] * zz[j] - 1.0f);
-                        }
-                    }
-                    st_a = lrew * invB; st_b = lsaf * invB; st_c = (p_lpo - logp) * invB;
+                    for (int j = 0; j < 8; ++j) { dd[j] = g_mu[j]; dd[8 + j] = g_ls[j]; }    // log sigma columns: 8 ..
                 } else {
-                    const float v = outv[0], ret = p_ret;
-                    float lv, gv;
-                    if (u.value_clip) {
-                        const float vt = p_val;
-                        const float dv = fminf(fmaxf(v - vt, -u.eps_clip), u.eps_clip);
-                        const float vc = vt + dv;
-                        const float vf1 = (ret - v) * (ret - v), vf2 = (ret - vc) * (ret - vc);
-                        const bool in_clip = (v - vt > -u.eps_clip) && (v - vt < u.eps_clip);
-                        if (vf1 > vf2) { lv = vf1; gv = 2.0f * (v - ret); }
-                        else if (vf1 < vf2) { lv = vf2; gv = in_clip ? 2.0f * (vc - ret) : 0.f; }
-                        else { lv = vf1; gv = in_clip ? 2.0f * (v - ret) : (v - ret); }
-                    } else {
-                        lv = (ret - v) * (ret - v);
-                        gv = 2.0f * (v - ret);
-                    }
-                    dd[0] = u.vf_coef * gv * invB;
-                    st_d = lv * invB;
+                    dd[0] = ppo_value_row(u, outv[0], p_ret, p_val, invB, st_d);
                 }
             }
             if (et == 0) STAMP(26);
@@ -1011,17 +956,13 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                     const int i = 288 + et;
                     const float tot = ((s_red[0][i] + s_red[1][i]) + s_red[2][i]) + s_red[3][i];
                     if (et < 16) wsn[DB3P_OFF + a * 16 + et] = tot;
-                    else if (stat_base) {
-                        float* stat = stat_base + (size_t)slot * FSRL_PPO_STATS;
+                    else {
+                        float* stat = u.stats + (size_t)slot * FSRL_PPO_STATS;
                         if (net == 0) { if (et == 16) atomicAdd(stat + ST_ACTOR_REW, tot); if (et == 17) atomicAdd(stat + ST_ACTOR_SAFETY, tot); if (et == 18) atomicAdd(stat + ST_KL, tot); }
                         else if (et == 19) atomicAdd(stat + ST_VF0 + (net - 1), tot);
                     }
                 }
-                if (net == 0 && a == 0 && et == 20 && stat_base) {
-                    float ent = 0.f;
-                    for (int jq = 0; jq < A; ++jq) ent += 0.5f + LOG_SQRT_2PI + sp_p[sm.b3 + 8 + jq];
-                    stat_base[(size_t)slot * FSRL_PPO_STATS + ST_ENTROPY] = ent;
-                }
+                if (net == 0 && a == 0 && et == 20) u.stats[(size_t)slot * FSRL_PPO_STATS + ST_ENTROPY] = ppo_entropy(sp_p + sm.b3 + 8, A);
             }
             fence_proxy_async_smem();                                // scratch stores before the next bulk copies into the ring
             epi_bar();
@@ -1122,7 +1063,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                                 src = wsn + DW3P_OFF + ((size_t)32 * b + oo) * OUTP + jj; stride = (size_t)H * OUTP;
                             } else {
                                 const int jj = i - sm.b3;
-                                real[e] = (jj < out) || (net == 0 && u.head_indep && jj >= 8 && jj < 8 + A);
+                                real[e] = (jj < out) || (net == 0 && jj >= 8 && jj < 8 + A);
                                 src = wsn + DB3P_OFF + jj; stride = 16;
                             }
                         }
@@ -1162,7 +1103,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 for (int i = et; i < sm.n; i += NEPI) {
                     bool real = true;
                     if (i >= sm.w3 && i < sm.b3) real = ((i - sm.w3) % OUTP) < out;
-                    else if (i >= sm.b3) { const int jj = i - sm.b3; real = (jj < out) || (net == 0 && u.head_indep && jj >= 8 && jj < 8 + A); }
+                    else if (i >= sm.b3) { const int jj = i - sm.b3; real = (jj < out) || (net == 0 && jj >= 8 && jj < 8 + A); }
                     if (real && (i < sm.b3 || b == 0)) sq = fmaf(sp_g[i], sp_g[i], sq);
                 }
             }
@@ -1188,7 +1129,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             nsq = warp_sum(nsq);
             float gscale = 1.0f;
             if (u.max_grad_norm > 0.f) gscale = fminf(u.max_grad_norm / (sqrtf(nsq) + 1e-6f), 1.0f);
-            if (blockIdx.x == 0 && et == 0 && stat_base) stat_base[(size_t)slot * FSRL_PPO_STATS + ST_GRADNORM] = sqrtf(nsq);
+            if (blockIdx.x == 0 && et == 0) u.stats[(size_t)slot * FSRL_PPO_STATS + ST_GRADNORM] = sqrtf(nsq);
             const AdamS ad = s_adam;
             if (et == 0) STAMP(24);
             // ---- clip + Adam: replicated small slices, then the owned W2 tile (registers) ------------------------
@@ -1215,7 +1156,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 if (i < sm.b2) { const int d = i / 32, kk = i % 32; dst = (d < D) ? o_w1 + (long long)d * H + 32 * b + kk : o_b1 + 32 * b + kk; }
                 else if (i < sm.w3) dst = o_b2 + 32 * b + (i - sm.b2);
                 else if (i < sm.b3) { const int oo = (i - sm.w3) / OUTP, jj = (i - sm.w3) % OUTP; if (jj < out) dst = o_w3 + (long long)(32 * b + oo) * out + jj; }
-                else if (b == 0) { const int jj = i - sm.b3; if (jj < out) dst = o_b3 + jj; else if (net == 0 && u.head_indep && jj >= 8 && jj < 8 + A) dst = o_ls + (jj - 8); }
+                else if (b == 0) { const int jj = i - sm.b3; if (jj < out) dst = o_b3 + jj; else if (net == 0 && jj >= 8 && jj < 8 + A) dst = o_ls + (jj - 8); }
                 if (dst >= 0) { u.theta[dst] = sp_p[i]; u.adam_m[dst] = sp_m[i]; u.adam_v[dst] = sp_v[i]; }
             }
         }
@@ -1249,7 +1190,6 @@ size_t ppo_persist_p2p_floats(int n_nets) { return (size_t)(FSRL_P2P_MAX_RANKS +
 
 bool ppo_persist_supported(const fsrl_ppo_update_t& u, long long n_total, int batch_size) {
     if (u.H != 256 || batch_size != pp::MB || n_total % pp::MB != 0 || n_total < pp::MB || n_total / pp::MB > pp::MAX_MB) return false;
-    if (u.mask != nullptr || u.gather == nullptr) return false;
     if (u.world > 1 && !(u.p2p_on && u.world <= FSRL_P2P_MAX_RANKS && (size_t)u.p2p_stride >= ppo_persist_p2p_floats(u.n_nets))) return false;
     if (u.D < 1 || u.D > pp::MAXD || u.A > 8 || u.n_nets < 1 || u.n_nets > 3) return false;
     if (u.persist_ws == nullptr || (size_t)u.persist_ws_floats < ppo_persist_ws_floats(u.n_nets, u.D, u.H)) return false;

@@ -13,19 +13,14 @@ class FusedAdam:
         self.step_count = 0
         self.m = None
         self.v = None
-        self.mask = None          # optional uint8 [n_params]; 0 = parameter not owned by this optimizer
 
     @property
     def lr(self):
         return self.param_groups[0]["lr"]
 
-    def attach(self, arena, owned_slots=None):
+    def attach(self, arena):
         self.m = torch.zeros_like(arena.theta)
         self.v = torch.zeros_like(arena.theta)
-        if owned_slots is not None:
-            self.mask = torch.zeros(arena.n_params, dtype=torch.uint8, device=arena.device)
-            for s in owned_slots:
-                self.mask[s.offset:s.offset + s.size] = 1
 
     def zero_grad(self, set_to_none: bool = False):
         pass   # gradients are fully overwritten by the wgrad kernel each step

@@ -98,12 +98,11 @@ class PPOLagrangian(LagrangianPolicy):
         u.adam_m, u.adam_v = self.optim.m.data_ptr(), self.optim.v.data_ptr()
         u.w2n, u.scratch = self._w2n.data_ptr(), self._scratch.data_ptr()
         u.norm_sq, u.stats = self._norm_sq.data_ptr(), self._stats_dev.data_ptr()
-        u.mask = None if self.optim.mask is None else self.optim.mask.data_ptr()
         for i, s in enumerate(ar.slots):
             u.net_off[i] = s.offset
         u.n_params = ar.n_params
         u.n_nets, u.D, u.H, u.A, u.C = len(ar.slots), s0.D, s0.H, s0.out, self.critics_num
-        u.actor_out, u.bmax, u.head_indep = s0.out, self._bmax, 1
+        u.actor_out, u.bmax = s0.out, self._bmax
         u.obs, u.act, u.logp_old = batch.obs.data_ptr(), batch.act.data_ptr(), batch.logp_old.data_ptr()
         u.adv, u.ret, u.values = batch.adv.data_ptr(), batch.ret.data_ptr(), batch.v.data_ptr()
         u.ld = batch.adv.shape[1]

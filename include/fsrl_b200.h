@@ -149,10 +149,9 @@ int fsrl_rollout_steps(const fsrl_rollout_t* r, int n_steps, void* stream);
 #define FSRL_PPO_STATS 8 /* per-minibatch: actor_rew, actor_safety, kl, vf0, vf1, entropy, grad_norm, - */
 typedef struct fsrl_ppo_update {
     float *theta, *grad, *adam_m, *adam_v, *w2n, *scratch, *norm_sq, *stats;
-    const unsigned char* mask;     /* optional [n_params]: 0 = frozen parameter */
     long long net_off[3];
     long long n_params;
-    int n_nets, D, H, A, C, actor_out, bmax, head_indep;
+    int n_nets, D, H, A, C, actor_out, bmax, pad2;
     /* the processed batch (flat env-major arrays) and the minibatch permutation */
     const float *obs, *act, *logp_old, *adv, *ret, *values; /* adv/ret/values: [C][ld] */
     long long ld;
@@ -169,13 +168,14 @@ typedef struct fsrl_ppo_update {
     double* moments_w;
     const double* moments;
     int world, batch_size;
-    /* optional [N*(D+A+1+3C)] floats: the epoch driver gathers the permuted batch into it once
+    /* required [N*(D+A+1+3C)] floats: the epoch driver gathers the permuted batch into it once
      * per repeat so that every minibatch is a contiguous row range */
     float* gather;
     /* [n_minibatches][2][2] floats: (mean, 1/std) of the advantages of every minibatch of the
      * repeat, filled by the epoch driver */
     float* mb_stats;
-    /* device u64 ticket counter of the in-kernel grid barrier (fused wgrad + Adam launch) */
+    /* required device u64: ticket counter of the in-kernel grid barrier (fused wgrad + Adam
+     * launch), reset by the epoch driver */
     unsigned long long* barrier;
     /* peer-memory gradient exchange (world > 1, optional; NCCL all-reduce when p2p_on == 0):
      * rank r's exchange block (fsrl_p2p_alloc) mapped into this process -- p2p_xg[b][r] its

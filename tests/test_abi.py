@@ -25,9 +25,11 @@ def test_library_exports_every_declared_symbol():
         assert n in names, f"{n} bound in python but not declared in include/fsrl_b200.h"
 
 
-def test_abi_version_and_error_text():
+def test_abi_version_2_and_error_text():
+    """Version 2: fsrl_ppo_update_t no longer carries `mask` and `head_indep`, so a binding built against version 1
+    would misread every field after `stats`."""
     from fsrl_b200 import _lib
-    assert _lib.lib.fsrl_abi_version() == 1
+    assert _lib.lib.fsrl_abi_version() == 2
     assert isinstance(_lib.last_error(), str)
 
 
@@ -43,6 +45,24 @@ def test_argument_validation_needs_no_gpu():
     with pytest.raises(ValueError):
         _lib.check(rc)
     assert _lib.lib.fsrl_gae_dual_workspace_bytes(614400) > 0
+
+
+def test_ppo_epoch_requires_gather_and_barrier():
+    """The PPO epoch driver always gathers the permuted batch and always resets the grid barrier's ticket counter:
+    a descriptor without either buffer is rejected before anything is enqueued (the pointers below are never
+    dereferenced)."""
+    from fsrl_b200 import _lib
+    fake = 1 << 20
+    u = _lib.PpoUpdate()
+    for f in ("theta", "grad", "adam_m", "adam_v", "w2n", "scratch", "norm_sq", "stats",
+              "obs", "act", "logp_old", "adv", "ret", "perm", "gather", "barrier"):
+        setattr(u, f, fake)
+    u.n_nets, u.D, u.H, u.A, u.C, u.actor_out, u.bmax = 3, 8, 256, 2, 2, 2, 1024
+    for missing in ("gather", "barrier"):
+        setattr(u, missing, None)
+        rc = _lib.lib.fsrl_ppo_lag_epoch(u, 1024, 256, 0, 0, None, None)
+        assert rc == _lib.FSRL_EINVAL and "gather or barrier" in _lib.last_error()
+        setattr(u, missing, fake)
 
 
 def test_ops_refuse_cpu_tensors():
