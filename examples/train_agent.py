@@ -19,8 +19,8 @@ import bullet_safety_gym  # noqa: E402,F401  (task registration side effect in t
 import gymnasium as gym  # noqa: E402
 from tianshou.env import ShmemVectorEnv, SubprocVectorEnv  # noqa: E402,F401
 
-from fsrl.agent import CPOAgent, DDPGLagAgent, FOCOPSAgent, PPOLagAgent, SACLagAgent, TRPOLagAgent  # noqa: E402
-from fsrl.config import cpo_cfg, ddpgl_cfg, focosp_cfg, ppol_cfg, sacl_cfg, trpol_cfg  # noqa: E402
+from fsrl.agent import CPOAgent, CVPOAgent, DDPGLagAgent, FOCOPSAgent, PPOLagAgent, SACLagAgent, TRPOLagAgent  # noqa: E402
+from fsrl.config import cpo_cfg, cvpo_cfg, ddpgl_cfg, focosp_cfg, ppol_cfg, sacl_cfg, trpol_cfg  # noqa: E402
 from fsrl.utils import BaseLogger  # noqa: E402
 from fsrl.utils.exp_util import auto_name  # noqa: E402
 
@@ -54,6 +54,12 @@ ALGOS = {
     "ddpgl": (ddpgl_cfg, DDPGLagAgent, dict(actor_lr="actor_lr", critic_lr="critic_lr", hidden_sizes="hidden_sizes",
               tau="tau", exploration_noise="exploration_noise", n_step="n_step", use_lagrangian="use_lagrangian",
               lagrangian_pid="lagrangian_pid", rescaling="rescaling", gamma="gamma")),
+    "cvpo": (cvpo_cfg, CVPOAgent, dict(estep_iter_num="estep_iter_num", estep_kl="estep_kl",
+             estep_dual_max="estep_dual_max", estep_dual_lr="estep_dual_lr", sample_act_num="sample_act_num",
+             mstep_iter_num="mstep_iter_num", mstep_kl_mu="mstep_kl_mu", mstep_kl_std="mstep_kl_std",
+             mstep_dual_max="mstep_dual_max", mstep_dual_lr="mstep_dual_lr", actor_lr="actor_lr", critic_lr="critic_lr",
+             gamma="gamma", n_step="n_step", tau="tau", hidden_sizes="hidden_sizes", double_critic="double_critic",
+             conditioned_sigma="conditioned_sigma", unbounded="unbounded", last_layer_scale="last_layer_scale")),
 }
 
 

@@ -147,11 +147,21 @@ class Cpo(ctypes.Structure):
                 ("log_sigma", c_vp)]
 
 
+class Cvpo(ctypes.Structure):
+    _fields_ = [("off", OffPolicy), ("K", c_int), ("estep_iters", c_int), ("mstep_iters", c_int),
+                ("cond_sigma", c_int), ("estep_kl", c_f32), ("estep_dual_max", c_f32), ("estep_dual_lr", c_f32),
+                ("qc_thres", c_f32), ("mstep_kl_mu", c_f32), ("mstep_kl_std", c_f32), ("mstep_dual_max", c_f32),
+                ("mstep_dual_lr", c_f32), ("estep_state", c_vp), ("mstep_state", c_vp), ("particles", c_vp),
+                ("part_idx", c_vp), ("mu_old", c_vp), ("std_old", c_vp), ("comb", c_vp), ("weights", c_vp),
+                ("log_sigma", c_vp), ("log_sigma_old", c_vp)]
+
+
 ALGO_SAC, ALGO_DDPG = 0, 1
 OFF_STATS = 8
+CVPO_STATS = 16
 
 MODE_TRAIN, MODE_EVAL, MODE_RANDOM = 0, 1, 2
-HEAD_GAUSS_INDEP, HEAD_GAUSS_COND, HEAD_DETERMINISTIC = 0, 1, 2
+HEAD_GAUSS_INDEP, HEAD_GAUSS_COND, HEAD_DETERMINISTIC, HEAD_GAUSS_COND_RAW = 0, 1, 2, 3
 BOUND_NONE, BOUND_CLIP, BOUND_TANH = 0, 1, 2
 PPO_STATS = 8
 
@@ -205,6 +215,8 @@ SIGNATURES = {
     "fsrl_nstep_prepare": (c_int, [ctypes.POINTER(OffPolicy), c_vp, c_int, c_vp]),
     "fsrl_offpolicy_steps": (c_int, [ctypes.POINTER(OffPolicy), c_vp, c_int, c_int, ctypes.c_longlong,
                                      ctypes.c_longlong, ctypes.c_ulonglong, c_vp, c_vp]),
+    "fsrl_cvpo_steps": (c_int, [ctypes.POINTER(Cvpo), c_vp, c_int, c_int, ctypes.c_longlong, ctypes.c_longlong,
+                                ctypes.c_ulonglong, c_vp, c_vp]),
     "fsrl_ppo_scratch_floats": (c_size, [c_int, c_int, c_int]),
     "fsrl_ppo_sync_mirror": (c_int, [ctypes.POINTER(PpoUpdate), c_vp]),
     "fsrl_ppo_persist_ws_floats": (c_size, [c_int, c_int, c_int]),
@@ -234,7 +246,7 @@ def _check_abi_sizes():
     lib.fsrl_abi_sizeof.restype = c_size
     lib.fsrl_abi_sizeof.argtypes = [c_int]
     for which, cls in enumerate((Mlp3, CollectStats, Rollout, PpoUpdate, NetRef, NetList, Engine, EngInput,
-                                 OffPolicy, Cpo)):
+                                 OffPolicy, Cpo, Cvpo)):
         want = lib.fsrl_abi_sizeof(which)
         if want != ctypes.sizeof(cls):
             raise ImportError(f"ABI mismatch: {cls.__name__} is {ctypes.sizeof(cls)} bytes in python, "

@@ -178,7 +178,7 @@ def install(force: bool = False) -> List[str]:
                        TensorboardLogger=_logger.TensorboardLogger, WandbLogger=_logger.WandbLogger,
                        exp_util=_exp_util, optim_util=_optim_util, net=f_net, logger=f_logger)
         cfgs = {}
-        for key in ("ppol", "cpo", "sacl", "ddpgl", "trpol", "focops", "focosp"):
+        for key in ("ppol", "cpo", "sacl", "ddpgl", "trpol", "focops", "focosp", "cvpo"):
             m = getattr(_config, key + "_cfg")
             sys.modules[f"fsrl.config.{key}_cfg"] = m
             cfgs[key + "_cfg"] = m

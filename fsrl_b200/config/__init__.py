@@ -1,5 +1,5 @@
 """Training configurations with the reference's field names and defaults
-(/root/reference/fsrl/config/{ppol,cpo,sacl,ddpgl,trpol,focosp}_cfg.py, SURVEY.md Appendix E), generated from
+(/root/reference/fsrl/config/{ppol,cpo,sacl,ddpgl,trpol,focosp,cvpo}_cfg.py, SURVEY.md Appendix E), generated from
 one compact table so that the CLI/YAML surface of ``examples/`` keeps working.  Pure data."""
 from __future__ import annotations
 
@@ -52,12 +52,28 @@ _TABLES: Dict[str, Dict[str, Any]] = {
                    deterministic_eval=True, action_scaling=True, action_bound_method="clip", epoch=200,
                    episode_per_collect=20, step_per_epoch=10000, repeat_per_collect=4, training_num=20,
                    batch_size=256, prefix="focops", **_COMMON_TAIL),
+    "cvpo": dict(_HEAD, estep_iter_num=1, estep_kl=0.02, estep_dual_max=20, estep_dual_lr=0.02, sample_act_num=16,
+                 mstep_iter_num=1, mstep_kl_mu=0.005, mstep_kl_std=0.0005, mstep_dual_max=0.5, mstep_dual_lr=0.1,
+                 actor_lr=5e-4, critic_lr=1e-3, gamma=0.97, n_step=2, tau=0.05, hidden_sizes=(128, 128),
+                 double_critic=False, conditioned_sigma=True, unbounded=False, last_layer_scale=False, epoch=200,
+                 episode_per_collect=10, step_per_epoch=10000, update_per_step=0.2, buffer_size=200000,
+                 worker="ShmemVectorEnv", training_num=20, testing_num=2, batch_size=256, reward_threshold=10000,
+                 save_interval=4, deterministic_eval=True, action_scaling=True, action_bound_method="clip",
+                 resume=False, save_ckpt=True, verbose=False, render=False, logdir="logs", project="fast-safe-rl",
+                 group=None, name=None, prefix="cvpo", suffix=""),
 }
 # per-suite overrides (class name -> changed fields); off-policy Mujoco adds gamma / n_step / buffer
 _ON_MUJOCO = dict(task="SafetyPointCircle1Gymnasium-v0", epoch=250, cost_limit=25, episode_per_collect=20,
                   step_per_epoch=20000, repeat_per_collect=4)
 _OFF_MUJOCO = dict(task="SafetyPointCircle1Gymnasium-v0", epoch=250, cost_limit=25, gamma=0.99, n_step=3,
                    step_per_epoch=20000, buffer_size=800000)
+# CVPO's Mujoco suite (cvpo_cfg.py) has its own base and per-class overrides, and a Mujoco5MCfg
+_CVPO_MUJOCO = dict(task="SafetyPointCircle1Gymnasium-v0", epoch=250, cost_limit=25, unbounded=True, gamma=0.995,
+                    n_step=3, step_per_epoch=20000, buffer_size=200000)
+_CVPO_MUJOCO_CLASSES = (("Mujoco2MCfg", dict(epoch=100)),
+                        ("Mujoco5MCfg", dict(epoch=250, unbounded=False, gamma=0.98, n_step=3, buffer_size=40000)),
+                        ("Mujoco20MCfg", dict(epoch=1000, sample_act_num=64)),
+                        ("Mujoco10MCfg", dict(epoch=500, unbounded=False, gamma=0.98, sample_act_num=32)))
 
 
 def _dc(name, fields: Dict[str, Any], base=None):
@@ -74,6 +90,11 @@ def _module(key: str) -> types.ModuleType:
     m.TrainCfg = base
     for nm, ep in (("Bullet1MCfg", 100), ("Bullet5MCfg", 500), ("Bullet10MCfg", 1000)):
         setattr(m, nm, _dc(nm, {"epoch": ep}, base))
+    if key == "cvpo":
+        mj = m.MujocoBaseCfg = _dc("MujocoBaseCfg", _CVPO_MUJOCO, base)
+        for nm, over in _CVPO_MUJOCO_CLASSES:
+            setattr(m, nm, _dc(nm, over, mj))
+        return m
     mj = _dc("MujocoBaseCfg", _ON_MUJOCO if key in ("ppol", "cpo", "trpol", "focops") else _OFF_MUJOCO, base)
     m.MujocoBaseCfg = mj
     for nm, ep in (("Mujoco2MCfg", 100), ("Mujoco10MCfg", 500), ("Mujoco20MCfg", 1000)):
@@ -81,6 +102,6 @@ def _module(key: str) -> types.ModuleType:
     return m
 
 
-ppol_cfg, cpo_cfg, sacl_cfg, ddpgl_cfg, trpol_cfg, focops_cfg = (
-    _module(k) for k in ("ppol", "cpo", "sacl", "ddpgl", "trpol", "focops"))
+ppol_cfg, cpo_cfg, sacl_cfg, ddpgl_cfg, trpol_cfg, focops_cfg, cvpo_cfg = (
+    _module(k) for k in ("ppol", "cpo", "sacl", "ddpgl", "trpol", "focops", "cvpo"))
 focosp_cfg = focops_cfg

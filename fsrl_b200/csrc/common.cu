@@ -61,6 +61,7 @@ extern "C" size_t fsrl_abi_sizeof(int which) {
         case 7: return sizeof(fsrl_eng_input_t);
         case 8: return sizeof(fsrl_offpolicy_t);
         case 9: return sizeof(fsrl_cpo_t);
+        case 10: return sizeof(fsrl_cvpo_t);
         default: return 0;
     }
 }

@@ -11,12 +11,9 @@
 // One call runs `n_steps` complete gradient steps back to back (the loop of
 // OffpolicyTrainer.policy_update_fn, offpolicy.py:102-104) without returning to the host.
 #include "arena.cuh"
-#include "fsrl_b200.h"
+#include "offpolicy.cuh"
 
 namespace fsrl {
-
-constexpr int OD_LD = 16;    // row stride of the engine's out / dout scratch
-constexpr uint32_t KEY_UPD = 0x55504454u;   // 'UPDT': noise stream of the update's rsample()
 
 // ---- n-step bookkeeping (base_policy.py:481-493, :552-566) --------------------------------------
 // For each sampled transition: walk buffer.next() n_step-1 times, accumulate the discounted
@@ -255,10 +252,12 @@ __global__ void alpha_step_kernel(const fsrl_offpolicy_t d, const float* __restr
     stat_out[FSRL_OFF_ST_ALPHA] = expf(nla);
 }
 
-static inline fsrl_eng_input_t mk_in(const float* xa, const int* ia, int Da, const float* xb, const int* ib, int Db) {
-    fsrl_eng_input_t in;
-    in.xa = xa; in.ia = ia; in.xb = xb; in.ib = ib; in.Da = Da; in.Db = Db;
-    return in;
+void launch_nstep_target(const fsrl_offpolicy_t& d, int B, cudaStream_t s) {
+    sac_target_kernel<<<(B + 127) / 128, 128, 0, s>>>(d, B);
+}
+
+void launch_critic_grad(const fsrl_offpolicy_t& d, int B, float* stat, cudaStream_t s) {
+    critic_grad_kernel<<<(B + 127) / 128, 128, 0, s>>>(d, B, stat);
 }
 
 }  // namespace fsrl
@@ -323,14 +322,14 @@ extern "C" int fsrl_offpolicy_steps(const fsrl_offpolicy_t* d, const int* idx_al
             FSRL_LAUNCH_CHECK();
             fsrl_eng_input_t inq = mk_in(d->b_obs_next, d->w_term_idx, D, d->w_act_next, nullptr, A);
             OFF_CHECK(fsrl_engine_forward(&d->eng, &d->critics_old, &inq, B, 0, stream));
-            sac_target_kernel<<<G, T, 0, s>>>(*d, B);
+            launch_nstep_target(*d, B, s);
             FSRL_LAUNCH_CHECK();
         }
         // ---- critics_loss (sac_lag.py:185-210 / ddpg_lag.py:165-189) ---------------------------------
         {
             fsrl_eng_input_t in = mk_in(d->b_obs, idx, D, d->b_act, idx, A);
             OFF_CHECK(fsrl_engine_forward(&d->eng, &d->critics, &in, B, 1, stream));
-            critic_grad_kernel<<<G, T, 0, s>>>(*d, B, stat);
+            launch_critic_grad(*d, B, stat, s);
             FSRL_LAUNCH_CHECK();
             OFF_CHECK(fsrl_engine_backward(&d->eng, &d->critics, B, 0, stream));
             OFF_CHECK(fsrl_engine_wgrad(&d->eng, &d->critics, &in, B, 0, nullptr, stream));

@@ -96,7 +96,7 @@ rollout_step_kernel(const fsrl_rollout_t a) {
             // tianshou ActorProb, state-independent sigma (collect_dataset.py:199-214)
             mu[j] = a.bounded ? a.max_action * tanhf(out[j]) : out[j];
             sig[j] = expf(__ldg(a.log_sigma + j));
-        } else if (a.head == FSRL_HEAD_GAUSS_COND) {
+        } else if (a.head == FSRL_HEAD_GAUSS_COND || a.head == FSRL_HEAD_GAUSS_COND_RAW) {
             mu[j] = a.bounded ? a.max_action * tanhf(out[j]) : out[j];
             sig[j] = expf(fminf(fmaxf(out[A + j], a.sigma_min), a.sigma_max));
         } else {   // FSRL_HEAD_DETERMINISTIC (tianshou Actor): max_action * tanh(logits)
@@ -118,8 +118,8 @@ rollout_step_kernel(const fsrl_rollout_t a) {
             act[j] = sq;
         }
         logp = lp;
-    } else if (a.head == FSRL_HEAD_GAUSS_INDEP && a.mode != FSRL_MODE_RANDOM) {
-        // Independent(Normal(mu, sigma), 1).log_prob(act)  (ppo_lag.py:148)
+    } else if ((a.head == FSRL_HEAD_GAUSS_INDEP || a.head == FSRL_HEAD_GAUSS_COND_RAW) && a.mode != FSRL_MODE_RANDOM) {
+        // Independent(Normal(mu, sigma), 1).log_prob(act)  (ppo_lag.py:148; CVPO, cvpo.py:245, no squash)
         float lp = 0.f;
 #pragma unroll
         for (int j = 0; j < A; ++j) {

@@ -6,6 +6,7 @@ from .ddpg_lag import DDPGLagrangian, GaussianNoise
 from .cpo import CPO
 from .trpo_lag import TRPOLagrangian
 from .focops import FOCOPS
+from .cvpo import CVPO
 
 __all__ = ["ActorCritic", "BasePolicy", "DeviceBatch", "LagrangianPolicy", "PPOLagrangian",
-           "SACLagrangian", "DDPGLagrangian", "GaussianNoise", "CPO", "TRPOLagrangian", "FOCOPS"]
+           "SACLagrangian", "DDPGLagrangian", "GaussianNoise", "CPO", "TRPOLagrangian", "FOCOPS", "CVPO"]

@@ -1,5 +1,7 @@
-"""Shared device machinery of the off-policy Lagrangian learners (SAC / DDPG): engine context,
-work arrays, descriptor for csrc/offpolicy.cu, batched gradient steps.
+"""Shared device machinery of the off-policy learners: ``OffPolicyEngine`` holds what SAC, DDPG and CVPO
+all need (engine context, work arrays, replay-buffer half of the csrc/offpolicy.cu descriptor, batch-index
+sampling, n-step returns); ``OffPolicyLagrangian`` adds the PID-Lagrangian multiplier and the batched gradient
+steps of SAC / DDPG.
 
 Reference call path being replaced: OffpolicyTrainer.policy_update_fn
 (fsrl/trainer/offpolicy.py:93-106) -> BasePolicy.update (base_policy.py:332-355) ->
@@ -18,10 +20,11 @@ from .. import _lib
 from ..data.batch import Batch
 from ..engine import EngineCtx
 from ..nets import SIGMA_MAX, SIGMA_MIN
+from .base_policy import BasePolicy
 from .lagrangian_base import LagrangianPolicy
 
 
-class OffPolicyLagrangian(LagrangianPolicy):
+class OffPolicyEngine(BasePolicy):
     _algo = _lib.ALGO_SAC
 
     def _init_offpolicy(self, tau, n_step, actor_lr, critic_lr):
@@ -47,7 +50,7 @@ class OffPolicyLagrangian(LagrangianPolicy):
         if self._eng is None or self._eng.bmax < bmax:
             self._eng = EngineCtx(self.arena, max(bmax, 256))
             B, dev = self._eng.bmax, self.device
-            A = self.arena.slots[0].out if self._algo == _lib.ALGO_DDPG else self.arena.slots[0].out // 2
+            A = int(self.actor.output_dim)
             self._A = A
             self._w = dict(
                 term_idx=torch.zeros(B, dtype=torch.int32, device=dev),
@@ -61,7 +64,11 @@ class OffPolicyLagrangian(LagrangianPolicy):
                 logp=torch.zeros(B, dtype=torch.float32, device=dev),
                 keep=torch.zeros((B, 24), dtype=torch.float32, device=dev),
             )
+            self._alloc_work(B)
         return self._eng
+
+    def _alloc_work(self, bmax: int) -> None:
+        pass
 
     def _descriptor(self, buffer) -> "_lib.OffPolicy":
         eng = self._eng
@@ -78,7 +85,6 @@ class OffPolicyLagrangian(LagrangianPolicy):
         d.twin = int(self._twin)
         d.n_step = self._n_step
         d.bounded = int(not getattr(self.actor, "_unbounded", False))
-        d.use_lagrangian = int(self.use_lagrangian and self.critics_num > 1)
         d.seed = self._upd_seed
         d.gamma, d.tau = self._gamma, self.tau
         # learning rates are read from the caller's optimizers every time (an lr scheduler stepping them takes effect); the
@@ -98,9 +104,8 @@ class OffPolicyLagrangian(LagrangianPolicy):
         d.max_action = float(self.actor._max)
         d.sigma_min, d.sigma_max = SIGMA_MIN, SIGMA_MAX
         d.tanh_eps = float(np.finfo(np.float32).eps)
-        lags = self.lagrangians()
-        d.lagrangian = lags[0] if lags else 0.0
-        d.rescaling = self.rescaling_factor() if self.use_lagrangian else 1.0
+        d.rescaling = 1.0
+        self._fill_lagrangian(d)
         d.b_obs, d.b_obs_next, d.b_act = buffer.obs.data_ptr(), buffer.obs_next.data_ptr(), buffer.act.data_ptr()
         d.b_rew, d.b_cost = buffer.rew.data_ptr(), buffer.cost.data_ptr()
         d.b_term, d.b_trunc = buffer.terminated.data_ptr(), buffer.truncated.data_ptr()
@@ -128,6 +133,9 @@ class OffPolicyLagrangian(LagrangianPolicy):
         return d
 
     def _fill_algo(self, d) -> None:
+        pass
+
+    def _fill_lagrangian(self, d) -> None:
         pass
 
     # ---- reference hooks ---------------------------------------------------------------------------------
@@ -180,24 +188,36 @@ class OffPolicyLagrangian(LagrangianPolicy):
         batch.rets = torch.stack(rets, dim=-1)
         return batch
 
+
+    # ---- batched gradient steps: one C call per chunk, parameterised by the learner --------------------------
+    _stats_width = _lib.OFF_STATS
+
+    def _run_steps(self, buffer, idx: torch.Tensor, n: int, batch_size: int, stats: torch.Tensor) -> None:
+        d = self._descriptor(buffer)
+        _lib.check(_lib.lib.fsrl_offpolicy_steps(ctypes.byref(d), idx.data_ptr(), n, int(batch_size), self._critic_t,
+                                                 self._actor_t, self._noise_t, stats.data_ptr(), self._stream()))
+
+    def _engine_rows(self, batch_size: int) -> int:
+        return batch_size
+
+    def _actor_steps_per_update(self) -> int:
+        return 1
+
     def update_many(self, n_updates: int, batch_size: int, buffer, chunk: int = 4096) -> None:
         """`n_updates` x policy.update(batch_size, buffer) without returning to Python per step."""
         if buffer is None or n_updates <= 0:
             return
-        self._ensure_engine(batch_size)
+        self._ensure_engine(self._engine_rows(batch_size))
         self.updating = True
         stats_all = []
         done = 0
         while done < n_updates:
             n = min(chunk, n_updates - done)
             idx = self.sample_batch_indices(buffer, n, batch_size)
-            stats = torch.zeros((n, _lib.OFF_STATS), dtype=torch.float32, device=self.device)
-            d = self._descriptor(buffer)
+            stats = torch.zeros((n, self._stats_width), dtype=torch.float32, device=self.device)
             with torch.cuda.device(self.device):
-                _lib.check(_lib.lib.fsrl_offpolicy_steps(ctypes.byref(d), idx.data_ptr(), n, int(batch_size),
-                                                         self._critic_t, self._actor_t, self._noise_t,
-                                                         stats.data_ptr(), self._stream()))
-            self._critic_t += n; self._actor_t += n; self._noise_t += n
+                self._run_steps(buffer, idx, n, batch_size, stats)
+            self._critic_t += n; self._actor_t += n * self._actor_steps_per_update(); self._noise_t += n
             self.gradient_steps += n
             stats_all.append(stats)
             done += n
@@ -213,6 +233,17 @@ class OffPolicyLagrangian(LagrangianPolicy):
 
     def learn(self, batch, **kwargs):
         raise RuntimeError("off-policy learners are driven through update()/update_many() on the device")
+
+    def _log_stats(self, st: np.ndarray) -> None:
+        raise NotImplementedError
+
+
+class OffPolicyLagrangian(OffPolicyEngine, LagrangianPolicy):
+    def _fill_lagrangian(self, d) -> None:
+        d.use_lagrangian = int(self.use_lagrangian and self.critics_num > 1)
+        lags = self.lagrangians()
+        d.lagrangian = lags[0] if lags else 0.0
+        d.rescaling = self.rescaling_factor() if self.use_lagrangian else 1.0
 
     def _log_stats(self, st: np.ndarray) -> None:
         resc = self.rescaling_factor() if self.use_lagrangian else 1.0

@@ -77,7 +77,10 @@ typedef struct fsrl_mlp3 {
  * (base_policy.py:226-256), env.step, cost extraction, buffer.add and the episode
  * bookkeeping incl. the surplus-env rule (:357-363), for all ready envs, on the device. */
 enum { FSRL_MODE_TRAIN = 0, FSRL_MODE_EVAL = 1, FSRL_MODE_RANDOM = 2 };
-enum { FSRL_HEAD_GAUSS_INDEP = 0, FSRL_HEAD_GAUSS_COND = 1, FSRL_HEAD_DETERMINISTIC = 2 };
+/* GAUSS_COND is SAC's tanh-squashed head; GAUSS_COND_RAW is the same conditioned-sigma Gaussian
+ * without the squash (CVPO: act = mu + sigma*eps, logp = Independent(Normal(mu, sigma)).log_prob(act)) */
+enum { FSRL_HEAD_GAUSS_INDEP = 0, FSRL_HEAD_GAUSS_COND = 1, FSRL_HEAD_DETERMINISTIC = 2,
+       FSRL_HEAD_GAUSS_COND_RAW = 3 };
 enum { FSRL_BOUND_NONE = 0, FSRL_BOUND_CLIP = 1, FSRL_BOUND_TANH = 2 };
 enum { FSRL_ENV_CAR_CIRCLE = 0, FSRL_ENV_CAR_RUN = 1, FSRL_ENV_BALL_CIRCLE = 2,
        FSRL_ENV_BALL_RUN = 3, FSRL_ENV_ANT_CIRCLE = 4, FSRL_ENV_POINT_GOAL = 5 };
@@ -317,6 +320,45 @@ int fsrl_nstep_prepare(const fsrl_offpolicy_t* d, const int* idx, int B, void* s
 int fsrl_offpolicy_steps(const fsrl_offpolicy_t* d, const int* idx_all, int n_steps, int B,
                          long long critic_t0, long long actor_t0, unsigned long long noise_t0,
                          float* stats, void* stream);
+
+/* ---- f4: CVPO gradient steps ------------------------------------------------------------------------
+ * fsrl_cvpo_steps runs n_steps iterations of CVPO.update (fsrl/policy/cvpo.py:206-430): n-step targets
+ * with an unsquashed sample of the CURRENT actor and min-over-heads critics_old (:206-222), critic
+ * regression (:248-276), E-step on K particles of actor_old scored by the just-updated critics (dual
+ * Adam, clamp, softmax weights; :320-363, including the in-place `combined_q -=` of :284 that keeps
+ * subtracting lambda*q_c from q_r), mstep_iters M-steps (weighted MLE + decoupled KL with the dual
+ * Adam and the clip of its uses; :369-418), Polyak of critics_old (:201-204).  No host sync: every dual
+ * and its Adam moments live in the device arrays below.  `off` carries the engine, the net lists
+ * (actor, actor_old, critics, critics_old), the replay ring and the n-step work arrays; off.use_alpha
+ * must be 0.  Single GPU (off.world <= 1), C <= 2, A <= 8, K*B <= off.eng.bmax.
+ *   estep_state [8]: eta, lambda, adam m[2], adam v[2], adam step, -   (persists for the policy's life)
+ *   mstep_state [8]: dual_mu, dual_std, adam m[2], adam v[2], adam step, -   (zeroed by pre_update_fn)
+ *   particles [K*B][A], part_idx [K*B], mu_old / std_old [B][A], comb / weights [K*B]: work arrays
+ *   log_sigma / log_sigma_old: sigma_param [A] of the actor / actor_old (the nets' extra parameter)
+ *   when cond_sigma == 0, NULL otherwise
+ * stats: [n_steps][FSRL_CVPO_STATS] (zeroed by the caller), columns FSRL_CVPO_ST_*; the
+ * last E-step / M-step iteration of a step is reported (the reference logs every iteration). */
+#define FSRL_CVPO_STATS 16
+enum { FSRL_CVPO_ST_Q0 = 0, FSRL_CVPO_ST_Q1 = 1, FSRL_CVPO_ST_VAL_Q0 = 2, FSRL_CVPO_ST_VAL_Q1 = 3,
+       FSRL_CVPO_ST_ESTEP_LOSS = 4, FSRL_CVPO_ST_DUAL0 = 5, FSRL_CVPO_ST_DUAL1 = 6, FSRL_CVPO_ST_KL_MU = 7,
+       FSRL_CVPO_ST_KL_STD = 8, FSRL_CVPO_ST_LOSS_KL = 9, FSRL_CVPO_ST_LOSS_MLE = 10, FSRL_CVPO_ST_LOSS_TOTAL = 11,
+       FSRL_CVPO_ST_DUAL_MU = 12, FSRL_CVPO_ST_DUAL_STD = 13, FSRL_CVPO_ST_ENTROPY = 14 };
+typedef struct fsrl_cvpo {
+    fsrl_offpolicy_t off;
+    int K, estep_iters, mstep_iters, cond_sigma;
+    float estep_kl, estep_dual_max, estep_dual_lr, qc_thres;
+    float mstep_kl_mu, mstep_kl_std, mstep_dual_max, mstep_dual_lr;
+    float* estep_state;
+    float* mstep_state;
+    float* particles;
+    int* part_idx;
+    float *mu_old, *std_old, *comb, *weights;
+    const float *log_sigma, *log_sigma_old;
+} fsrl_cvpo_t;
+
+int fsrl_cvpo_steps(const fsrl_cvpo_t* d, const int* idx_all, int n_steps, int B,
+                    long long critic_t0, long long actor_t0, unsigned long long noise_t0, float* stats,
+                    void* stream);
 
 /* ---- a11: CPO (and the CG / Fisher machinery TRPO-Lag shares) ------------------------------------
  * Replaces CPO._get_objective/_get_cost_surrogate/_MVP/_conjugate_gradients/policy_loss
