@@ -400,8 +400,8 @@ __device__ __forceinline__ float4 wg_reduced4(const float* red, int m, int n4) {
     return s4;
 }
 
-// Device-wide barrier for co-resident grids (cooperative launch): monotonically increasing ticket
-// counter, one arrival per CTA, spin on an acquire load.
+// Device-wide barrier for a grid whose CTAs are all resident at once (ordinary launch, see ppo_launch_minibatch):
+// monotonically increasing ticket counter, one arrival per CTA, spin on an acquire load.
 __device__ __forceinline__ void grid_barrier(unsigned long long* counter, unsigned long long target) {
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -913,20 +913,16 @@ static int adam_plain_blocks(const fsrl_ppo_update_t& u, int H) {
     return (int)((plain + 255) / 256);
 }
 
-// One link of the per-minibatch kernel chain: programmatic dependent launch (see pdl_wait), plus
-// the cooperative attribute for the kernel that contains the grid barrier.
+// One link of the per-minibatch kernel chain: programmatic dependent launch (see pdl_wait).
 template <class... KArgs, class... Args>
 static cudaError_t launch_chain(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
-                                bool cooperative, Args... args) {
+                                Args... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
-    cudaLaunchAttribute at[2];
-    int n = 0;
-    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-    if (cooperative) { at[n].id = cudaLaunchAttributeCooperative; at[n].val.cooperative = 1; ++n; }
-    cfg.attrs = at; cfg.numAttrs = n;
+    cudaLaunchAttribute at;
+    at.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at.val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = &at; cfg.numAttrs = 1;
     ++g_launches;
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
@@ -947,8 +943,8 @@ static int ppo_launch_minibatch(const fsrl_ppo_update_t& u, int mb_off, int B, i
         setB = smemB;
     }
     const dim3 gA((B + TT::R - 1) / TT::R, H / SLAB_NS, u.n_nets);
-    FSRL_CUDA(launch_chain(ppo_fwd_kernel<H>, gA, dim3(MLP_TPB), smemF, s, false, u, mb_off, B));
-    FSRL_CUDA(launch_chain(ppo_bwd_kernel<H>, gA, dim3(MLP_TPB), smemB, s, false, u, mb_off, B, slot));
+    FSRL_CUDA(launch_chain(ppo_fwd_kernel<H>, gA, dim3(MLP_TPB), smemF, s, u, mb_off, B));
+    FSRL_CUDA(launch_chain(ppo_bwd_kernel<H>, gA, dim3(MLP_TPB), smemB, s, u, mb_off, B, slot));
     constexpr int NTT = H / WG_T;
     const dim3 gB((H / WG_TKT) * NTT + 2 * NTT, u.n_nets);
     const size_t smemW = sizeof(float) * WG_SMEM_FLOATS;
@@ -971,7 +967,7 @@ static int ppo_launch_minibatch(const fsrl_ppo_update_t& u, int mb_off, int B, i
         // waiting on anything but the barrier (the preceding bwd CTAs drain unconditionally, the next fwd
         // CTAs are only scheduled after ALL of these have triggered), and grid_barrier traps after 20 s
         // instead of spinning forever should that reasoning ever be violated.
-        FSRL_CUDA(launch_chain(ppo_wgrad_adam_kernel<H>, gB, dim3(WG_TPB), smemW, s, false, u, mb_off, B, ad, u.barrier,
+        FSRL_CUDA(launch_chain(ppo_wgrad_adam_kernel<H>, gB, dim3(WG_TPB), smemW, s, u, mb_off, B, ad, u.barrier,
                                target, slot));
         return FSRL_OK;
     }
@@ -980,11 +976,11 @@ static int ppo_launch_minibatch(const fsrl_ppo_update_t& u, int mb_off, int B, i
         const unsigned long long id = (unsigned long long)adam_t;
         fsrl_ppo_update_t ux = u;
         ux.grad = const_cast<float*>(u.p2p_xg[id & 1ULL][u.p2p_rank]);
-        FSRL_CUDA(launch_chain(ppo_wgrad_kernel<H>, gB, dim3(WG_TPB), smemW, s, false, ux, mb_off, B));
+        FSRL_CUDA(launch_chain(ppo_wgrad_kernel<H>, gB, dim3(WG_TPB), smemW, s, ux, mb_off, B));
         const unsigned nblk = (unsigned)((u.n_params + 1023) / 1024);
-        FSRL_CUDA(launch_chain(ppo_dp_reduce_kernel, dim3(nblk), dim3(256), (size_t)0, s, false, u, id));
+        FSRL_CUDA(launch_chain(ppo_dp_reduce_kernel, dim3(nblk), dim3(256), (size_t)0, s, u, id));
     } else {
-    FSRL_CUDA(launch_chain(ppo_wgrad_kernel<H>, gB, dim3(WG_TPB), smemW, s, false, u, mb_off, B));
+    FSRL_CUDA(launch_chain(ppo_wgrad_kernel<H>, gB, dim3(WG_TPB), smemW, s, u, mb_off, B));
     }
     if (u.world > 1 && !u.p2p_on) {
         // data parallel: ONE all-reduce of the flat gradient buffer per optimiser step, then the
@@ -996,7 +992,7 @@ static int ppo_launch_minibatch(const fsrl_ppo_update_t& u, int mb_off, int B, i
     }
     const int n_plain = adam_plain_blocks(u, H);
     const int n_tiles = u.n_nets * (H / 32) * (H / 32);
-    FSRL_CUDA(launch_chain(adam_kernel, dim3(n_plain + n_tiles), dim3(256), (size_t)0, s, false, u, ad, slot, n_plain));
+    FSRL_CUDA(launch_chain(adam_kernel, dim3(n_plain + n_tiles), dim3(256), (size_t)0, s, u, ad, slot, n_plain));
     return FSRL_OK;
 }
 

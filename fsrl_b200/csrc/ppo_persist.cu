@@ -31,7 +31,9 @@
 // rows through shared memory behind one 64-thread barrier per warp pair (stage_acc).
 // The 8 CTAs of a row block form a thread-block cluster: operand chunks that several of them need are multicast
 // from L2 once into all of them (copy_operand), their head partials travel over distributed shared memory
-// (st.async + mbarrier complete_tx); all other hops are flag lines in L2.  The cross terms of the 3-term split
+// (st.async + mbarrier complete_tx); all other hops are flag lines in L2.  The grid is launched as clusters only: the
+// gate (ppo_persist_supported) admits a shape only when all 4 x n_nets clusters can be co-resident, and everything it
+// rejects runs on the three-launch chain of ppo.cu.  The cross terms of the 3-term split
 // accumulate in their own registers.  With world > 1 the <DP = true> instantiation exchanges gradients itself over peer
 // memory (dp_* functions below: tagged + hashed 16-byte packets pushed into the peers' buffers).
 #include "ppo_persist.cuh"
@@ -63,17 +65,16 @@ constexpr int H_ = 256;
 constexpr int IMG = 65536;               // floats per image (256 x 256)
 enum { I_H1A_HI, I_H1A_LO, I_H1T_HI, I_H1T_LO, I_DZA_HI, I_DZA_LO, I_DZT_HI, I_DZT_LO, I_W2A_HI, I_W2A_LO, I_W2B_HI, I_W2B_LO, N_IMG };
 // per-network partial buffers (floats)
-constexpr int HEADP_OFF = N_IMG * IMG;                          // [4 a][8 b][64 r][OUTP]
-constexpr int DB2P_OFF = HEADP_OFF + 4 * 8 * 64 * OUTP;         // [4 a][H]
+constexpr int DB2P_OFF = N_IMG * IMG;                           // [4 a][H]
 constexpr int DW3P_OFF = DB2P_OFF + 4 * H_;                     // [4 a][H][OUTP]
 constexpr int DB3P_OFF = DW3P_OFF + 4 * H_ * OUTP;              // [4 a][16]
 constexpr int DW1P_OFF = DB3P_OFF + 4 * 16;                     // [4 rb][MAXD + 1][H]
 constexpr int MAXD = 40;
 constexpr int NET_WS = DW1P_OFF + 4 * WQ * (MAXD + 1) * H_;   // [row block 4][warp-in-subpartition WQ][MAXD + 1][H]
 constexpr int SUMSQ_FLOATS = 128;                               // global tail: per-CTA sums of squares
-// flag lines (32 unsigned each): per net A, C, D1, B[4]; global D2
+// flag lines (32 unsigned each): per net A, C, D1; global D2
 constexpr int FLAG_LINE = 32;
-constexpr int F_A = 0, F_C = 1, F_D1 = 2, F_B = 3, F_PER_NET = 7;
+constexpr int F_A = 0, F_C = 1, F_D1 = 2, F_PER_NET = 3;
 // The two cross terms a_lo b_hi + a_hi b_lo accumulate in their OWN registers and meet the a_hi b_hi sum only in the
 // epilogue: the cross terms are 2^-11 of the main ones, and a tensor-core accumulator add may drop low bits of a small
 // addend.  Same MMA count, 8 more accumulator registers per instruction column.
@@ -91,7 +92,6 @@ constexpr int TILE_PK = (64 * 64 / NEPI + 2) / 3;                // packets per 
 constexpr int TILE_FLOATS = TILE_PK * NEPI * 4;                  // [packet][thread][4]
 constexpr int SLICE_PK = (NSMAX + 2) / 3;
 constexpr int XG_PER_NET = 16 * TILE_FLOATS + 8 * SLICE_PK * 4;
-constexpr int XG_FLAG_FLOATS = 8 * 128 * 2;                      // (reserved: flag lines of the fenced protocol)
 constexpr int MAX_MB = 16384;                                    // minibatches per launch (Adam scalar table)
 constexpr long long WAIT_CYCLES = 6000000000LL;                  // ~3 s: a lost partner must not hang the GPU
 
@@ -105,7 +105,6 @@ struct Args {
     const float* adam_tab;   // [n_mb][2]: 1 / sqrt(1 - beta2^t), -(lr / (1 - beta1^t)) of every step (host doubles -> f32)
     long long* dbg;          // optional [n_cta][DBG_N] clock stamps of step dbg_step
     int dbg_step;
-    int cluster;             // launched as clusters of 8 CTAs (one row block): hop B runs over distributed shared memory
     unsigned dp_seq;         // data-parallel runs: launch sequence number (same on every rank), upper half of the packet tags
     int dp_direct;           // W2 gradient tiles exchanged in one hop (2 ranks) instead of the two-hop owner scheme
 };
@@ -249,11 +248,12 @@ __device__ __forceinline__ void acc_st(float* accs, int row, int col, const floa
 // One GEMM of the step, issued by warpgroup 0 alone straight from the operand ring: NCH chunks of KC k, A = 64 rows,
 // B = N rows, full-width m64nNk8 MMAs.  Every output element accumulates over all of K in one register chain, in the
 // same order as with narrower MMAs: the result does not depend on how the columns are cut into instructions.  Each warp
-// releases a slot once its MMAs have read it: lane r < n_dst arrives on the bar_empty of cluster rank r (bar_empty
-// counts the 4 MMA warps of each of the n_dst CTAs whose bulk copies write into the slot).  One group stays in flight.
+// releases a slot once its MMAs have read it: lane r < 8 arrives on the bar_empty of cluster rank r (a CTA's multicast
+// copies write into the slot of all 8, so its bar_empty counts the 4 MMA warps of each of them).  One group stays in
+// flight.
 template <int N>
 __device__ __forceinline__ void gemm_phase(const unsigned char* ring, unsigned& qq, uint64_t* bar_full, uint32_t empty_r,
-                                           int n_dst, float (&dm)[N / 2], float (&dc)[N / 2], int* err, int code, int lane) {
+                                           float (&dm)[N / 2], float (&dc)[N / 2], int* err, int code, int lane) {
 #pragma unroll
     for (int e = 0; e < N / 2; ++e) dm[e] = dc[e] = 0.f;
     const uint32_t ring_a = smem_u32(ring);
@@ -263,13 +263,15 @@ __device__ __forceinline__ void gemm_phase(const unsigned char* ring, unsigned& 
         if (!mbar_wait(&bar_full[s], (qq / NSLOT) & 1, WAIT_CYCLES)) fail(err, code);
         __syncwarp();
         wgmma_fence();
+        // descriptors of the slot's k-step 0; k-step ks starts 2048 (A) / 2 b_lbo (B) bytes further (the address field
+        // holds bytes / 16 and the ring ends far below its 256 KB range, so adding the offset never carries out of it)
         const uint32_t base = ring_a + (uint32_t)s * SLOT_BYTES;
+        const uint64_t ah0 = smem_desc(base, 1024, 128), al0 = smem_desc(base + A_CHUNK, 1024, 128);
+        const uint64_t bh0 = smem_desc(base + 2 * A_CHUNK, b_lbo, 128), bl0 = smem_desc(base + 2 * A_CHUNK + b_chunk, b_lbo, 128);
 #pragma unroll
         for (int ks = 0; ks < KC / 8; ++ks) {
-            const uint64_t ah = smem_desc(base + ks * 2048, 1024, 128);
-            const uint64_t al = smem_desc(base + A_CHUNK + ks * 2048, 1024, 128);
-            const uint64_t bh = smem_desc(base + 2 * A_CHUNK + ks * 2 * b_lbo, b_lbo, 128);
-            const uint64_t bl = smem_desc(base + 2 * A_CHUNK + ks * 2 * b_lbo + b_chunk, b_lbo, 128);
+            const uint64_t ah = ah0 + ks * (2048 / 16), al = al0 + ks * (2048 / 16);
+            const uint64_t bh = bh0 + ks * (2 * b_lbo / 16), bl = bl0 + ks * (2 * b_lbo / 16);
             if constexpr (N == 32) {
                 mma_m64n32k8_tf32(dc, al, bh);
                 mma_m64n32k8_tf32(dc, ah, bl);
@@ -284,13 +286,13 @@ __device__ __forceinline__ void gemm_phase(const unsigned char* ring, unsigned& 
         if (j > 0) {
             wgmma_wait<1>();
             __syncwarp();
-            if (lane < n_dst) mbar_arrive_cluster(empty_r + 8 * ((qq - 1) % NSLOT));
+            if (lane < 8) mbar_arrive_cluster(empty_r + 8 * ((qq - 1) % NSLOT));
         }
     }
     wgmma_wait<0>();
     reg_fence(dm); reg_fence(dc);
     __syncwarp();
-    if (lane < n_dst) mbar_arrive_cluster(empty_r + 8 * ((qq - 1) % NSLOT));
+    if (lane < 8) mbar_arrive_cluster(empty_r + 8 * ((qq - 1) % NSLOT));
 }
 // Warp w of warpgroup 0 stages its fragment (main + cross terms, rows 16 w .. + 15, all N columns) into accs; warps w
 // and w + 4 read those rows back in the epilogue, so one 64-thread barrier per warp pair (ids 2 .. 5) orders them.
@@ -548,18 +550,18 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     float* sp_m = small + sm.n;          // Adam first moment
     float* sp_v = small + 2 * sm.n;      // Adam second moment
     float* sp_g = small + 3 * sm.n;      // reduced gradient of the current step
-    float* land = small + 4 * sm.n;      // head partials pushed by the 8 CTAs of this row block [b][64][OUTP] (cluster
-                                         // mode), G2's observation block
+    float* land = small + 4 * sm.n;      // head partials pushed by the 8 CTAs of this row block [b][64][OUTP] (hop B),
+                                         // G2's observation block
 
     if (tid == 0) {
-        for (int i = 0; i < NSLOT; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 4 * (P.cluster ? 8 : 1)); }
+        for (int i = 0; i < NSLOT; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 4 * 8); }
         mbar_init(&bar_b, 1);                // per step: one local expect_tx arrival + 16 KB of remote st.async bytes
         fence_mbar_init();
     }
     __syncthreads();
     if (DP && threadIdx.x < 2 * FSRL_P2P_MAX_RANKS) s_xg[threadIdx.x / FSRL_P2P_MAX_RANKS][threadIdx.x % FSRL_P2P_MAX_RANKS] = P.u.p2p_xg[threadIdx.x / FSRL_P2P_MAX_RANKS][threadIdx.x % FSRL_P2P_MAX_RANKS];
     if (DP) __syncthreads();
-    if (P.cluster) cluster_sync_all();       // every CTA's barriers exist before a peer may arrive on them
+    cluster_sync_all();                      // every CTA's barriers exist before a peer may arrive on them
 
     // parameter offsets of this network inside the flat arena
     const long long pbase = u.net_off[net];
@@ -575,6 +577,8 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 if (!flag_wait_ge<true>(fl_net + F_A * FLAG_LINE, 32u * (t + 1), WAIT_CYCLES)) fail(P.err, 10);
                 STAMP(12);
                 fence_proxy_async();
+                // the producer loops stay rolled: one thread runs them, and the kernel's instruction footprint is tight
+#pragma unroll 1
                 for (int j = 0; j < NCH; ++j, ++qq) {             // G1: K = k in chunks of KC
                     const int s = qq % NSLOT;
                     if (!mbar_wait(&bar_empty[s], ((qq / NSLOT) & 1) ^ 1, WAIT_CYCLES)) fail(P.err, 11);
@@ -582,7 +586,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                     mbar_expect_tx(&bar_full[s], 3 * A_CHUNK);
                     const size_t ao = (size_t)a * 16384 + (size_t)j * 64 * KC, bo = (size_t)b * 8192 + (size_t)j * 32 * KC;
                     // A = H1A block a: the same for the 8 CTAs of the row block (cluster)
-                    copy_operand(dst, wsn + (size_t)I_H1A_HI * IMG + ao, A_CHUNK, &bar_full[s], P.cluster ? 8 : 1, b, 0xff);
+                    copy_operand(dst, wsn + (size_t)I_H1A_HI * IMG + ao, A_CHUNK, &bar_full[s], 8, b, 0xff);
                     copy_operand(dst + 2 * A_CHUNK, wsn + (size_t)I_W2A_HI * IMG + bo, A_CHUNK / 2, &bar_full[s], 1, 0, 0);
                 }
                 STAMP(13);
@@ -591,18 +595,18 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 fence_proxy_async();
                 const int ia = is_g2 ? I_W2B_HI : I_DZT_HI, ib = is_g2 ? I_DZA_HI : I_H1T_HI;
                 const int blk_a = is_g2 ? ka : q4, blk_b = is_g2 ? q4 : ka;
-                // with clusters, the k block ka (G2: A = W2B, G3: B = H1T) is shared by the 4 CTAs with the same b >> 2,
-                // the block q4 (G2: B = DZA, G3: A = DZT) by the CTAs b and b ^ 4
-                const int g4 = P.cluster ? 4 : 1, g2 = P.cluster ? 2 : 1;
+                // the k block ka (G2: A = W2B, G3: B = H1T) is shared by the 4 CTAs with the same b >> 2, the block q4
+                // (G2: B = DZA, G3: A = DZT) by the CTAs b and b ^ 4
                 const uint16_t m4 = (uint16_t)(0xfu << (b & 4)), m2 = (uint16_t)(0x11u << (b & 3));
+#pragma unroll 1
                 for (int j = 0; j < NCH; ++j, ++qq) {             // G2: K = o ; G3: K = r ; chunks of KC
                     const int s = qq % NSLOT;
                     if (!mbar_wait(&bar_empty[s], ((qq / NSLOT) & 1) ^ 1, WAIT_CYCLES)) fail(P.err, 13);
                     unsigned char* dst = ring + (size_t)s * SLOT_BYTES;
                     mbar_expect_tx(&bar_full[s], 4 * A_CHUNK);
                     const size_t ao = (size_t)blk_a * 16384 + (size_t)j * 64 * KC, bo = (size_t)blk_b * 16384 + (size_t)j * 64 * KC;
-                    copy_operand(dst, wsn + (size_t)ia * IMG + ao, A_CHUNK, &bar_full[s], is_g2 ? g4 : g2, is_g2 ? b & 3 : b >> 2, is_g2 ? m4 : m2);
-                    copy_operand(dst + 2 * A_CHUNK, wsn + (size_t)ib * IMG + bo, A_CHUNK, &bar_full[s], is_g2 ? g2 : g4, is_g2 ? b >> 2 : b & 3, is_g2 ? m2 : m4);
+                    copy_operand(dst, wsn + (size_t)ia * IMG + ao, A_CHUNK, &bar_full[s], is_g2 ? 4 : 2, is_g2 ? b & 3 : b >> 2, is_g2 ? m4 : m2);
+                    copy_operand(dst + 2 * A_CHUNK, wsn + (size_t)ib * IMG + bo, A_CHUNK, &bar_full[s], is_g2 ? 2 : 4, is_g2 ? b >> 2 : b & 3, is_g2 ? m2 : m4);
                 }
             }
         }
@@ -616,16 +620,15 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
         const int cb1 = 16 * half + C1 * wq;        // first of this thread's C1 columns of a 32-column tile
         const int cb2 = 32 * half + C2 * wq;        // first of this thread's C2 columns of a 64-column tile
         unsigned qq = 0;                            // operand ring position
-        // ring releases go to every CTA whose bulk copies write into this one's slots: with clusters, all 8 (multicast)
-        const int n_dst = P.cluster ? 8 : 1;
-        const uint32_t empty_r = mapa_u32(smem_u32(bar_empty), lane < n_dst ? lane : 0);
+        // ring releases go to every CTA whose bulk copies write into this one's slots: all 8 of the cluster (multicast)
+        const uint32_t empty_r = mapa_u32(smem_u32(bar_empty), lane < 8 ? lane : 0);
         float w2p[C2], w2m[C2], w2v[C2];            // owned W2 tile (G3 CTAs): parameters and Adam moments
         // ---- data-parallel exchange over peer memory (NVLink): every CTA pushes its local gradient piece into its
         // rank's region of EVERY rank's exchange buffer, one thread fences and release-stores the step id into the same
         // slot of every rank's flag array; the receiver waits for the ranks' flags and sums their pieces from its own
         // memory in rank order -- point-to-point between equal CTAs, one NVLink one-way latency, no remote loads,
         // bit-identical sums on every rank.
-        const int world = (DP && u.world > 1) ? u.world : 1;
+        const int world = DP ? u.world : 1;
         // W2 tiles travel in two hops (reduce-scatter + all-gather, 2 (W - 1) / W tile volumes per rank instead of W - 1):
         // packet q of epilogue warp w is OWNED by rank (6 w + q) mod W -- every rank sends it there, the owner sums the
         // ranks' packets in rank order and pushes the mean into everybody's result region (region 8).  Both hops are
@@ -784,7 +787,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             // ---- G1 (wgmma), then its epilogue: h2 = relu(acc + b2), head partial over this tile's 32 columns ----
             {
                 float dm[16], dc[16];
-                if (wq == 0) gemm_phase<32>(ring, qq, bar_full, empty_r, n_dst, dm, dc, P.err, 30, lane);
+                if (wq == 0) gemm_phase<32>(ring, qq, bar_full, empty_r, dm, dc, P.err, 30, lane);
                 else qq += NCH;
                 stage_acc<32>(accs, dm, dc, wq, sp, lane);
             }
@@ -820,56 +823,32 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             float outv[OUTP];
 #pragma unroll
             for (int jj = 0; jj < OUTP; ++jj) outv[jj] = sp_p[sm.b3 + jj];
-            if (P.cluster) {
-                // hop B inside the cluster (8 CTAs = the column blocks of this row block): push the partial rows into every
-                // peer's landing zone, one remote mbarrier arrival per peer, then wait for the 8 arrivals on the own barrier
-                if (et == 0) {
-                    STAMP(3);
-                    mbar_expect_tx(&bar_b, 8u * 64u * OUTP * (uint32_t)sizeof(float));
-                }
-                if (half == 0 && wq == 0) {
-                    const uint32_t mine = smem_u32(land + ((size_t)b * 64 + trow) * OUTP);
-                    const uint32_t bb_ = smem_u32(&bar_b);
+            // hop B inside the cluster (8 CTAs = the column blocks of this row block): push the partial rows into every
+            // peer's landing zone, one remote mbarrier arrival per peer, then wait for the 8 arrivals on the own barrier
+            if (et == 0) {
+                STAMP(3);
+                mbar_expect_tx(&bar_b, 8u * 64u * OUTP * (uint32_t)sizeof(float));
+            }
+            if (half == 0 && wq == 0) {
+                const uint32_t mine = smem_u32(land + ((size_t)b * 64 + trow) * OUTP);
+                const uint32_t bb_ = smem_u32(&bar_b);
 #pragma unroll
-                    for (int r = 0; r < 8; ++r) {
-                        const uint32_t ra = mapa_u32(mine, r), rb = mapa_u32(bb_, r);
-                        st_async4(ra, make_float4(hp[0], hp[1], hp[2], hp[3]), rb);
-                        st_async4(ra + 16, make_float4(hp[4], hp[5], hp[6], hp[7]), rb);
-                    }
+                for (int r = 0; r < 8; ++r) {
+                    const uint32_t ra = mapa_u32(mine, r), rb = mapa_u32(bb_, r);
+                    st_async4(ra, make_float4(hp[0], hp[1], hp[2], hp[3]), rb);
+                    st_async4(ra + 16, make_float4(hp[4], hp[5], hp[6], hp[7]), rb);
                 }
-                if (!mbar_wait_cluster(&bar_b, t & 1, WAIT_CYCLES)) fail(P.err, 31);
-                __syncwarp();
-                if (et == 0) STAMP(4);
+            }
+            if (!mbar_wait_cluster(&bar_b, t & 1, WAIT_CYCLES)) fail(P.err, 31);
+            __syncwarp();
+            if (et == 0) STAMP(4);
 #pragma unroll
-                for (int bb = 0; bb < 8; ++bb) {
-                    const float* src = land + ((size_t)bb * 64 + trow) * OUTP;
-                    const float4 v0 = *reinterpret_cast<const float4*>(src);
-                    const float4 v1 = *reinterpret_cast<const float4*>(src + 4);
-                    outv[0] += v0.x; outv[1] += v0.y; outv[2] += v0.z; outv[3] += v0.w;
-                    outv[4] += v1.x; outv[5] += v1.y; outv[6] += v1.z; outv[7] += v1.w;
-                }
-            } else {
-                if (half == 0 && wq == 0) {
-                    float* dst = wsn + HEADP_OFF + ((size_t)(a * 8 + b) * 64 + trow) * OUTP;
-                    *reinterpret_cast<float4*>(dst) = make_float4(hp[0], hp[1], hp[2], hp[3]);
-                    *reinterpret_cast<float4*>(dst + 4) = make_float4(hp[4], hp[5], hp[6], hp[7]);
-                }
-                epi_bar();
-                if (et == 0) {
-                    STAMP(3);
-                    flag_add_release(fl_net + (F_B + a) * FLAG_LINE);
-                    if (!flag_wait_ge(fl_net + (F_B + a) * FLAG_LINE, 8u * (t + 1), WAIT_CYCLES)) fail(P.err, 31);
-                    STAMP(4);
-                }
-                epi_bar();
-#pragma unroll
-                for (int bb = 0; bb < 8; ++bb) {
-                    const float* src = wsn + HEADP_OFF + ((size_t)(a * 8 + bb) * 64 + trow) * OUTP;
-                    const float4 v0 = __ldcg(reinterpret_cast<const float4*>(src));
-                    const float4 v1 = __ldcg(reinterpret_cast<const float4*>(src + 4));
-                    outv[0] += v0.x; outv[1] += v0.y; outv[2] += v0.z; outv[3] += v0.w;
-                    outv[4] += v1.x; outv[5] += v1.y; outv[6] += v1.z; outv[7] += v1.w;
-                }
+            for (int bb = 0; bb < 8; ++bb) {
+                const float* src = land + ((size_t)bb * 64 + trow) * OUTP;
+                const float4 v0 = *reinterpret_cast<const float4*>(src);
+                const float4 v1 = *reinterpret_cast<const float4*>(src + 4);
+                outv[0] += v0.x; outv[1] += v0.y; outv[2] += v0.z; outv[3] += v0.w;
+                outv[4] += v1.x; outv[5] += v1.y; outv[6] += v1.z; outv[7] += v1.w;
             }
             // ---- loss gradient at the head (ppo_lag.py:152-212): dd[j] = d loss / d head_j --------------
             float dd[16];
@@ -997,7 +976,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             }
             {
                 float dm[32], dc[32];
-                if (wq == 0) gemm_phase<64>(ring, qq, bar_full, empty_r, n_dst, dm, dc, P.err, 32, lane);
+                if (wq == 0) gemm_phase<64>(ring, qq, bar_full, empty_r, dm, dc, P.err, 32, lane);
                 else qq += NCH;
                 stage_acc<64>(accs, dm, dc, wq, sp, lane);
             }
@@ -1032,7 +1011,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             } else {
                 float g[C2];
                 acc_ld<C2>(accs, trow, cb2, g);
-                if (DP && world > 1) {
+                if (DP) {
                     dp_tile_send(dp_ctx(t), (size_t)(net * 16 + (c - 16)) * TILE_FLOATS + (size_t)et * 4, accs, trow, cb2, et);
                     if (et == 0) STAMP(32);
                 } else {
@@ -1086,7 +1065,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             if (et == 0) { STAMP(7); if (!flag_wait_ge(fl_net + F_D1 * FLAG_LINE, 16u * (t + 1), WAIT_CYCLES)) fail(P.err, 33); STAMP(8); }
             epi_bar();
             reduce_slices(0, sm.b2);
-            if (DP && world > 1) {
+            if (DP) {
                 const DpCtx d = dp_ctx(t);
                 const size_t off_t = (size_t)(net * 16 + (c - 16)) * TILE_FLOATS + (size_t)et * 4;
                 epi_bar();                                    // sp_g complete
@@ -1170,12 +1149,45 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
         }
     }
     __syncthreads();
-    if (P.cluster) cluster_sync_all();
+    cluster_sync_all();
 }
 
 static size_t smem_bytes(int D) {
     return (size_t)NSLOT * SLOT_BYTES + sizeof(float) * 64 * ACC_LD + 4 * sizeof(float) * SliceMap(D).n +
            sizeof(float) * 8 * 64 * OUTP;
+}
+
+// 32 CTAs per network in clusters of 8 (the column blocks of one row block); `at` holds the cluster attribute
+static cudaLaunchConfig_t cluster_launch(int n_nets, size_t smem, cudaStream_t s, cudaLaunchAttribute* at) {
+    at->id = cudaLaunchAttributeClusterDimension;
+    at->val.clusterDim.x = 8; at->val.clusterDim.y = 1; at->val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(32 * n_nets); cfg.blockDim = dim3(TPB); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    return cfg;
+}
+
+// The instantiation for world > 1 (dp) or a single GPU, with its dynamic shared memory opted in once for the largest D
+// the gate admits, and how many of its clusters of 8 can be co-resident (0 if the opt-in fails).  The count is the same
+// at every D: the shared memory of one CTA rules out a second on the same SM.
+struct Instance {
+    void (*kern)(const Args);
+    int max_clusters;
+};
+static const Instance& instance(bool dp) {
+    static Instance inst[2] = {};
+    Instance& in = inst[dp];
+    if (!in.kern) {
+        in.kern = dp ? ppo_persist_kernel<true> : ppo_persist_kernel<false>;
+        cudaLaunchAttribute at;
+        const cudaLaunchConfig_t cfg = cluster_launch(1, smem_bytes(MAXD), nullptr, &at);
+        if (cudaFuncSetAttribute(in.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes) != cudaSuccess ||
+            cudaOccupancyMaxActiveClusters(&in.max_clusters, in.kern, &cfg) != cudaSuccess) {
+            cudaGetLastError();
+            in.max_clusters = 0;
+        }
+    }
+    return in;
 }
 
 }  // namespace pp
@@ -1186,7 +1198,7 @@ size_t ppo_persist_ws_floats(int n_nets, int D, int H) {
            2 * (size_t)pp::MAX_MB + 2 * (size_t)32 * n_nets * pp::DBG_N;
 }
 
-size_t ppo_persist_p2p_floats(int n_nets) { return (size_t)(FSRL_P2P_MAX_RANKS + 1) * n_nets * pp::XG_PER_NET + pp::XG_FLAG_FLOATS + 64; }
+size_t ppo_persist_p2p_floats(int n_nets) { return (size_t)(FSRL_P2P_MAX_RANKS + 1) * n_nets * pp::XG_PER_NET + 64; }
 
 bool ppo_persist_supported(const fsrl_ppo_update_t& u, long long n_total, int batch_size) {
     if (u.H != 256 || batch_size != pp::MB || n_total % pp::MB != 0 || n_total < pp::MB || n_total / pp::MB > pp::MAX_MB) return false;
@@ -1194,13 +1206,8 @@ bool ppo_persist_supported(const fsrl_ppo_update_t& u, long long n_total, int ba
     if (u.D < 1 || u.D > pp::MAXD || u.A > 8 || u.n_nets < 1 || u.n_nets > 3) return false;
     if (u.persist_ws == nullptr || (size_t)u.persist_ws_floats < ppo_persist_ws_floats(u.n_nets, u.D, u.H)) return false;
     if (32 * u.n_nets > sm_count()) return false;
-    static int smem_optin = -1;
-    if (smem_optin < 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    }
-    return pp::smem_bytes(u.D) + 8192 <= (size_t)smem_optin;
+    // the CTAs of a step wait for each other: every cluster of the grid must be resident at once
+    return pp::instance(u.world > 1).max_clusters >= 4 * u.n_nets;
 }
 
 // ug: descriptor whose batch pointers are the gathered (contiguous) arrays; mb_stats filled.
@@ -1237,33 +1244,9 @@ int ppo_persist_run(const fsrl_ppo_update_t& ug, int n_mb, int stats_slot0, long
         a.dbg = reinterpret_cast<long long*>(tab_dev + 2 * (size_t)pp::MAX_MB);
         a.dbg_step = atoi(e);
     }
-    // clusters of 8 CTAs (the column blocks of one row block) when all clusters can be co-resident; otherwise hop B goes
-    // through global memory like the other hops, and every CTA copies its operands itself
-    bool cluster = !getenv("FSRL_PPO_NO_CLUSTER");
-    const size_t smem = pp::smem_bytes(ug.D);
-    const bool dp = ug.world > 1 || getenv("FSRL_PPO_FORCE_DP_KERNEL") != nullptr;   // (the env switch: code-generation experiments)
-    void (*kern)(const pp::Args) = dp ? pp::ppo_persist_kernel<true> : pp::ppo_persist_kernel<false>;
-    static size_t set[2] = {0, 0};
-    if (smem > set[dp]) {
-        FSRL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        set[dp] = smem;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(32 * ug.n_nets); cfg.blockDim = dim3(pp::TPB); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 8; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    if (cluster) {
-        cfg.attrs = at; cfg.numAttrs = 1;
-        int n_clusters = 0;
-        if (cudaOccupancyMaxActiveClusters(&n_clusters, kern, &cfg) != cudaSuccess || n_clusters < 4 * ug.n_nets) {
-            cudaGetLastError();
-            cluster = false;
-        }
-    }
-    if (!cluster) { cfg.attrs = nullptr; cfg.numAttrs = 0; }
-    a.cluster = cluster ? 1 : 0;
-    FSRL_CUDA(cudaLaunchKernelEx(&cfg, kern, a));
+    cudaLaunchAttribute at;
+    const cudaLaunchConfig_t cfg = pp::cluster_launch(ug.n_nets, pp::smem_bytes(ug.D), s, &at);
+    FSRL_CUDA(cudaLaunchKernelEx(&cfg, pp::instance(ug.world > 1).kern, a));
     ++g_launches;
     return FSRL_OK;
 }

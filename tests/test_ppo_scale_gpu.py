@@ -169,14 +169,6 @@ def test_persistent_path_small_epoch_matches_oracle():
     _assert_params_within_fp32_noise(policy, [a2] + c2, actor, critics, osub, lag, 32)
 
 
-def test_persistent_path_without_clusters_matches_oracle(monkeypatch):
-    """The same epochs with hop B through global memory instead of a thread-block cluster (FSRL_PPO_NO_CLUSTER=1; also
-    the launch used when 12 clusters of 8 cannot be co-resident): the G2 epilogue then stages its observation block in
-    the operand ring the GEMM has just read."""
-    monkeypatch.setenv("FSRL_PPO_NO_CLUSTER", "1")
-    test_persistent_path_small_epoch_matches_oracle()
-
-
 def _group_names(policy):
     names = []
     for i in range(1 + policy.critics_num):

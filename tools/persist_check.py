@@ -85,7 +85,7 @@ def main():
     # decode the images (they hold the operands of the LAST step = the only step)
     ws = policy._persist_ws.detach().cpu().numpy()
     from fsrl_b200 import _lib as _fl
-    lib_net_ws = int(_fl.lib.fsrl_ppo_persist_ws_floats(2, 8, 256)) - int(_fl.lib.fsrl_ppo_persist_ws_floats(1, 8, 256)) - 7 * 32 - 2 * 32 * 48
+    lib_net_ws = int(_fl.lib.fsrl_ppo_persist_ws_floats(2, 8, 256)) - int(_fl.lib.fsrl_ppo_persist_ws_floats(1, 8, 256)) - 3 * 32 - 2 * 32 * 48
     x = sub.obs.cpu().double().numpy()
     perm = None
     for net in range(3):
@@ -142,7 +142,7 @@ def main():
         del os.environ["FSRL_PPO_PERSIST_DBG"]
         ws = policy2._persist_ws.detach().cpu().numpy()
         dbg = ws[-2 * 96 * 48:].view(np.int64).reshape(96, 48)
-        names = {1: "S done (h1 tile + W2 images)", 2: "G1 accumulators ready", 3: "head partial written", 4: "flag B passed",
+        names = {1: "S done (h1 tile + W2 images)", 2: "G1 accumulators ready", 3: "head partial written", 4: "hop B passed",
                  5: "dz2 + partials written", 6: "G2/G3 accumulators ready", 7: "G2/G3 epilogue done", 8: "flag D1 passed",
                  9: "slices reduced, sumsq out", 10: "flag D2 passed", 11: "Adam done (step end)", 12: "[producer] flag A passed",
                  13: "[producer] G1 copies issued", 14: "[producer] flag C passed", 22: "G2: mask applied",
