@@ -156,6 +156,22 @@ class Cvpo(ctypes.Structure):
                 ("log_sigma", c_vp), ("log_sigma_old", c_vp)]
 
 
+class TrajRow(ctypes.Structure):
+    _fields_ = [("env", c_int), ("start", c_int), ("len", c_int), ("finish", c_int), ("terminated", c_int),
+                ("truncated", c_int), ("ret", c_f64), ("cost", c_f64)]
+
+
+class TrajScan(ctypes.Structure):
+    _fields_ = [("last", c_vp), ("open", c_vp), ("open_len", c_vp), ("steps", c_vp), ("rew", c_vp),
+                ("cost", c_vp), ("rows", c_vp), ("n_rows", c_vp), ("row_cap", c_int), ("pad", c_int)]
+
+
+class TrajArena(ctypes.Structure):
+    _fields_ = [("obs", c_vp), ("obs_next", c_vp), ("act", c_vp), ("rew", c_vp), ("cost", c_vp),
+                ("term", c_vp), ("trunc", c_vp), ("stride", ctypes.c_longlong), ("n_slots", ctypes.c_longlong),
+                ("D", c_int), ("A", c_int)]
+
+
 ALGO_SAC, ALGO_DDPG = 0, 1
 OFF_STATS = 8
 CVPO_STATS = 16
@@ -179,6 +195,10 @@ SIGNATURES = {
     "fsrl_env_reset_all": (c_int, [ctypes.POINTER(Rollout), c_vp]),
     "fsrl_collect_begin": (c_int, [ctypes.POINTER(Rollout), c_int, c_vp]),
     "fsrl_rollout_steps": (c_int, [ctypes.POINTER(Rollout), c_int, c_vp]),
+    "fsrl_traj_begin": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_vp]),
+    "fsrl_traj_scan": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_int, c_vp]),
+    "fsrl_traj_copy": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajArena), c_vp, c_int, c_vp]),
+    "fsrl_traj_gather": (c_int, [ctypes.POINTER(TrajArena), ctypes.POINTER(TrajArena), c_vp, c_int, c_vp]),
     "fsrl_mlp_forward": (c_int, [ctypes.POINTER(Mlp3), c_vp, c_vp, ctypes.c_longlong, c_vp, c_vp]),
     "fsrl_engine_slot_floats": (c_size, [c_int, c_int]),
     "fsrl_engine_forward": (c_int, [ctypes.POINTER(Engine), ctypes.POINTER(NetList), ctypes.POINTER(EngInput), c_int, c_int, c_vp]),
@@ -246,7 +266,7 @@ def _check_abi_sizes():
     lib.fsrl_abi_sizeof.restype = c_size
     lib.fsrl_abi_sizeof.argtypes = [c_int]
     for which, cls in enumerate((Mlp3, CollectStats, Rollout, PpoUpdate, NetRef, NetList, Engine, EngInput,
-                                 OffPolicy, Cpo, Cvpo)):
+                                 OffPolicy, Cpo, Cvpo, TrajRow, TrajScan, TrajArena)):
         want = lib.fsrl_abi_sizeof(which)
         if want != ctypes.sizeof(cls):
             raise ImportError(f"ABI mismatch: {cls.__name__} is {ctypes.sizeof(cls)} bytes in python, "

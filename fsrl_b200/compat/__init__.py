@@ -124,7 +124,7 @@ def install(force: bool = False) -> List[str]:
     if want("tianshou"):
         vec = {n: _vector_env_class(n) for n in ("DummyVectorEnv", "ShmemVectorEnv", "SubprocVectorEnv")}
         t_env = _mod("tianshou.env", BaseVectorEnv=_envs.DeviceVectorEnv, **vec)
-        t_data = _mod("tianshou.data", Batch=_data.Batch, ReplayBuffer=_data.VectorReplayBuffer,
+        t_data = _mod("tianshou.data", Batch=_data.Batch, ReplayBuffer=_data.ReplayBuffer,
                       ReplayBufferManager=_data.VectorReplayBuffer, VectorReplayBuffer=_data.VectorReplayBuffer,
                       to_numpy=_data.to_numpy, to_torch_as=_data.to_torch_as)
 

@@ -62,6 +62,9 @@ extern "C" size_t fsrl_abi_sizeof(int which) {
         case 8: return sizeof(fsrl_offpolicy_t);
         case 9: return sizeof(fsrl_cpo_t);
         case 10: return sizeof(fsrl_cvpo_t);
+        case 11: return sizeof(fsrl_traj_row_t);
+        case 12: return sizeof(fsrl_traj_scan_t);
+        case 13: return sizeof(fsrl_traj_arena_t);
         default: return 0;
     }
 }

@@ -27,6 +27,16 @@ __device__ __forceinline__ float xs(float a, float b) { return __fsub_rn(a, b); 
 __device__ __forceinline__ float xd(float a, float b) { return __fdiv_rn(a, b); }
 __device__ __forceinline__ float xq(float a) { return __fsqrt_rn(a); }
 
+// map_action (base_policy.py:244-256): the policy's action -> what the env receives.  Bound to
+// [-1, 1] by clipping or tanh (bound = FSRL_BOUND_*), then stretch onto [lo, hi].  The rollout
+// kernel steps the env with it and the trajectory copy stores it, so both must call this one.
+__device__ __forceinline__ float map_action(float v, int bound, int scaling, float lo, float hi) {
+    if (bound == 1) v = fminf(1.0f, fmaxf(-1.0f, v));
+    else if (bound == 2) v = tanhf(v);
+    if (scaling) v = xa(lo, xd(xm(xs(hi, lo), xa(v, 1.0f)), 2.0f));
+    return v;
+}
+
 // rotate the unit heading (c, s) by a small angle d with polynomial sin/cos, renormalise
 __device__ __forceinline__ void rotate_heading(float& c, float& s, float d) {
     const float d2 = xm(d, d);

@@ -16,6 +16,7 @@
 namespace fsrl {
 
 static_assert(sizeof(fsrl_mlp3_t) == sizeof(Mlp3), "ABI struct mismatch");
+static_assert(FSRL_BOUND_CLIP == 1 && FSRL_BOUND_TANH == 2, "map_action() codes");
 
 template <int KIND, int H>
 __global__ void __launch_bounds__(MLP_TPB)
@@ -135,13 +136,8 @@ rollout_step_kernel(const fsrl_rollout_t a) {
     }
     // ---- map_action (base_policy.py:244-256) ---------------------------------------------------
 #pragma unroll
-    for (int j = 0; j < A; ++j) {
-        float v = act[j];
-        if (a.action_bound == FSRL_BOUND_CLIP) v = fminf(1.0f, fmaxf(-1.0f, v));
-        else if (a.action_bound == FSRL_BOUND_TANH) v = tanhf(v);
-        if (a.action_scaling) v = xa(a.act_low[j], xd(xm(xs(a.act_high[j], a.act_low[j]), xa(v, 1.0f)), 2.0f));
-        aenv[j] = v;
-    }
+    for (int j = 0; j < A; ++j)
+        aenv[j] = map_action(act[j], a.action_bound, a.action_scaling, a.act_low[j], a.act_high[j]);
     // ---- env.step ---------------------------------------------------------------------------------
     float s[S];
 #pragma unroll

@@ -126,3 +126,9 @@ class DeviceVectorReplayBuffer:
 
 # the names the reference imports
 VectorReplayBuffer = DeviceVectorReplayBuffer
+
+
+def ReplayBuffer(size: int, buffer_num: int = 1, **kwargs) -> DeviceVectorReplayBuffer:
+    """tianshou's ``ReplayBuffer(size)``: one sub-buffer of ``size`` slots (``BasicCollector``'s buffer,
+    basic_collector.py:56; collect_dataset.py:335).  ``ReplayBuffer(size, n)`` keeps meaning n sub-buffers."""
+    return DeviceVectorReplayBuffer(size, buffer_num, **kwargs)

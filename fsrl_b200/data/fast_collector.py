@@ -22,12 +22,13 @@ from .. import _lib
 from ..envs import DeviceVectorEnv
 from .batch import Batch
 from .buffer import DeviceVectorReplayBuffer
+from .traj_buf import TrajectoryBuffer, TrajectoryHarvest
 
 
 class FastCollector(object):
     def __init__(self, policy, env: DeviceVectorEnv, buffer: Optional[DeviceVectorReplayBuffer] = None,
                  preprocess_fn: Optional[Callable[..., Batch]] = None,
-                 exploration_noise: bool = False) -> None:
+                 exploration_noise: bool = False, traj_buffer: Optional[TrajectoryBuffer] = None) -> None:
         super().__init__()
         if not isinstance(env, DeviceVectorEnv):
             raise TypeError("fsrl_b200.FastCollector steps DeviceVectorEnv instances on the GPU; "
@@ -38,6 +39,11 @@ class FastCollector(object):
         self.env_num = len(env)
         self.exploration_noise = exploration_noise
         self._store = buffer is not None
+        self.traj_buffer = traj_buffer
+        if traj_buffer is not None:
+            self._harvest = TrajectoryHarvest(self.env_num, env.device)
+            if buffer is None:      # the harvest reads finished episodes from a ring: a private one of the least size
+                buffer = DeviceVectorReplayBuffer(self.env_num * self.min_ring_capacity(), self.env_num)
         self._assign_buffer(buffer)
         self.policy = policy
         self.preprocess_fn = None
@@ -70,6 +76,18 @@ class FastCollector(object):
     def reset_env(self, gym_reset_kwargs: Optional[Dict[str, Any]] = None) -> None:
         self.env.reset()
 
+    def min_ring_capacity(self, n_episode: Optional[int] = None) -> int:
+        """Ring slots per env a ``traj_buffer`` harvest needs: an episode must still be in the ring when the scan
+        after its last step runs.  That is once after the collect when every ready env runs one episode
+        (``n_episode <= env_num``), else after every chunk of ``min(T, 64)`` steps."""
+        T = self.env.max_episode_steps
+        if n_episode is not None and n_episode <= self.env_num:
+            return T
+        return T + self._chunk()
+
+    def _chunk(self) -> int:
+        return max(1, min(self.env.max_episode_steps, 64))
+
     # ------------------------------------------------------------------------------------------------
     def _descriptor(self, random: bool) -> "_lib.Rollout":
         r = _lib.Rollout()
@@ -101,18 +119,28 @@ class FastCollector(object):
         r = self._descriptor(random)
         r.inline_done = 1 if n_episode <= self.env_num else 0
         T = env.max_episode_steps
+        traj = self.traj_buffer
+        if traj is not None and self.buffer.cap < self.min_ring_capacity(n_episode):
+            raise ValueError(f"a traj_buffer harvest of collect(n_episode={n_episode}) needs a ring of at least "
+                             f"{self.min_ring_capacity(n_episode)} slots per env; the buffer has {self.buffer.cap}")
         with torch.cuda.device(env.device):
             stream = torch.cuda.current_stream().cuda_stream
             _lib.check(_lib.lib.fsrl_collect_begin(ctypes.byref(r), int(n_episode), stream))
+            if traj is not None:
+                self._harvest.begin(r, stream)
             if r.inline_done:
                 # every ready env runs exactly one episode of at most T steps
                 _lib.check(_lib.lib.fsrl_rollout_steps(ctypes.byref(r), T, stream))
                 st = env.read_stats()
+                if traj is not None:
+                    self._harvest_into(traj, r, min(n_episode, self.env_num), T, stream)
             else:
-                chunk = max(1, min(T, 64))
+                chunk = self._chunk()
                 while True:
                     _lib.check(_lib.lib.fsrl_rollout_steps(ctypes.byref(r), chunk, stream))
                     st = env.read_stats()
+                    if traj is not None:
+                        self._harvest_into(traj, r, 0, chunk, stream)
                     if st.finished:
                         break
         if not st.finished:
@@ -141,3 +169,8 @@ class FastCollector(object):
             "truncated": st.trunc_count / done_count,
             "terminated": st.term_count / done_count,
         }
+
+    def _harvest_into(self, traj: TrajectoryBuffer, r, n_ready: int, window: int, stream: int) -> None:
+        rows = self._harvest.scan(r, n_ready, window, stream)
+        env = self.env
+        traj._commit(r, rows, env.max_episode_steps, env.D, env.A, env.device, stream)

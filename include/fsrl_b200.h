@@ -137,6 +137,52 @@ int fsrl_collect_begin(const fsrl_rollout_t* r, int n_episode, void* stream);
 /* n_steps vector steps; steps after stats->finished are no-ops */
 int fsrl_rollout_steps(const fsrl_rollout_t* r, int n_steps, void* stream);
 
+/* ---- offline datasets: finished episodes of the rollout ring -> trajectory arena ----------------
+ * Replaces the per-transition Batch.cat / return sums of TrajectoryBuffer.store
+ * (fsrl/data/traj_buf.py:60-95), fed by BasicCollector (basic_collector.py:238-248), and the
+ * Batch.cat of get_all() (:183-189).  The host decides which episodes to keep; the device scans,
+ * copies and packs.
+ *   fsrl_traj_begin  start of a collect: the harvest state forgets any open episode
+ *   fsrl_traj_scan   walk every env's ring slots written since the last scan; append one row per
+ *                    episode that finished there to rows[] (atomic counter *n_rows, which keeps
+ *                    counting past row_cap: the caller treats *n_rows > row_cap as an error).  Ring
+ *                    slots may be overwritten only after the scan that saw them, and an env's
+ *                    unscanned slots must be fewer than cap, except on the one-episode-per-env path:
+ *                    there n_ready > 0, and a ready env (e < n_ready) whose pointer did not move
+ *                    wrote exactly cap slots.  n_ready = 0 otherwise.
+ *   fsrl_traj_copy   jobs[n][4] = (env, start slot, length, arena slot): copy episodes into the
+ *                    arena; act is stored remapped, as the env received it (map_action)
+ *   fsrl_traj_gather jobs[n][3] = (arena slot, length, first output row): pack into `out`, whose
+ *                    arrays are contiguous rows (out->stride and out->n_slots are ignored) */
+typedef struct fsrl_traj_row {
+    int env, start, len;      /* ring slot of the first transition, number of transitions */
+    int finish;               /* transitions env wrote since fsrl_traj_begin, the last one included */
+    int terminated, truncated;
+    double ret, cost;         /* fp64 sums of the stored fp32 rewards / costs in time order */
+} fsrl_traj_row_t;
+typedef struct fsrl_traj_scan {
+    int *last, *open, *open_len, *steps; /* [E] ring pointer at the last scan, first slot and length of the
+                                          * open episode, transitions since fsrl_traj_begin */
+    double *rew, *cost;                  /* [E] running sums of the open episode */
+    fsrl_traj_row_t* rows;
+    int* n_rows;
+    int row_cap, pad;
+} fsrl_traj_scan_t;
+typedef struct fsrl_traj_arena {
+    float *obs, *obs_next, *act, *rew, *cost; /* [n_slots * stride] rows of D / D / A / 1 / 1 floats */
+    unsigned char *term, *trunc;
+    long long stride;                          /* transitions per slot (the env's max_episode_steps) */
+    long long n_slots;
+    int D, A;
+} fsrl_traj_arena_t;
+
+int fsrl_traj_begin(const fsrl_rollout_t* r, const fsrl_traj_scan_t* h, void* stream);
+int fsrl_traj_scan(const fsrl_rollout_t* r, const fsrl_traj_scan_t* h, int n_ready, void* stream);
+int fsrl_traj_copy(const fsrl_rollout_t* r, const fsrl_traj_arena_t* a, const int* jobs, int n_jobs,
+                   void* stream);
+int fsrl_traj_gather(const fsrl_traj_arena_t* a, const fsrl_traj_arena_t* out, const long long* jobs,
+                     int n_jobs, void* stream);
+
 /* ---- a9/a10: PPO-Lagrangian update --------------------------------------------------------
  * Replaces PPOLagrangian.policy_loss / critics_loss / learn
  * (fsrl/policy/ppo_lag.py:152-257) and LagrangianPolicy.safety_loss
