@@ -3,7 +3,8 @@
 //
 // The reference's physics engines are absent and irreproducible (SURVEY.md F5), so these are
 // OUR documented analytic models with the task structure of Bullet-Safety-Gym's Circle / Run
-// tasks (dense reward, binary cost, fixed horizon, truncation only).  Every arithmetic step
+// tasks (dense reward, binary cost, fixed horizon; the Drone tasks also terminate on a crash or a
+// flip, every other task is truncation only).  Every arithmetic step
 // uses only IEEE-exact operations (+ - * / sqrt, no FMA contraction, polynomial sin/cos), so
 // the CPU twin in oracle/envs.py reproduces trajectories BIT-EXACTLY from the same actions.
 //
@@ -14,7 +15,8 @@
 namespace fsrl {
 
 enum EnvKind { ENV_CAR_CIRCLE = 0, ENV_CAR_RUN = 1, ENV_BALL_CIRCLE = 2, ENV_BALL_RUN = 3,
-               ENV_ANT_CIRCLE = 4, ENV_POINT_GOAL = 5, ENV_KIND_COUNT = 6 };
+               ENV_ANT_CIRCLE = 4, ENV_POINT_GOAL = 5, ENV_ANT_RUN = 6, ENV_DRONE_CIRCLE = 7,
+               ENV_DRONE_RUN = 8, ENV_KIND_COUNT = 9 };
 
 constexpr int ENV_MAX_D = 64;
 constexpr int ENV_MAX_A = 8;
@@ -73,6 +75,14 @@ namespace ant {
 constexpr float DT = 0.05f, R = 3.0f, XLIM = 2.25f, VMAX = 2.0f, WMAX = 2.0f, AV = 0.1f, AW = 0.15f;
 constexpr float KA = 20.0f, KQ = 10.0f, KD = 4.0f;
 }
+namespace antr {
+constexpr float YLIM = 1.0f, VLIM = 0.8f, RSCALE = 1.0f;
+}
+namespace drone {
+constexpr float DT = 0.05f, G = 9.8f, TM = 4.9f, KM = 0.3f, KT = 20.0f, KP = 25.0f, KD = 6.0f;
+constexpr float KY = 4.0f, KDY = 2.0f, DRAG = 0.5f, Z0 = 1.0f, FLIP = 0.8f;
+constexpr float R = 1.5f, XLIM = 1.125f, YLIM = 0.6f, VLIM = 1.0f, RSCALE = 1.0f;
+}
 namespace pgoal {
 constexpr float DT = 0.05f, VMAX = 1.0f, WMAX = 3.0f, AV = 0.2f, AW = 0.3f, ARENA = 2.0f;
 constexpr float GOAL_R = 0.3f, HAZ_R = 0.2f, LIDAR_MAX = 3.0f;
@@ -89,6 +99,9 @@ __host__ __device__ inline EnvDims env_dims(int kind) {
         case ENV_BALL_RUN: return {7, 2, 5, 100};
         case ENV_ANT_CIRCLE: return {34, 8, 30, 500};
         case ENV_POINT_GOAL: return {60, 2, 28, 1000};
+        case ENV_ANT_RUN: return {34, 8, 31, 300};
+        case ENV_DRONE_CIRCLE: return {18, 4, 17, 300};
+        case ENV_DRONE_RUN: return {19, 4, 18, 200};
         default: return {0, 0, 0, 0};
     }
 }
@@ -253,6 +266,22 @@ struct Env<ENV_BALL_RUN> {
 // modelled as damped oscillators.  Joints 0-3 contribute thrust, 4-7 contribute turning.
 // state: x, y, c, s, v, w, q[8], qd[8], a_prev[8]
 // ---------------------------------------------------------------------------------------------
+// the 8 joints (shared with Ant-Run): integrate, remember the action, sum thrust / turn / a.a
+__device__ __forceinline__ void ant_joints(float* st, const float* a, float& thrust, float& turn, float& ctrl) {
+    using namespace ant;
+    thrust = 0.0f; turn = 0.0f; ctrl = 0.0f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        float q = st[6 + j], qd = st[14 + j];
+        // qd += (KA*a - KQ*q - KD*qd) * dt ; q += qd * dt
+        qd = xa(qd, xm(xs(xs(xm(KA, a[j]), xm(KQ, q)), xm(KD, qd)), DT));
+        q = xa(q, xm(qd, DT));
+        st[6 + j] = q; st[14 + j] = qd; st[22 + j] = a[j];
+        if (j < 4) thrust = xa(thrust, q); else turn = xa(turn, q);
+        ctrl = xa(ctrl, xm(a[j], a[j]));
+    }
+}
+
 template <>
 struct Env<ENV_ANT_CIRCLE> {
     static constexpr int D = 34, A = 8, S = 30, T = 500;
@@ -295,17 +324,8 @@ struct Env<ENV_ANT_CIRCLE> {
     __device__ static void step(float* st, const float* a, uint32_t, uint32_t, uint32_t,
                                 float& rew, float& cost, bool& term) {
         using namespace ant;
-        float thrust = 0.0f, turn = 0.0f, ctrl = 0.0f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            float q = st[6 + j], qd = st[14 + j];
-            // qd += (KA*a - KQ*q - KD*qd) * dt ; q += qd * dt
-            qd = xa(qd, xm(xs(xs(xm(KA, a[j]), xm(KQ, q)), xm(KD, qd)), DT));
-            q = xa(q, xm(qd, DT));
-            st[6 + j] = q; st[14 + j] = qd; st[22 + j] = a[j];
-            if (j < 4) thrust = xa(thrust, q); else turn = xa(turn, q);
-            ctrl = xa(ctrl, xm(a[j], a[j]));
-        }
+        float thrust, turn, ctrl;
+        ant_joints(st, a, thrust, turn, ctrl);
         // joint deflection (bounded to [-1,1]) commands the torso
         float f = fminf(1.0f, fmaxf(-1.0f, xm(thrust, 0.25f)));
         float g = fminf(1.0f, fmaxf(-1.0f, xm(turn, 0.25f)));
@@ -430,6 +450,210 @@ struct Env<ENV_POINT_GOAL> {
             if (xa(xm(dx, dx), xm(dy, dy)) <= HAZ_R * HAZ_R) cost = 1.0f;
         }
         term = false;
+    }
+};
+
+// ---------------------------------------------------------------------------------------------
+// Ant-Run (D = 34, A = 8, T = 300): Ant-Circle's joints and torso on the Run task.  Reward is the
+// forward progress in x per second minus Ant-Circle's control cost; cost 1 when |y| leaves the
+// corridor or the torso speed exceeds VLIM.
+// state: x, y, c, s, v, w, q[8], qd[8], a_prev[8], cost_sum
+// ---------------------------------------------------------------------------------------------
+template <>
+struct Env<ENV_ANT_RUN> {
+    static constexpr int D = 34, A = 8, S = 31, T = 300;
+    __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
+        uint32_t r[4];
+        Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
+        st[0] = 0.0f;
+        st[1] = xm(usym(r[0]), 0.2f);
+        heading_from_box(1.0f, xm(usym(r[1]), 0.3f), st[2], st[3]);
+        st[4] = 0.0f; st[5] = 0.0f;
+        uint32_t q[4];
+        Philox::gen(env, ep, 1u, 0u, seed, KEY_RESET, q);
+        uint32_t q2[4];
+        Philox::gen(env, ep, 2u, 0u, seed, KEY_RESET, q2);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            st[6 + j] = xm(usym(q[j]), 0.1f);
+            st[10 + j] = xm(usym(q2[j]), 0.1f);
+        }
+#pragma unroll
+        for (int j = 0; j < 17; ++j) st[14 + j] = 0.0f;
+    }
+    __device__ static void observe(const float* st, float* o) {
+        using namespace ant;
+        const float y = st[1], c = st[2], s = st[3], v = st[4], w = st[5];
+        o[0] = y; o[1] = xm(v, c); o[2] = xm(v, s); o[3] = c; o[4] = s;
+        o[5] = xd(w, WMAX); o[6] = xd(v, antr::VLIM); o[7] = xd(st[0], 10.0f);
+        float aq = 0.0f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            o[8 + j] = st[6 + j];
+            o[16 + j] = xm(st[14 + j], 0.1f);
+            o[24 + j] = st[22 + j];
+            aq = xa(aq, fabsf(st[6 + j]));
+        }
+        o[32] = xs(fabsf(y), antr::YLIM);
+        o[33] = xa(0.5f, xm(aq, 0.0125f));
+    }
+    __device__ static void step(float* st, const float* a, uint32_t, uint32_t, uint32_t,
+                                float& rew, float& cost, bool& term) {
+        using namespace ant;
+        const float x_old = st[0];
+        float thrust, turn, ctrl;
+        ant_joints(st, a, thrust, turn, ctrl);
+        float f = fminf(1.0f, fmaxf(-1.0f, xm(thrust, 0.25f)));
+        float g = fminf(1.0f, fmaxf(-1.0f, xm(turn, 0.25f)));
+        car_advance(st, f, g, VMAX, WMAX, AV, AW, DT);
+        rew = xs(xm(xd(xs(st[0], x_old), DT), antr::RSCALE), xm(0.005f, ctrl));
+        cost = (fabsf(st[1]) > antr::YLIM || st[4] > antr::VLIM) ? 1.0f : 0.0f;
+        st[30] = xa(st[30], cost);
+        term = false;
+    }
+};
+
+// ---------------------------------------------------------------------------------------------
+// Quadrotor (A = 4), shared by Drone-Circle and Drone-Run.
+//   motors   m_j += ((a_j + 1)/2 - m_j) * KM         (first-order lag; a = 0 is hover, m = 1/2)
+//   mix      thrust = TM * sum m  (TM * 2 = G);  roll = m0+m3-m1-m2, pitch = m0+m1-m2-m3,
+//            yaw = m0+m2-m1-m3
+//   attitude roll / pitch are small angles with an attitude-hold spring and damped rates:
+//            p += (KT*roll - KP*phi - KD*p) * dt ; phi += p * dt   (same for pitch)
+//            the yaw rate is damped (KY, KDY) and turns the unit heading (c, s) by rotate_heading
+//   forces   body-frame (thrust*sin(pitch), thrust*sin(roll)) rotated into the world by the
+//            heading, vertical thrust*cos(roll)*cos(pitch) - G, linear drag DRAG on every axis;
+//            sin / cos are the polynomials of rotate_heading
+//   termination: altitude z <= 0 (crash), or |roll| or |pitch| > FLIP
+// state: x, y, z, c, s, vx, vy, vz, phi, theta, p, q, r, m[4] [, cost_sum (run)]
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void poly_sincos(float d, float& sn, float& cs) {
+    const float d2 = xm(d, d);
+    sn = xm(d, xs(1.0f, xm(xd(d2, 6.0f), xs(1.0f, xd(d2, 20.0f)))));
+    cs = xs(1.0f, xm(xd(d2, 2.0f), xs(1.0f, xm(xd(d2, 12.0f), xs(1.0f, xd(d2, 30.0f))))));
+}
+
+// reset: hover at Z0 with the motors at hover thrust, small random x, y (x = 0 for Run) and tilt,
+// random heading
+__device__ __forceinline__ void drone_reset(float* st, bool run, uint32_t seed, uint32_t env, uint32_t ep) {
+    uint32_t r[4];
+    Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
+    st[0] = run ? 0.0f : xm(usym(r[0]), 0.3f);
+    st[1] = xm(usym(r[1]), 0.3f);
+    st[2] = drone::Z0;
+    heading_from_box(usym(r[2]), usym(r[3]), st[3], st[4]);
+    uint32_t q[4];
+    Philox::gen(env, ep, 1u, 0u, seed, KEY_RESET, q);
+    st[5] = 0.0f; st[6] = 0.0f; st[7] = 0.0f;
+    st[8] = xm(usym(q[0]), 0.1f);
+    st[9] = xm(usym(q[1]), 0.1f);
+    st[10] = 0.0f; st[11] = 0.0f; st[12] = 0.0f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) st[13 + j] = 0.5f;
+}
+
+// one step of the body; returns terminated
+__device__ __forceinline__ bool drone_advance(float* st, const float* a) {
+    using namespace drone;
+    float m[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        m[j] = xa(st[13 + j], xm(xs(xm(xa(a[j], 1.0f), 0.5f), st[13 + j]), KM));
+        st[13 + j] = m[j];
+    }
+    const float thr = xm(TM, xa(xa(m[0], m[1]), xa(m[2], m[3])));
+    const float tr = xs(xa(m[0], m[3]), xa(m[1], m[2]));
+    const float tp = xs(xa(m[0], m[1]), xa(m[2], m[3]));
+    const float ty = xs(xa(m[0], m[2]), xa(m[1], m[3]));
+    float x = st[0], y = st[1], z = st[2], c = st[3], s = st[4], vx = st[5], vy = st[6], vz = st[7];
+    float phi = st[8], th = st[9], p = st[10], q = st[11], r = st[12];
+    p = xa(p, xm(xs(xs(xm(KT, tr), xm(KP, phi)), xm(KD, p)), DT));
+    phi = xa(phi, xm(p, DT));
+    q = xa(q, xm(xs(xs(xm(KT, tp), xm(KP, th)), xm(KD, q)), DT));
+    th = xa(th, xm(q, DT));
+    r = xa(r, xm(xs(xm(KY, ty), xm(KDY, r)), DT));
+    rotate_heading(c, s, xm(r, DT));
+    float sp, cp, sth, cth;
+    poly_sincos(phi, sp, cp);
+    poly_sincos(th, sth, cth);
+    const float axb = xm(thr, sth), ayb = xm(thr, sp);
+    const float ax = xs(xm(c, axb), xm(s, ayb));
+    const float ay = xa(xm(s, axb), xm(c, ayb));
+    const float az = xs(xm(xm(thr, cp), cth), G);
+    vx = xa(vx, xm(xs(ax, xm(DRAG, vx)), DT));
+    vy = xa(vy, xm(xs(ay, xm(DRAG, vy)), DT));
+    vz = xa(vz, xm(xs(az, xm(DRAG, vz)), DT));
+    x = xa(x, xm(vx, DT));
+    y = xa(y, xm(vy, DT));
+    z = xa(z, xm(vz, DT));
+    st[0] = x; st[1] = y; st[2] = z; st[3] = c; st[4] = s; st[5] = vx; st[6] = vy; st[7] = vz;
+    st[8] = phi; st[9] = th; st[10] = p; st[11] = q; st[12] = r;
+    return z <= 0.0f || fabsf(phi) > FLIP || fabsf(th) > FLIP;
+}
+
+// the 15 body channels of both Drone tasks
+__device__ __forceinline__ void drone_body_obs(const float* st, float* o) {
+    o[0] = xs(st[2], drone::Z0);
+    o[1] = st[5]; o[2] = st[6]; o[3] = st[7];
+    o[4] = st[3]; o[5] = st[4];
+    o[6] = st[8]; o[7] = st[9];
+    o[8] = st[10]; o[9] = st[11]; o[10] = st[12];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) o[11 + j] = xm(xs(st[13 + j], 0.5f), 2.0f);
+}
+
+// Drone-Circle (D = 18, T = 300): Car/Ball-Circle's reward and cost on the quadrotor
+template <>
+struct Env<ENV_DRONE_CIRCLE> {
+    static constexpr int D = 18, A = 4, S = 17, T = 300;
+    __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
+        drone_reset(st, false, seed, env, ep);
+    }
+    __device__ static void observe(const float* st, float* o) {
+        using namespace drone;
+        const float x = st[0], y = st[1];
+        const float r = xq(xa(xm(x, x), xm(y, y)));
+        o[0] = xd(x, R); o[1] = xd(y, R);
+        drone_body_obs(st, o + 2);
+        o[17] = xd(xs(r, R), R);
+    }
+    __device__ static void step(float* st, const float* a, uint32_t, uint32_t, uint32_t,
+                                float& rew, float& cost, bool& term) {
+        using namespace drone;
+        term = drone_advance(st, a);
+        const float x = st[0], y = st[1], vx = st[5], vy = st[6];
+        const float r = xq(xa(xm(x, x), xm(y, y)));
+        rew = xd(xs(xm(x, vy), xm(y, vx)), xm(R, xa(1.0f, fabsf(xs(r, R)))));
+        cost = (fabsf(x) > XLIM) ? 1.0f : 0.0f;
+    }
+};
+
+// Drone-Run (D = 19, T = 200): Car/Ball-Run's reward and cost on the quadrotor
+template <>
+struct Env<ENV_DRONE_RUN> {
+    static constexpr int D = 19, A = 4, S = 18, T = 200;
+    __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
+        drone_reset(st, true, seed, env, ep);
+        st[17] = 0.0f;
+    }
+    __device__ static void observe(const float* st, float* o) {
+        using namespace drone;
+        const float vx = st[5], vy = st[6];
+        const float sp = xq(xa(xm(vx, vx), xm(vy, vy)));
+        o[0] = st[1];
+        drone_body_obs(st, o + 1);
+        o[16] = xs(sp, VLIM); o[17] = xs(fabsf(st[1]), YLIM); o[18] = xd(st[0], 10.0f);
+    }
+    __device__ static void step(float* st, const float* a, uint32_t, uint32_t, uint32_t,
+                                float& rew, float& cost, bool& term) {
+        using namespace drone;
+        const float x_old = st[0];
+        term = drone_advance(st, a);
+        const float vx = st[5], vy = st[6];
+        const float sp = xq(xa(xm(vx, vx), xm(vy, vy)));
+        rew = xm(xd(xs(st[0], x_old), DT), RSCALE);
+        cost = (fabsf(st[1]) > YLIM || sp > VLIM) ? 1.0f : 0.0f;
+        st[17] = xa(st[17], cost);
     }
 };
 

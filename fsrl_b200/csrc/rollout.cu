@@ -362,6 +362,9 @@ static int check_rollout(const fsrl_rollout_t* a) {
         case ENV_BALL_RUN: { constexpr int K = ENV_BALL_RUN; CALL; } break;          \
         case ENV_ANT_CIRCLE: { constexpr int K = ENV_ANT_CIRCLE; CALL; } break;      \
         case ENV_POINT_GOAL: { constexpr int K = ENV_POINT_GOAL; CALL; } break;      \
+        case ENV_ANT_RUN: { constexpr int K = ENV_ANT_RUN; CALL; } break;            \
+        case ENV_DRONE_CIRCLE: { constexpr int K = ENV_DRONE_CIRCLE; CALL; } break;  \
+        case ENV_DRONE_RUN: { constexpr int K = ENV_DRONE_RUN; CALL; } break;        \
         default: set_error("unknown env kind %d", kind); return FSRL_EINVAL;         \
     }
 

@@ -23,6 +23,7 @@ from .spaces import Box
 KINDS = {
     "SafetyCarCircle-v0": 0, "SafetyCarRun-v0": 1, "SafetyBallCircle-v0": 2, "SafetyBallRun-v0": 3,
     "SafetyAntCircle-v0": 4, "SafetyPointGoal1Gymnasium-v0": 5, "SafetyPointGoal1-v0": 5,
+    "SafetyAntRun-v0": 6, "SafetyDroneCircle-v0": 7, "SafetyDroneRun-v0": 8,
 }
 
 
