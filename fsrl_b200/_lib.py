@@ -195,6 +195,9 @@ SIGNATURES = {
     "fsrl_env_reset_all": (c_int, [ctypes.POINTER(Rollout), c_vp]),
     "fsrl_collect_begin": (c_int, [ctypes.POINTER(Rollout), c_int, c_vp]),
     "fsrl_rollout_steps": (c_int, [ctypes.POINTER(Rollout), c_int, c_vp]),
+    "fsrl_rollout_steps_act": (c_int, [ctypes.POINTER(Rollout), c_f32p, c_vp]),
+    "fsrl_env_step": (c_int, [ctypes.POINTER(Rollout), c_f32p, c_vp, c_int, c_f32p, c_f32p, c_f32p, c_u8p, c_u8p, c_vp]),
+    "fsrl_env_reset_ids": (c_int, [ctypes.POINTER(Rollout), c_vp, c_int, c_f32p, c_vp]),
     "fsrl_traj_begin": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_vp]),
     "fsrl_traj_scan": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_int, c_vp]),
     "fsrl_traj_copy": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajArena), c_vp, c_int, c_vp]),

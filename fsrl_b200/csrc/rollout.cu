@@ -18,12 +18,85 @@ namespace fsrl {
 static_assert(sizeof(fsrl_mlp3_t) == sizeof(Mlp3), "ABI struct mismatch");
 static_assert(FSRL_BOUND_CLIP == 1 && FSRL_BOUND_TANH == 2, "map_action() codes");
 
+// Everything of one collect step that follows the policy's action, for env e: map_action, env.step,
+// buffer.add of (obs, act, logp), statistics and the done bookkeeping.  The fused step and the
+// caller-action step both end here, so the two collect paths apply the same episode rules.
+template <int KIND>
+__device__ __forceinline__ void collect_step_tail(const fsrl_rollout_t& a, int e, const float* obs,
+                                                  const float* act, float logp) {
+    using E_ = Env<KIND>;
+    constexpr int D = E_::D, A = E_::A, S = E_::S;
+    fsrl_collect_stats_t* st = a.stats;
+    float aenv[A];
+    // ---- map_action (base_policy.py:244-256) ---------------------------------------------------
+#pragma unroll
+    for (int j = 0; j < A; ++j)
+        aenv[j] = map_action(act[j], a.action_bound, a.action_scaling, a.act_low[j], a.act_high[j]);
+    // ---- env.step ---------------------------------------------------------------------------------
+    float s[S];
+#pragma unroll
+    for (int i = 0; i < S; ++i) s[i] = a.env_state[(size_t)i * a.E + e];
+    float rew, cost;
+    bool term;
+    const uint32_t ep = a.ep_idx[e] - 1u;
+    E_::step(s, aenv, a.seed_env, (uint32_t)e, ep, rew, cost, term);
+    const int t_new = a.env_t[e] + 1;
+    const bool trunc = (t_new >= a.max_steps) && !term;
+    const bool done = term || trunc;
+    float on[D];
+    E_::observe(s, on);
+
+    // ---- buffer.add (env-major sub-buffer ring; reserved keys of tianshou's buffer) -----------
+    if (a.b_obs) {
+        const int ptr = a.b_ptr[e];
+        const size_t p = (size_t)e * a.cap + ptr;
+#pragma unroll
+        for (int k = 0; k < D; ++k) {
+            a.b_obs[p * D + k] = obs[k];
+            a.b_obs_next[p * D + k] = on[k];
+        }
+#pragma unroll
+        for (int j = 0; j < A; ++j) a.b_act[p * A + j] = act[j];
+        a.b_rew[p] = rew; a.b_cost[p] = cost; a.b_logp[p] = logp;
+        a.b_term[p] = term ? 1 : 0; a.b_trunc[p] = trunc ? 1 : 0;
+        a.b_ptr[e] = (ptr + 1 == a.cap) ? 0 : ptr + 1;
+        const int len = a.b_len[e];
+        if (len < a.cap) a.b_len[e] = len + 1;
+    }
+    // ---- statistics (:326, :338-348) --------------------------------------------------------------
+    atomicAdd(&st->step_count, 1ull);
+    if (cost != 0.f) atomicAdd(&st->total_cost, (double)cost);
+    const double er = a.ep_rew[e] + (double)rew;
+    const int el = a.ep_len[e] + 1;
+    a.ep_rew[e] = er; a.ep_len[e] = el;
+    a.env_t[e] = t_new;
+
+    if (done) {
+        if (a.inline_done) {
+            // n_episode <= ready envs: every finished env is surplus (:357-363) -> retire it
+            atomicAdd(&st->sum_ep_rew, er);
+            atomicAdd(&st->sum_ep_len, (unsigned long long)el);
+            atomicAdd(term ? &st->term_count : &st->trunc_count, 1);
+            a.active[e] = 0;
+            a.ep_rew[e] = 0.0; a.ep_len[e] = 0;
+            const int c = atomicAdd(&st->episode_count, 1) + 1;
+            if (c >= st->n_episode) st->finished_next = 1;
+        } else {
+            a.done_now[e] = term ? 1 : 2;
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < S; ++i) a.env_state[(size_t)i * a.E + e] = s[i];
+#pragma unroll
+    for (int k = 0; k < D; ++k) a.obs_cur[(size_t)e * D + k] = on[k];
+}
+
 template <int KIND, int H>
 __global__ void __launch_bounds__(MLP_TPB)
 rollout_step_kernel(const fsrl_rollout_t a) {
     using E_ = Env<KIND>;
     using TT = MlpTile<H>;
-    constexpr int D = E_::D, A = E_::A, S = E_::S;
+    constexpr int D = E_::D, A = E_::A;
     extern __shared__ __align__(16) float smem[];
     fsrl_collect_stats_t* st = a.stats;
     if (st->finished) return;
@@ -64,7 +137,7 @@ rollout_step_kernel(const fsrl_rollout_t a) {
     const int e = e0 + r;
     if (part != 0 || e >= a.E || !a.active[e]) return;
 
-    float act[A], mu[A], sig[A], aenv[A];
+    float act[A], mu[A], sig[A];
     float logp = 0.f;
     const uint32_t ctr = a.act_ctr[e];
     float eps[(A + 3) / 4 * 4];
@@ -134,67 +207,22 @@ rollout_step_kernel(const fsrl_rollout_t a) {
 #pragma unroll
         for (int j = 0; j < A; ++j) act[j] = fmaf(a.expl_sigma, eps[j], act[j]);
     }
-    // ---- map_action (base_policy.py:244-256) ---------------------------------------------------
-#pragma unroll
-    for (int j = 0; j < A; ++j)
-        aenv[j] = map_action(act[j], a.action_bound, a.action_scaling, a.act_low[j], a.act_high[j]);
-    // ---- env.step ---------------------------------------------------------------------------------
-    float s[S];
-#pragma unroll
-    for (int i = 0; i < S; ++i) s[i] = a.env_state[(size_t)i * a.E + e];
-    float rew, cost;
-    bool term;
-    const uint32_t ep = a.ep_idx[e] - 1u;
-    E_::step(s, aenv, a.seed_env, (uint32_t)e, ep, rew, cost, term);
-    const int t_new = a.env_t[e] + 1;
-    const bool trunc = (t_new >= a.max_steps) && !term;
-    const bool done = term || trunc;
-    float on[D];
-    E_::observe(s, on);
+    collect_step_tail<KIND>(a, e, xtile + r * INP, act, logp);
+}
 
-    // ---- buffer.add (env-major sub-buffer ring; reserved keys of tianshou's buffer) -----------
-    if (a.b_obs) {
-        const int ptr = a.b_ptr[e];
-        const size_t p = (size_t)e * a.cap + ptr;
+// One collect step with the caller's actions act[E][A] (the generic FastCollector path: any torch
+// policy computes them).  The raw action is stored, as the reference stores `act`, and logp = 0, as
+// in random mode; act_ctr does not move.  Followed by rollout_resolve_kernel like the fused step.
+template <int KIND>
+__global__ void __launch_bounds__(128) rollout_act_step_kernel(const fsrl_rollout_t a, const float* __restrict__ act_in) {
+    constexpr int D = Env<KIND>::D, A = Env<KIND>::A;
+    if (a.stats->finished) return;
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.E || !a.active[e]) return;
+    float act[A];
 #pragma unroll
-        for (int k = 0; k < D; ++k) {
-            a.b_obs[p * D + k] = xtile[r * INP + k];
-            a.b_obs_next[p * D + k] = on[k];
-        }
-#pragma unroll
-        for (int j = 0; j < A; ++j) a.b_act[p * A + j] = act[j];
-        a.b_rew[p] = rew; a.b_cost[p] = cost; a.b_logp[p] = logp;
-        a.b_term[p] = term ? 1 : 0; a.b_trunc[p] = trunc ? 1 : 0;
-        a.b_ptr[e] = (ptr + 1 == a.cap) ? 0 : ptr + 1;
-        const int len = a.b_len[e];
-        if (len < a.cap) a.b_len[e] = len + 1;
-    }
-    // ---- statistics (:326, :338-348) --------------------------------------------------------------
-    atomicAdd(&st->step_count, 1ull);
-    if (cost != 0.f) atomicAdd(&st->total_cost, (double)cost);
-    const double er = a.ep_rew[e] + (double)rew;
-    const int el = a.ep_len[e] + 1;
-    a.ep_rew[e] = er; a.ep_len[e] = el;
-    a.env_t[e] = t_new;
-
-    if (done) {
-        if (a.inline_done) {
-            // n_episode <= ready envs: every finished env is surplus (:357-363) -> retire it
-            atomicAdd(&st->sum_ep_rew, er);
-            atomicAdd(&st->sum_ep_len, (unsigned long long)el);
-            atomicAdd(term ? &st->term_count : &st->trunc_count, 1);
-            a.active[e] = 0;
-            a.ep_rew[e] = 0.0; a.ep_len[e] = 0;
-            const int c = atomicAdd(&st->episode_count, 1) + 1;
-            if (c >= st->n_episode) st->finished_next = 1;
-        } else {
-            a.done_now[e] = term ? 1 : 2;
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < S; ++i) a.env_state[(size_t)i * a.E + e] = s[i];
-#pragma unroll
-    for (int k = 0; k < D; ++k) a.obs_cur[(size_t)e * D + k] = on[k];
+    for (int j = 0; j < A; ++j) act[j] = act_in[(size_t)e * A + j];
+    collect_step_tail<KIND>(a, e, a.obs_cur + (size_t)e * D, act, 0.f);
 }
 
 // Resolve finished episodes in env order (general path, n_episode > n_env): count, retire the
@@ -278,14 +306,12 @@ __global__ void __launch_bounds__(1024) rollout_resolve_kernel(const fsrl_rollou
     }
 }
 
-// reset_env (fast_collector.py:131-152): fresh episode in every env; stats untouched
+// fresh episode in env e: its k-th reset draws Philox stream (e, k) on every path; returns obs in o
 template <int KIND>
-__global__ void env_reset_all_kernel(const fsrl_rollout_t a) {
+__device__ __forceinline__ void env_reset_one(const fsrl_rollout_t& a, int e, float* o) {
     using E_ = Env<KIND>;
     constexpr int D = E_::D, S = E_::S;
-    const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= a.E) return;
-    float s[S], o[D];
+    float s[S];
     const uint32_t ep = a.ep_idx[e];
     E_::reset(s, a.seed_env, (uint32_t)e, ep);
     a.ep_idx[e] = ep + 1u;
@@ -294,6 +320,82 @@ __global__ void env_reset_all_kernel(const fsrl_rollout_t a) {
     E_::observe(s, o);
     for (int i = 0; i < S; ++i) a.env_state[(size_t)i * a.E + e] = s[i];
     for (int k = 0; k < D; ++k) a.obs_cur[(size_t)e * D + k] = o[k];
+}
+
+// reset_env (fast_collector.py:131-152): fresh episode in every env; stats untouched
+template <int KIND>
+__global__ void env_reset_all_kernel(const fsrl_rollout_t a) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.E) return;
+    float o[Env<KIND>::D];
+    env_reset_one<KIND>(a, e, o);
+}
+
+// Env ids of rows [i0, i0 + n) of a gym-protocol call, passed by value (the ids are host data, checked
+// on the host).  all != 0: row i is env i and e[] is unused.
+constexpr int ENV_IDS_CHUNK = 512;
+struct EnvIds {
+    int n, i0, all, pad;
+    int e[ENV_IDS_CHUNK];
+};
+
+__device__ __forceinline__ int env_of_row(const EnvIds& ids, int k) { return ids.all ? ids.i0 + k : ids.e[k]; }
+
+// reset(id): fresh episode in the listed envs, obs[i] = the new observation of row i (obs may be NULL)
+template <int KIND>
+__global__ void __launch_bounds__(128) env_reset_ids_kernel(const fsrl_rollout_t a, const __grid_constant__ EnvIds ids,
+                                                            float* __restrict__ obs) {
+    constexpr int D = Env<KIND>::D;
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= ids.n) return;
+    float o[D];
+    env_reset_one<KIND>(a, env_of_row(ids, k), o);
+    if (obs) {
+        const size_t i = (size_t)(ids.i0 + k);
+#pragma unroll
+        for (int c = 0; c < D; ++c) obs[i * D + c] = o[c];
+    }
+}
+
+// step(act, id): gymnasium's env.step with env-range actions act[n][A] (no map_action, no ring, no
+// collect statistics).  Advances the same per-env state the collect reads (env_state, obs_cur, env_t,
+// ep_rew, ep_len), so a later collect continues from it.
+template <int KIND>
+__global__ void __launch_bounds__(128) env_step_ids_kernel(const fsrl_rollout_t a, const __grid_constant__ EnvIds ids,
+                                                           const float* __restrict__ act, float* __restrict__ obs_next,
+                                                           float* __restrict__ rew_out, float* __restrict__ cost_out,
+                                                           uint8_t* __restrict__ term_out, uint8_t* __restrict__ trunc_out) {
+    using E_ = Env<KIND>;
+    constexpr int D = E_::D, A = E_::A, S = E_::S;
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= ids.n) return;
+    const size_t i = (size_t)(ids.i0 + k);
+    const int e = env_of_row(ids, k);
+    float aenv[A];
+#pragma unroll
+    for (int j = 0; j < A; ++j) aenv[j] = act[i * A + j];
+    float s[S];
+#pragma unroll
+    for (int c = 0; c < S; ++c) s[c] = a.env_state[(size_t)c * a.E + e];
+    float rew, cost;
+    bool term;
+    E_::step(s, aenv, a.seed_env, (uint32_t)e, a.ep_idx[e] - 1u, rew, cost, term);
+    const int t_new = a.env_t[e] + 1;
+    const bool trunc = (t_new >= a.max_steps) && !term;
+    float on[D];
+    E_::observe(s, on);
+    a.ep_rew[e] += (double)rew;
+    a.ep_len[e] += 1;
+    a.env_t[e] = t_new;
+#pragma unroll
+    for (int c = 0; c < S; ++c) a.env_state[(size_t)c * a.E + e] = s[c];
+#pragma unroll
+    for (int c = 0; c < D; ++c) {
+        a.obs_cur[(size_t)e * D + c] = on[c];
+        obs_next[i * D + c] = on[c];
+    }
+    rew_out[i] = rew; cost_out[i] = cost;
+    term_out[i] = term ? 1 : 0; trunc_out[i] = trunc ? 1 : 0;
 }
 
 // begin a collect: ready envs = first min(E, n_episode) (:235-236), zero the per-collect stats
@@ -339,18 +441,81 @@ static int launch_step_h(const fsrl_rollout_t& a, cudaStream_t s) {
     return FSRL_OK;
 }
 
+template <int KIND>
+static int launch_act_step(const fsrl_rollout_t& a, const float* act, cudaStream_t s) {
+    rollout_act_step_kernel<KIND><<<(a.E + 127) / 128, 128, 0, s>>>(a, act);
+    FSRL_LAUNCH_CHECK();
+    rollout_resolve_kernel<KIND><<<1, 1024, 0, s>>>(a);
+    FSRL_LAUNCH_CHECK();
+    return FSRL_OK;
+}
+
+// launch(chunk) once per ENV_IDS_CHUNK rows of host ids (once over all E rows without ids)
+template <typename F>
+static int for_id_chunks(const int32_t* ids, int n, F&& launch) {
+    EnvIds c;
+    c.pad = 0;
+    c.all = ids == nullptr;
+    const int step = ids ? ENV_IDS_CHUNK : n;
+    for (int i0 = 0; i0 < n; i0 += step) {
+        c.i0 = i0;
+        c.n = n - i0 < step ? n - i0 : step;
+        if (ids)
+            for (int k = 0; k < c.n; ++k) c.e[k] = ids[i0 + k];
+        int rc = launch(c);
+        if (rc) return rc;
+    }
+    return FSRL_OK;
+}
+
+template <int KIND>
+static int launch_env_step(const fsrl_rollout_t& a, const float* act, const int32_t* ids, int n, float* obs_next,
+                           float* rew, float* cost, uint8_t* term, uint8_t* trunc, cudaStream_t s) {
+    return for_id_chunks(ids, n, [&](const EnvIds& c) {
+        env_step_ids_kernel<KIND><<<(c.n + 127) / 128, 128, 0, s>>>(a, c, act, obs_next, rew, cost, term, trunc);
+        FSRL_LAUNCH_CHECK();
+        return FSRL_OK;
+    });
+}
+
+template <int KIND>
+static int launch_env_reset_ids(const fsrl_rollout_t& a, const int32_t* ids, int n, float* obs, cudaStream_t s) {
+    return for_id_chunks(ids, n, [&](const EnvIds& c) {
+        env_reset_ids_kernel<KIND><<<(c.n + 127) / 128, 128, 0, s>>>(a, c, obs);
+        FSRL_LAUNCH_CHECK();
+        return FSRL_OK;
+    });
+}
+
 }  // namespace fsrl
 
 using namespace fsrl;
 
-static int check_rollout(const fsrl_rollout_t* a) {
+// the env half of the descriptor (what every entry point touches)
+static int check_env_state(const fsrl_rollout_t* a) {
     FSRL_REQUIRE(a != nullptr, "rollout: null descriptor");
     FSRL_REQUIRE(a->kind >= 0 && a->kind < ENV_KIND_COUNT, "rollout: unknown env kind %d", a->kind);
     FSRL_REQUIRE(a->E > 0, "rollout: E must be positive");
-    const EnvDims d = env_dims(a->kind);
-    FSRL_REQUIRE(a->actor.in == d.D || a->mode == FSRL_MODE_RANDOM, "rollout: actor input dim %d != obs dim %d", a->actor.in, d.D);
     FSRL_REQUIRE(a->env_state && a->obs_cur && a->env_t && a->ep_idx && a->act_ctr && a->active &&
                  a->ep_rew && a->ep_len && a->done_now && a->stats, "rollout: null state pointer");
+    return FSRL_OK;
+}
+
+static int check_rollout(const fsrl_rollout_t* a) {
+    int rc = check_env_state(a);
+    if (rc) return rc;
+    const EnvDims d = env_dims(a->kind);
+    FSRL_REQUIRE(a->actor.in == d.D || a->mode == FSRL_MODE_RANDOM, "rollout: actor input dim %d != obs dim %d", a->actor.in, d.D);
+    return FSRL_OK;
+}
+
+// n rows, each an env id in [0, E) when ids (host) is given
+static int check_ids(const char* fn, const fsrl_rollout_t* a, const int32_t* ids, int n) {
+    FSRL_REQUIRE(n >= 1 && n <= a->E, "%s: n = %d outside [1, E = %d]", fn, n, a->E);
+    FSRL_REQUIRE(ids != nullptr || n == a->E, "%s: without ids, n must be E = %d (got %d)", fn, a->E, n);
+    if (ids)
+        for (int i = 0; i < n; ++i)
+            FSRL_REQUIRE(ids[i] >= 0 && ids[i] < a->E, "%s: ids[%d] = %d outside [0, E = %d)", fn, i, ids[i], a->E);
     return FSRL_OK;
 }
 
@@ -385,7 +550,7 @@ extern "C" int fsrl_env_reset_all(const fsrl_rollout_t* a, void* stream) {
 }
 
 extern "C" int fsrl_collect_begin(const fsrl_rollout_t* a, int n_episode, void* stream) {
-    int rc = check_rollout(a);
+    int rc = check_env_state(a);     // either collect path follows: the actor is checked by its steps
     if (rc) return rc;
     FSRL_REQUIRE(n_episode > 0, "n_episode must be positive");   // fast_collector.py:234
     cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -406,4 +571,35 @@ extern "C" int fsrl_rollout_steps(const fsrl_rollout_t* a, int n_steps, void* st
         DISPATCH_KIND(a->kind, { int r2 = launch_step_h<K>(*a, s); if (r2) return r2; });
     }
     return FSRL_OK;
+}
+
+extern "C" int fsrl_rollout_steps_act(const fsrl_rollout_t* a, const float* act, void* stream) {
+    int rc = check_env_state(a);
+    if (rc) return rc;
+    FSRL_REQUIRE(act != nullptr, "fsrl_rollout_steps_act: null action array");
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    DISPATCH_KIND(a->kind, rc = launch_act_step<K>(*a, act, s));
+    return rc;
+}
+
+extern "C" int fsrl_env_step(const fsrl_rollout_t* a, const float* act, const int32_t* ids, int n, float* obs_next,
+                             float* rew, float* cost, uint8_t* term, uint8_t* trunc, void* stream) {
+    int rc = check_env_state(a);
+    if (rc) return rc;
+    rc = check_ids("fsrl_env_step", a, ids, n);
+    if (rc) return rc;
+    FSRL_REQUIRE(act && obs_next && rew && cost && term && trunc, "fsrl_env_step: null action or output array");
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    DISPATCH_KIND(a->kind, rc = launch_env_step<K>(*a, act, ids, n, obs_next, rew, cost, term, trunc, s));
+    return rc;
+}
+
+extern "C" int fsrl_env_reset_ids(const fsrl_rollout_t* a, const int32_t* ids, int n, float* obs, void* stream) {
+    int rc = check_env_state(a);
+    if (rc) return rc;
+    rc = check_ids("fsrl_env_reset_ids", a, ids, n);
+    if (rc) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    DISPATCH_KIND(a->kind, rc = launch_env_reset_ids<K>(*a, ids, n, obs, s));
+    return rc;
 }

@@ -9,9 +9,15 @@ finished envs are retired first (:357-363); every collect ends with a reset of a
 (:375-388).  When ``n_episode <= env_num`` each ready env runs exactly one episode and the
 bookkeeping is done inline by the step kernel; otherwise a one-CTA resolve kernel applies
 the ordered surplus rule after each step.
+
+A policy the rollout kernel cannot run (its own ``forward``, or an actor the parameter arena
+rejects) takes the generic path (``collector.fused == False``): per vector step the collector calls
+``policy(batch)`` and ``exploration_noise`` in torch, then a step kernel with those actions runs the
+same map_action, env step, buffer store and episode bookkeeping as the fused kernel.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import time
 from typing import Any, Callable, Dict, Optional
@@ -23,6 +29,25 @@ from ..envs import DeviceVectorEnv
 from .batch import Batch
 from .buffer import DeviceVectorReplayBuffer
 from .traj_buf import TrajectoryBuffer, TrajectoryHarvest
+
+
+def _fused_policy(policy) -> bool:
+    """Whether the policy's actor runs inside the fused rollout kernel.  That takes a ``fill_rollout``
+    the policy itself defines, or the built-in one of a ``BasePolicy`` that keeps the built-in
+    ``forward`` and whose networks the parameter arena can hold.  Any other policy is called per step."""
+    from ..policy.base_policy import BasePolicy
+    if not hasattr(policy, "fill_rollout"):
+        return False
+    if not isinstance(policy, BasePolicy):
+        return True
+
+    def ours(name):
+        owner = next(c for c in type(policy).__mro__ if name in vars(c))
+        return owner.__module__.startswith("fsrl_b200.")
+
+    if not ours("fill_rollout"):
+        return True
+    return ours("forward") and policy._arena_holds_nets()
 
 
 class FastCollector(object):
@@ -46,6 +71,8 @@ class FastCollector(object):
                 buffer = DeviceVectorReplayBuffer(self.env_num * self.min_ring_capacity(), self.env_num)
         self._assign_buffer(buffer)
         self.policy = policy
+        # fused: the actor runs inside the rollout kernel; generic: the policy is called once per vector step
+        self.fused = _fused_policy(policy)
         self.preprocess_fn = None
         self._action_space = env.action_space
         self.reset(False)
@@ -94,18 +121,34 @@ class FastCollector(object):
         self.env.fill(r)
         if self.buffer is not None:
             self.buffer.fill(r)
-        if hasattr(self.policy, "fill_rollout"):
+        if self.fused:
             self.policy.fill_rollout(r, exploration_noise=self.exploration_noise)
-        elif not random:
-            raise TypeError("the policy does not expose fill_rollout(); only random=True "
-                            "collection is possible with it")
         else:
+            # the policy's own map_action settings, the reference's defaults without them
             r.actor.H = 64
             r.action_bound = {"": 0, "clip": 1, "tanh": 2}[getattr(self.policy, "action_bound_method", "clip")]
             r.action_scaling = int(getattr(self.policy, "action_scaling", True))
         if random:
             r.mode = _lib.MODE_RANDOM
         return r
+
+    def _generic_steps(self, r, n_steps: int, stream: int, no_grad: bool) -> None:
+        """n vector steps of the generic path: policy(batch) -> exploration_noise on all E rows (retired
+        envs included), then one caller-action step kernel + the resolve kernel.  No host sync.  The policy
+        sees a copy of the observations (a device tensor), so keeping or editing batch.obs cannot reach
+        the env state; exploration_noise receives the policy's action as the device tensor it returned."""
+        env, policy = self.env, self.policy
+        want = (env.env_num, env.A)
+        for _ in range(n_steps):
+            with torch.no_grad() if no_grad else contextlib.nullcontext():
+                batch = Batch(obs=env.obs_cur.clone(), info=Batch())
+                act = policy(batch, None).act
+                if self.exploration_noise:
+                    act = policy.exploration_noise(act, batch)
+            act = torch.as_tensor(act, dtype=torch.float32, device=env.device).contiguous()
+            if tuple(act.shape) != want:
+                raise ValueError(f"the policy returned actions of shape {tuple(act.shape)}; the collect needs {want}")
+            _lib.check(_lib.lib.fsrl_rollout_steps_act(ctypes.byref(r), act.data_ptr(), stream))
 
     def collect(self, n_episode: int = 1, random: bool = False, render: bool = False,
                 no_grad: bool = True, gym_reset_kwargs: Optional[Dict[str, Any]] = None) -> Dict[str, Any]:
@@ -125,19 +168,25 @@ class FastCollector(object):
                              f"{self.min_ring_capacity(n_episode)} slots per env; the buffer has {self.buffer.cap}")
         with torch.cuda.device(env.device):
             stream = torch.cuda.current_stream().cuda_stream
+            if self.fused or random:
+                def steps(n):
+                    _lib.check(_lib.lib.fsrl_rollout_steps(ctypes.byref(r), n, stream))
+            else:
+                def steps(n):
+                    self._generic_steps(r, n, stream, no_grad)
             _lib.check(_lib.lib.fsrl_collect_begin(ctypes.byref(r), int(n_episode), stream))
             if traj is not None:
                 self._harvest.begin(r, stream)
             if r.inline_done:
                 # every ready env runs exactly one episode of at most T steps
-                _lib.check(_lib.lib.fsrl_rollout_steps(ctypes.byref(r), T, stream))
+                steps(T)
                 st = env.read_stats()
                 if traj is not None:
                     self._harvest_into(traj, r, min(n_episode, self.env_num), T, stream)
             else:
                 chunk = self._chunk()
                 while True:
-                    _lib.check(_lib.lib.fsrl_rollout_steps(ctypes.byref(r), chunk, stream))
+                    steps(chunk)
                     st = env.read_stats()
                     if traj is not None:
                         self._harvest_into(traj, r, 0, chunk, stream)

@@ -4,7 +4,8 @@ fsrl/data/fast_collector.py:134,172,286; tianshou BaseVectorEnv).
 
 The dynamics are the analytic models of csrc/envs.cuh (bullet_safety_gym / safety_gymnasium
 are absent and irreproducible; SURVEY.md F5).  All state lives in HBM as SoA tensors; the
-fused rollout kernel (csrc/rollout.cu) steps every env without host involvement.
+fused rollout kernel (csrc/rollout.cu) steps every env without host involvement.  ``step`` /
+``reset(id)`` give the gym protocol on the same state, for loops that bring their own actions.
 """
 from __future__ import annotations
 
@@ -111,26 +112,82 @@ class DeviceVectorEnv:
         for j in range(self.A):
             r.act_low[j], r.act_high[j] = float(low[j]), float(high[j])
 
-    def reset(self, ids=None, **kwargs):
-        """Start a fresh episode in every env (partial resets happen inside the rollout
-        kernel; ``ids`` other than None/all is not part of the device protocol)."""
-        if ids is not None and len(ids) != self.env_num:
-            raise NotImplementedError("DeviceVectorEnv resets individual envs on the device only")
+    def _ids(self, id) -> Optional[np.ndarray]:
+        """The ``id`` argument of the vector-env protocol as host int32 env ids (None: every env in
+        order).  The C ABI checks the range."""
+        if id is None:
+            return None
+        if isinstance(id, torch.Tensor):
+            id = id.cpu().numpy()
+        ids = np.atleast_1d(np.asarray(id))
+        if ids.ndim != 1 or ids.size == 0 or not np.issubdtype(ids.dtype, np.integer):
+            raise ValueError(f"env ids must be a non-empty 1-D integer array (got shape {ids.shape}, "
+                             f"dtype {ids.dtype})")
+        return np.ascontiguousarray(ids, dtype=np.int32)
+
+    def _stream(self) -> int:
+        if self.device.type != "cuda":
+            raise RuntimeError(f"DeviceVectorEnv steps CUDA devices only (device={self.device})")
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def reset(self, id=None, **kwargs):
+        """Start a fresh episode in every env, or in the envs ``id`` lists (tianshou's
+        ``reset(id)``); returns their observations, device tensors, and one empty info dict each.
+        A full reset returns the live ``obs_cur``.  ``ids=`` is accepted as another name of ``id``; other
+        keywords (gymnasium's ``seed`` / ``options``) are ignored: the reset streams are keyed by the
+        vector env's seed."""
+        if "ids" in kwargs:
+            if id is not None:
+                raise TypeError("reset() got both id and ids")
+            id = kwargs.pop("ids")
+        ids = self._ids(id)
         r = _lib.Rollout()
         self.fill(r)
         r.mode = _lib.MODE_RANDOM
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib.fsrl_env_reset_all(ctypes.byref(r), torch.cuda.current_stream().cuda_stream))
-        return self.obs_cur, [{} for _ in range(self.env_num)]
+            stream = self._stream()
+            if ids is None:
+                _lib.check(_lib.lib.fsrl_env_reset_all(ctypes.byref(r), stream))
+                return self.obs_cur, [{} for _ in range(self.env_num)]
+            obs = torch.empty((len(ids), self.D), dtype=torch.float32, device=self.device)
+            _lib.check(_lib.lib.fsrl_env_reset_ids(ctypes.byref(r), ids.ctypes.data, len(ids), obs.data_ptr(), stream))
+        return obs, [{} for _ in range(len(ids))]
 
     def read_stats(self) -> "_lib.CollectStats":
         self._stats_host.copy_(self.stats, non_blocking=False)
         return _lib.CollectStats.from_buffer_copy(self._stats_host.numpy().tobytes())
 
     def step(self, action, id=None):
-        raise NotImplementedError(
-            "DeviceVectorEnv is stepped by the fused rollout kernel (FastCollector.collect); "
-            "a host-side step() would round-trip every action through PCIe")
+        """gymnasium's ``step`` over the envs ``id`` lists (all, in order, by default):
+        ``action`` is (n, A) in the env's range, a CUDA tensor (used in place) or anything
+        ``torch.as_tensor`` takes (uploaded).  Returns ``(obs_next, rew, terminated, truncated,
+        info)`` as device tensors with ``info = Batch(cost=..., env_id=...)``.  Envs are not reset
+        here: call ``reset(id)`` on the ones that finished.  ``truncated`` is set only when the
+        horizon is reached without a termination, as in the collector's buffer.  A listed env must
+        appear once."""
+        from .data.batch import Batch
+        ids = self._ids(id)
+        n = self.env_num if ids is None else len(ids)
+        act = torch.as_tensor(action, dtype=torch.float32,
+                              device=action.device if isinstance(action, torch.Tensor) else None)
+        if tuple(act.shape) != (n, self.A):
+            raise ValueError(f"action must have shape ({n}, {self.A}), got {tuple(act.shape)}")
+        stream = self._stream()
+        act = act.to(self.device).contiguous()
+        dev = self.device
+        obs_next = torch.empty((n, self.D), dtype=torch.float32, device=dev)
+        rew = torch.empty(n, dtype=torch.float32, device=dev)
+        cost = torch.empty(n, dtype=torch.float32, device=dev)
+        term = torch.empty(n, dtype=torch.bool, device=dev)        # written as 0 / 1 bytes
+        trunc = torch.empty(n, dtype=torch.bool, device=dev)
+        r = _lib.Rollout()
+        self.fill(r)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib.fsrl_env_step(ctypes.byref(r), act.data_ptr(), None if ids is None else ids.ctypes.data,
+                                              n, obs_next.data_ptr(), rew.data_ptr(), cost.data_ptr(),
+                                              term.data_ptr(), trunc.data_ptr(), stream))
+        env_id = np.arange(n) if ids is None else ids.astype(np.int64)
+        return obs_next, rew, term, trunc, Batch(cost=cost, env_id=env_id)
 
     def render(self, **kwargs):
         return None

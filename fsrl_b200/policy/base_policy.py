@@ -2,8 +2,9 @@
 (/root/reference/fsrl/policy/base_policy.py:83-512), backed by the flat device arena and the
 CUDA kernels instead of eager PyTorch + numba:
 
-* ``forward``              -> csrc/mlpfwd.cu (API compatibility; the collector fuses the
-                               forward into the rollout kernel and never calls this)
+* ``forward``              -> csrc/mlpfwd.cu (API compatibility; the fused collector runs the
+                               actor inside the rollout kernel; an actor the arena cannot hold runs as
+                               its own torch module, called per step by the generic collector)
 * ``compute_gae_returns``  -> batched critic forward + csrc/gae.cu dual scan (:384-451)
 * ``compute_nstep_returns``-> csrc/nstep.cu (:453-512)
 * ``soft_update``          -> csrc/polyak (:220-224)
@@ -114,6 +115,19 @@ class BasePolicy(ABC, nn.Module):
         self._arena = Arena(slots, device)
         return self._arena
 
+    def _arena_holds_nets(self) -> bool:
+        """Whether every network of the policy fits the flat device arena (tianshou Actor / ActorProb / Critic
+        with two equal hidden layers of width 64, 128, 256 or 512), which the rollout kernel and the fused
+        learners need.  Checked without allocating."""
+        if self._arena is not None:
+            return True
+        try:
+            for i, m in enumerate(self._net_list()):
+                slots_from_module("net%d" % i, m)
+        except (TypeError, ValueError, NotImplementedError, AttributeError):
+            return False
+        return True
+
     @property
     def arena(self) -> Arena:
         if self._arena is None:
@@ -196,7 +210,12 @@ class BasePolicy(ABC, nn.Module):
 
     # ---- reference hooks -----------------------------------------------------------------------------
     def forward(self, batch: Batch, state=None, **kwargs: Any) -> Batch:
-        """API-compatible policy forward on a device batch (base_policy.py:178-190)."""
+        """API-compatible policy forward on a device batch (base_policy.py:178-190).  The actor runs through
+        csrc/mlpfwd.cu when the arena holds the policy's networks; any other actor (more hidden layers,
+        LayerNorm, a user's own module) is the torch module the user wrote and runs as one, as in the
+        reference -- FastCollector then takes its generic path."""
+        if not self._arena_holds_nets():
+            return self._module_forward(batch, state)
         obs = torch.as_tensor(batch.obs, dtype=torch.float32, device=self.device).contiguous()
         out = self.net_forward(0, obs)
         a = self.actor
@@ -220,6 +239,23 @@ class BasePolicy(ABC, nn.Module):
             logits = a._max * torch.tanh(out)
             dist, act = None, logits
         return Batch(logits=logits, act=act, state=None, dist=dist)
+
+    def _module_forward(self, batch: Batch, state=None) -> Batch:
+        """The reference's forward (base_policy.py:178-190) with the actor module itself; without a dist_fn a
+        (mu, sigma) head samples mu + sigma * N(0, 1) as forward() does."""
+        logits, hidden = self.actor(batch.obs, state=state)
+        if self.dist_fn is not None:
+            dist = self.dist_fn(*logits) if isinstance(logits, tuple) else self.dist_fn(logits)
+        else:
+            dist = None
+        mean = logits[0] if isinstance(logits, tuple) else logits
+        if (self._deterministic_eval and not self.training) or (dist is None and not isinstance(logits, tuple)):
+            act = mean
+        elif dist is not None:
+            act = dist.sample()
+        else:
+            act = mean + logits[1] * torch.randn_like(mean)
+        return Batch(logits=logits, act=act, state=hidden, dist=dist)
 
     def pre_update_fn(self, **kwarg: Any) -> Any:
         pass

@@ -137,6 +137,26 @@ int fsrl_env_reset_all(const fsrl_rollout_t* r, void* stream);
 int fsrl_collect_begin(const fsrl_rollout_t* r, int n_episode, void* stream);
 /* n_steps vector steps; steps after stats->finished are no-ops */
 int fsrl_rollout_steps(const fsrl_rollout_t* r, int n_steps, void* stream);
+/* one vector step of collect() with the caller's actions instead of r->actor: act[E][A] are the
+ * policy's raw actions (after its exploration noise), one row per env, read for the active envs.
+ * map_action, env.step, buffer.add and the episode bookkeeping are those of fsrl_rollout_steps; the
+ * raw action is stored with logp = 0, and act_ctr is left alone.  r->actor, head and mode are unused. */
+int fsrl_rollout_steps_act(const fsrl_rollout_t* r, const float* act, void* stream);
+
+/* ---- gym vector-env protocol (tianshou BaseVectorEnv.step / reset with env ids) ----------------
+ * ids: HOST int32 [n] env ids, each in [0, E), or NULL for all envs in order (then n must be E).
+ * A listed env must appear once: duplicate ids are the caller's error (their order is undefined).
+ * Rows of act / outputs follow ids.
+ *   fsrl_env_step       act[n][A] env-range actions (no map_action); writes obs_next[n][D], rew[n],
+ *                       cost[n], term[n], trunc[n] (u8; trunc = horizon reached and not terminated)
+ *                       and advances env_state, obs_cur, env_t, ep_rew and ep_len of the listed envs.
+ *                       No ring store, no collect statistics.
+ *   fsrl_env_reset_ids  fresh episode in the listed envs (the same reset stream as every other
+ *                       reset path); obs[n][D] receives their observations (obs may be NULL)
+ * Both return FSRL_EINVAL before touching the device when n, an id or a pointer is invalid. */
+int fsrl_env_step(const fsrl_rollout_t* r, const float* act, const int32_t* ids, int n, float* obs_next,
+                  float* rew, float* cost, uint8_t* term, uint8_t* trunc, void* stream);
+int fsrl_env_reset_ids(const fsrl_rollout_t* r, const int32_t* ids, int n, float* obs, void* stream);
 
 /* ---- offline datasets: finished episodes of the rollout ring -> trajectory arena ----------------
  * Replaces the per-transition Batch.cat / return sums of TrajectoryBuffer.store

@@ -1,12 +1,12 @@
 """Time collect-only env-steps/s of every device environment.
 
-For each of the nine tasks a PPO-Lagrangian actor 2x256 collects one episode in each of 2048 envs
+For each of the nine tasks a PPO-Lagrangian actor 2x256 (2 x --hidden) collects one episode in each of 2048 envs
 (FastCollector.collect(n_episode=2048), the inline path); the collect is timed with CUDA events after a
 warm-up collect, the best of --reps.  An env-step is one stored transition (the collect's ``n/st``), so
 the Drone tasks, whose episodes end early on a crash, report the rate of the steps actually taken.  The
 card name and power limit are read in the same run.  Prints one JSON line per task.
 
-    python tools/env_collect_time.py [--envs 2048] [--reps 5] [--tasks SafetyDroneRun-v0,...]
+    python tools/env_collect_time.py [--envs 2048] [--reps 5] [--hidden 256] [--tasks SafetyDroneRun-v0,...]
 """
 from __future__ import annotations
 
@@ -39,6 +39,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--envs", type=int, default=2048)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--hidden", type=int, default=256)
     ap.add_argument("--tasks", default=",".join(TASKS))
     a = ap.parse_args()
     import torch
@@ -47,7 +48,7 @@ def main():
     name, plimit = _card()
     E = a.envs
     for task in a.tasks.split(","):
-        policy, venv, buf, col = build_ppo(task, hidden=(256, 256), n_env=E)
+        policy, venv, buf, col = build_ppo(task, hidden=(a.hidden, a.hidden), n_env=E)
         col.collect(n_episode=E)                    # warm-up
         times, steps = [], []
         for _ in range(a.reps):
@@ -61,7 +62,7 @@ def main():
             times.append(e0.elapsed_time(e1))
             steps.append(int(st["n/st"]))
         i = min(range(len(times)), key=lambda k: times[k] / steps[k])
-        print(json.dumps(dict(task=task, envs=E, hidden=256, horizon=venv.max_episode_steps, D=venv.D, A=venv.A,
+        print(json.dumps(dict(task=task, envs=E, hidden=a.hidden, horizon=venv.max_episode_steps, D=venv.D, A=venv.A,
                               env_steps=steps[i], ms=round(times[i], 3),
                               env_steps_per_s=round(steps[i] / (times[i] / 1e3)), terminated=st["terminated"],
                               ms_all=[round(t, 3) for t in times], gpu=name, power_limit=plimit)), flush=True)
