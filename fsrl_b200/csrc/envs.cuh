@@ -3,20 +3,26 @@
 //
 // The reference's physics engines are absent and irreproducible (SURVEY.md F5), so these are
 // OUR documented analytic models with the task structure of Bullet-Safety-Gym's Circle / Run
-// tasks (dense reward, binary cost, fixed horizon; the Drone tasks also terminate on a crash or a
-// flip, every other task is truncation only).  Every arithmetic step
+// tasks and Safety-Gymnasium's Point / Car Circle and Goal tasks (dense reward, binary cost, fixed
+// horizon; the Drone tasks also terminate on a crash or a flip, every other task is truncation
+// only).  Every arithmetic step
 // uses only IEEE-exact operations (+ - * / sqrt, no FMA contraction, polynomial sin/cos), so
 // the CPU twin in oracle/envs.py reproduces trajectories BIT-EXACTLY from the same actions.
 //
 // State lives in registers of the thread that owns the env; SoA [S][E] in HBM between steps.
+// step() and observe() also receive the env's Philox key (seed, env, episode), so a model may
+// regenerate data drawn at reset instead of storing it (the Goal2 layouts).
 #pragma once
 #include "common.cuh"
 
 namespace fsrl {
 
+// Kinds 0-8 are the Bullet-Safety-Gym tasks and PointGoal1; the Safety-Gymnasium navigation family
+// starts at 16.  Ids 9-15 are unassigned.
 enum EnvKind { ENV_CAR_CIRCLE = 0, ENV_CAR_RUN = 1, ENV_BALL_CIRCLE = 2, ENV_BALL_RUN = 3,
                ENV_ANT_CIRCLE = 4, ENV_POINT_GOAL = 5, ENV_ANT_RUN = 6, ENV_DRONE_CIRCLE = 7,
-               ENV_DRONE_RUN = 8, ENV_KIND_COUNT = 9 };
+               ENV_DRONE_RUN = 8, ENV_POINT_CIRCLE1 = 16, ENV_POINT_CIRCLE2 = 17, ENV_CAR_CIRCLE1 = 18,
+               ENV_CAR_CIRCLE2 = 19, ENV_POINT_GOAL2 = 20, ENV_CAR_GOAL1 = 21, ENV_CAR_GOAL2 = 22 };
 
 constexpr int ENV_MAX_D = 64;
 constexpr int ENV_MAX_A = 8;
@@ -88,6 +94,11 @@ constexpr float DT = 0.05f, VMAX = 1.0f, WMAX = 3.0f, AV = 0.2f, AW = 0.3f, AREN
 constexpr float GOAL_R = 0.3f, HAZ_R = 0.2f, LIDAR_MAX = 3.0f;
 constexpr int NHAZ = 8, NBIN = 16;
 }
+namespace nav {   // the Safety-Gymnasium family beyond PointGoal1 (the Point body uses pgoal's constants)
+constexpr float CAR_VW = 1.0f, CAR_AL = 0.2f, TRACK = 0.5f;    // Car: top wheel speed, wheel lag, track width
+constexpr float CIRC_R = 1.5f, WALL = 1.125f, START = 0.8f;    // Circle: circle radius, walls, reset box
+constexpr float VASE_R = 0.25f;                                // Goal2: robot-vase contact distance
+}
 
 struct EnvDims { int D, A, S, T; };
 
@@ -102,9 +113,15 @@ __host__ __device__ inline EnvDims env_dims(int kind) {
         case ENV_ANT_RUN: return {34, 8, 31, 300};
         case ENV_DRONE_CIRCLE: return {18, 4, 17, 300};
         case ENV_DRONE_RUN: return {19, 4, 18, 200};
+        case ENV_POINT_CIRCLE1: case ENV_POINT_CIRCLE2: case ENV_CAR_CIRCLE1: case ENV_CAR_CIRCLE2:
+            return {28, 2, 7, 500};
+        case ENV_POINT_GOAL2: case ENV_CAR_GOAL2: return {60, 2, 10, 1000};
+        case ENV_CAR_GOAL1: return {60, 2, 28, 1000};
         default: return {0, 0, 0, 0};
     }
 }
+
+__host__ __device__ inline bool env_kind_known(int kind) { return env_dims(kind).D != 0; }
 
 // ---------------------------------------------------------------------------------------------
 // Car (unicycle with first-order actuator lag).  state: x, y, c, s, v, w [, x0 (run)]
@@ -143,7 +160,7 @@ struct Env<ENV_CAR_CIRCLE> {
         heading_from_box(usym(r[2]), usym(r[3]), st[2], st[3]);
         st[4] = 0.0f; st[5] = 0.0f;
     }
-    __device__ static void observe(const float* st, float* o) {
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
         using namespace carc;
         const float x = st[0], y = st[1], c = st[2], s = st[3], v = st[4], w = st[5];
         const float r = xq(xa(xm(x, x), xm(y, y)));
@@ -174,7 +191,7 @@ struct Env<ENV_CAR_RUN> {
         heading_from_box(1.0f, xm(usym(r[1]), 0.3f), st[2], st[3]);
         st[4] = 0.0f; st[5] = 0.0f; st[6] = 0.0f;
     }
-    __device__ static void observe(const float* st, float* o) {
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
         using namespace carr;
         o[0] = st[1]; o[1] = xm(st[4], st[2]); o[2] = xm(st[4], st[3]); o[3] = st[2]; o[4] = st[3];
         o[5] = xd(st[5], WMAX); o[6] = xd(st[4], VLIM);
@@ -212,7 +229,7 @@ struct Env<ENV_BALL_CIRCLE> {
         Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
         st[0] = xm(usym(r[0]), 0.3f); st[1] = xm(usym(r[1]), 0.3f); st[2] = 0.0f; st[3] = 0.0f;
     }
-    __device__ static void observe(const float* st, float* o) {
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
         using namespace ball;
         const float x = st[0], y = st[1], vx = st[2], vy = st[3];
         const float r = xq(xa(xm(x, x), xm(y, y)));
@@ -240,7 +257,7 @@ struct Env<ENV_BALL_RUN> {
         Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
         st[0] = 0.0f; st[1] = xm(usym(r[0]), 0.2f); st[2] = 0.0f; st[3] = 0.0f; st[4] = 0.0f;
     }
-    __device__ static void observe(const float* st, float* o) {
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
         using namespace ball;
         const float y = st[1], vx = st[2], vy = st[3];
         const float sp = xq(xa(xm(vx, vx), xm(vy, vy)));
@@ -304,7 +321,7 @@ struct Env<ENV_ANT_CIRCLE> {
 #pragma unroll
         for (int j = 0; j < 16; ++j) st[14 + j] = 0.0f;
     }
-    __device__ static void observe(const float* st, float* o) {
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
         using namespace ant;
         const float x = st[0], y = st[1], c = st[2], s = st[3], v = st[4], w = st[5];
         const float r = xq(xa(xm(x, x), xm(y, y)));
@@ -339,10 +356,8 @@ struct Env<ENV_ANT_CIRCLE> {
 };
 
 // ---------------------------------------------------------------------------------------------
-// Point-Goal1 (D = 60, A = 2, T = 1000): unicycle robot, one goal (re-sampled when reached),
-// 8 hazards, 1 vase; three 16-bin pseudo-lidars computed with exact ops (sector membership by
-// cross products against constant bin-edge directions, no atan2).
-// state: x, y, c, s, v, w, gx, gy, goal_count, haz[8][2], vase[2], v_prev, w_prev
+// 16-bin pseudo-lidar of the Safety-Gymnasium tasks, computed with exact ops (sector membership by
+// cross products against constant bin-edge directions, no atan2).  The tasks follow the drones.
 // ---------------------------------------------------------------------------------------------
 __device__ __constant__ float LIDAR_EDGE_C[16] = {
     1.0f, 0.92387953f, 0.70710678f, 0.38268343f, 0.0f, -0.38268343f, -0.70710678f, -0.92387953f,
@@ -351,11 +366,11 @@ __device__ __constant__ float LIDAR_EDGE_S[16] = {
     0.0f, 0.38268343f, 0.70710678f, 0.92387953f, 1.0f, 0.92387953f, 0.70710678f, 0.38268343f,
     0.0f, -0.38268343f, -0.70710678f, -0.92387953f, -1.0f, -0.92387953f, -0.70710678f, -0.38268343f};
 
-__device__ __forceinline__ void lidar_add(float* bins, float rx, float ry) {
-    // rx, ry: object position in the robot frame.  Writes max(closeness) into its sector.
+// rx, ry: object position in the robot frame.  Returns its sector; val = its closeness.
+__device__ __forceinline__ int lidar_bin(float rx, float ry, float& val) {
     using namespace pgoal;
     const float d = xq(xa(xm(rx, rx), xm(ry, ry)));
-    const float val = fmaxf(0.0f, xs(1.0f, xd(d, LIDAR_MAX)));
+    val = fmaxf(0.0f, xs(1.0f, xd(d, LIDAR_MAX)));
     int bin = 0;
 #pragma unroll
     for (int k = 0; k < 16; ++k) {
@@ -364,94 +379,16 @@ __device__ __forceinline__ void lidar_add(float* bins, float rx, float ry) {
         const float c1 = xs(xm(LIDAR_EDGE_C[k1], ry), xm(LIDAR_EDGE_S[k1], rx));   // cross(edge_k+1, r)
         if (c0 >= 0.0f && c1 < 0.0f) bin = k;
     }
+    return bin;
+}
+
+// Writes max(closeness) into the object's sector.
+__device__ __forceinline__ void lidar_add(float* bins, float rx, float ry) {
+    float val;
+    const int bin = lidar_bin(rx, ry, val);
     bins[bin] = fmaxf(bins[bin], val);
 }
 
-template <>
-struct Env<ENV_POINT_GOAL> {
-    static constexpr int D = 60, A = 2, S = 28, T = 1000;
-    __device__ static void sample_goal(float* st, uint32_t seed, uint32_t env, uint32_t ep, uint32_t k) {
-        uint32_t r[4];
-        Philox::gen(env, ep, k, 0u, seed, KEY_GOAL, r);
-        st[6] = xm(usym(r[0]), pgoal::ARENA);
-        st[7] = xm(usym(r[1]), pgoal::ARENA);
-    }
-    __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
-        using namespace pgoal;
-        uint32_t r[4];
-        Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
-        st[0] = xm(usym(r[0]), 0.5f);
-        st[1] = xm(usym(r[1]), 0.5f);
-        heading_from_box(usym(r[2]), usym(r[3]), st[2], st[3]);
-        st[4] = 0.0f; st[5] = 0.0f;
-        sample_goal(st, seed, env, ep, 0u);
-        st[8] = 0.0f;
-#pragma unroll
-        for (int h = 0; h < 5; ++h) {   // 5 Philox calls -> 10 (x, y) pairs: 8 hazards, vase, spare
-            uint32_t q[4];
-            Philox::gen(env, ep, 1u + h, 0u, seed, KEY_RESET, q);
-            if (h < 4) {
-                st[9 + 4 * h] = xm(usym(q[0]), ARENA); st[10 + 4 * h] = xm(usym(q[1]), ARENA);
-                st[11 + 4 * h] = xm(usym(q[2]), ARENA); st[12 + 4 * h] = xm(usym(q[3]), ARENA);
-            } else {
-                st[25] = xm(usym(q[0]), ARENA); st[26] = xm(usym(q[1]), ARENA);
-            }
-        }
-        st[27] = 0.0f;
-    }
-    __device__ static void observe(const float* st, float* o) {
-        using namespace pgoal;
-        const float x = st[0], y = st[1], c = st[2], s = st[3], v = st[4], w = st[5];
-        // 12 proprioceptive channels
-        o[0] = xd(xs(v, st[27]), DT); o[1] = xm(v, w); o[2] = 9.81f;      // accelerometer
-        o[3] = v; o[4] = 0.0f; o[5] = 0.0f;                                // velocimeter (body frame)
-        o[6] = 0.0f; o[7] = 0.0f; o[8] = w;                                // gyro
-        o[9] = c; o[10] = xs(0.0f, s); o[11] = 0.0f;                       // magnetometer
-        float* gl = o + 12; float* hl = o + 28; float* vl = o + 44;
-#pragma unroll
-        for (int k = 0; k < 16; ++k) { gl[k] = 0.0f; hl[k] = 0.0f; vl[k] = 0.0f; }
-        // world -> robot frame: rx = c*dx + s*dy ; ry = -s*dx + c*dy
-        {
-            const float dx = xs(st[6], x), dy = xs(st[7], y);
-            lidar_add(gl, xa(xm(c, dx), xm(s, dy)), xs(xm(c, dy), xm(s, dx)));
-        }
-#pragma unroll
-        for (int h = 0; h < NHAZ; ++h) {
-            const float dx = xs(st[9 + 2 * h], x), dy = xs(st[10 + 2 * h], y);
-            lidar_add(hl, xa(xm(c, dx), xm(s, dy)), xs(xm(c, dy), xm(s, dx)));
-        }
-        {
-            const float dx = xs(st[25], x), dy = xs(st[26], y);
-            lidar_add(vl, xa(xm(c, dx), xm(s, dy)), xs(xm(c, dy), xm(s, dx)));
-        }
-    }
-    __device__ static void step(float* st, const float* a, uint32_t seed, uint32_t env, uint32_t ep,
-                                float& rew, float& cost, bool& term) {
-        using namespace pgoal;
-        const float dxo = xs(st[6], st[0]), dyo = xs(st[7], st[1]);
-        const float dist_old = xq(xa(xm(dxo, dxo), xm(dyo, dyo)));
-        st[27] = st[4];
-        car_advance(st, a[0], a[1], VMAX, WMAX, AV, AW, DT);
-        // keep the robot inside the arena walls
-        st[0] = fminf(ARENA, fmaxf(-ARENA, st[0]));
-        st[1] = fminf(ARENA, fmaxf(-ARENA, st[1]));
-        const float dxn = xs(st[6], st[0]), dyn = xs(st[7], st[1]);
-        const float dist = xq(xa(xm(dxn, dxn), xm(dyn, dyn)));
-        rew = xs(dist_old, dist);
-        if (dist <= GOAL_R) {
-            rew = xa(rew, 1.0f);
-            st[8] = xa(st[8], 1.0f);
-            sample_goal(st, seed, env, ep, 16u + (uint32_t)st[8]);
-        }
-        cost = 0.0f;
-#pragma unroll
-        for (int h = 0; h < NHAZ; ++h) {
-            const float dx = xs(st[9 + 2 * h], st[0]), dy = xs(st[10 + 2 * h], st[1]);
-            if (xa(xm(dx, dx), xm(dy, dy)) <= HAZ_R * HAZ_R) cost = 1.0f;
-        }
-        term = false;
-    }
-};
 
 // ---------------------------------------------------------------------------------------------
 // Ant-Run (D = 34, A = 8, T = 300): Ant-Circle's joints and torso on the Run task.  Reward is the
@@ -481,7 +418,7 @@ struct Env<ENV_ANT_RUN> {
 #pragma unroll
         for (int j = 0; j < 17; ++j) st[14 + j] = 0.0f;
     }
-    __device__ static void observe(const float* st, float* o) {
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
         using namespace ant;
         const float y = st[1], c = st[2], s = st[3], v = st[4], w = st[5];
         o[0] = y; o[1] = xm(v, c); o[2] = xm(v, s); o[3] = c; o[4] = s;
@@ -609,7 +546,7 @@ struct Env<ENV_DRONE_CIRCLE> {
     __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
         drone_reset(st, false, seed, env, ep);
     }
-    __device__ static void observe(const float* st, float* o) {
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
         using namespace drone;
         const float x = st[0], y = st[1];
         const float r = xq(xa(xm(x, x), xm(y, y)));
@@ -636,7 +573,7 @@ struct Env<ENV_DRONE_RUN> {
         drone_reset(st, true, seed, env, ep);
         st[17] = 0.0f;
     }
-    __device__ static void observe(const float* st, float* o) {
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
         using namespace drone;
         const float vx = st[5], vy = st[6];
         const float sp = xq(xa(xm(vx, vx), xm(vy, vy)));
@@ -656,5 +593,192 @@ struct Env<ENV_DRONE_RUN> {
         st[17] = xa(st[17], cost);
     }
 };
+
+// ---------------------------------------------------------------------------------------------
+// Safety-Gymnasium navigation: the Point and Car robots on the Circle and Goal tasks.
+//
+// Bodies (state x, y, c, s, v, w: forward speed and yaw rate):
+//   Point  PointGoal1's unicycle (car_advance, pgoal constants)
+//   Car    differential drive: the two actions command the left / right wheel speeds vl, vr, which
+//          follow them through a first-order lag; v = (vl + vr) / 2, w = (vr - vl) / TRACK.  Safety-
+//          Gymnasium's Car also carries rear-ball sensors; they are not modelled.
+// Both expose the same 12 proprioceptive channels (accelerometer, velocimeter, gyro, magnetometer).
+// ---------------------------------------------------------------------------------------------
+// The Car's wheel lag is linear, so it is the same lag on v and w: v follows (cl + cr) / 2 * CAR_VW and
+// w follows (cr - cl) / TRACK * CAR_VW for the wheel commands cl = a[0], cr = a[1].
+template <bool CAR>
+__device__ __forceinline__ void nav_advance(float* st, const float* a) {
+    using namespace nav;
+    if constexpr (CAR)
+        car_advance(st, xm(xa(a[0], a[1]), 0.5f), xm(xs(a[1], a[0]), 0.5f), CAR_VW, xd(xm(2.0f, CAR_VW), TRACK),
+                    CAR_AL, CAR_AL, pgoal::DT);
+    else
+        car_advance(st, a[0], a[1], pgoal::VMAX, pgoal::WMAX, pgoal::AV, pgoal::AW, pgoal::DT);
+}
+
+// the 12 proprioceptive channels from forward speed v, yaw rate w, the speed before the step, heading
+__device__ __forceinline__ void nav_sensors(float* o, float v, float w, float v_prev, float c, float s) {
+    o[0] = xd(xs(v, v_prev), pgoal::DT); o[1] = xm(v, w); o[2] = 9.81f;   // accelerometer
+    o[3] = v; o[4] = 0.0f; o[5] = 0.0f;                                    // velocimeter (body frame)
+    o[6] = 0.0f; o[7] = 0.0f; o[8] = w;                                    // gyro
+    o[9] = c; o[10] = xs(0.0f, s); o[11] = 0.0f;                           // magnetometer
+}
+
+// the world point (ox, oy) into a lidar of the robot at (x, y) with heading (c, s):
+// robot frame rx = c*dx + s*dy ; ry = -s*dx + c*dy
+__device__ __forceinline__ void lidar_world(float* bins, float ox, float oy, float x, float y, float c, float s) {
+    const float dx = xs(ox, x), dy = xs(oy, y);
+    lidar_add(bins, xa(xm(c, dx), xm(s, dy)), xs(xm(c, dy), xm(s, dx)));
+}
+
+// Circle (D = 28, A = 2, T = 500): the 12 channels, then a 16-bin lidar towards the circle's centre.
+// Reward is Safety-Gymnasium's 0.1 * (x*vy - y*vx) / (r * (1 + |r - R|)), with r kept away from 0.
+// Cost 1 outside the walls: |x| > WALL at level 1, |x| or |y| > WALL at level 2.  The walls do not
+// stop the robot.  Resets start inside the walls.
+// state: x, y, c, s, v, w, v_prev
+template <bool CAR, int LEVEL>
+struct NavCircle {
+    static constexpr int D = 28, A = 2, S = 7, T = 500;
+    __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
+        uint32_t r[4];
+        Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
+        st[0] = xm(usym(r[0]), nav::START);
+        st[1] = xm(usym(r[1]), nav::START);
+        heading_from_box(usym(r[2]), usym(r[3]), st[2], st[3]);
+        st[4] = 0.0f; st[5] = 0.0f; st[6] = 0.0f;
+    }
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
+        const float x = st[0], y = st[1], c = st[2], s = st[3];
+        nav_sensors(o, st[4], st[5], st[6], c, s);
+        // one object: its sector holds its closeness and the others 0, written without a dynamic index
+        // so that o stays in registers
+        const float dx = xs(0.0f, x), dy = xs(0.0f, y);
+        float val;
+        const int bin = lidar_bin(xa(xm(c, dx), xm(s, dy)), xs(xm(c, dy), xm(s, dx)), val);
+#pragma unroll
+        for (int k = 0; k < 16; ++k) o[12 + k] = k == bin ? val : 0.0f;
+    }
+    __device__ static void step(float* st, const float* a, uint32_t, uint32_t, uint32_t,
+                                float& rew, float& cost, bool& term) {
+        using namespace nav;
+        st[6] = st[4];
+        nav_advance<CAR>(st, a);
+        const float x = st[0], y = st[1], vx = xm(st[4], st[2]), vy = xm(st[4], st[3]);
+        const float r = xq(xa(xm(x, x), xm(y, y)));
+        rew = xm(xd(xs(xm(x, vy), xm(y, vx)), xm(fmaxf(r, 1e-6f), xa(1.0f, fabsf(xs(r, CIRC_R))))), 0.1f);
+        cost = (fabsf(x) > WALL || (LEVEL == 2 && fabsf(y) > WALL)) ? 1.0f : 0.0f;
+        term = false;
+    }
+};
+
+// Goal (D = 60, A = 2, T = 1000): one goal, re-sampled when reached (+1 and the distance progress as
+// reward); three 16-bin lidars (goal, hazards, vases).  Level 1: 8 hazards and 1 vase, the layout
+// stored in the state; cost 1 inside a hazard.  Level 2: 10 hazards and 10 vases; the 40 floats do
+// not fit ENV_MAX_S, so step / observe regenerate them from the reset's Philox stream.  Vases are
+// static discs: touching one (distance <= VASE_R) costs 1 like a hazard, and Safety-Gymnasium's
+// vase-velocity cost has no counterpart.  The arena walls clamp the robot.
+// state, level 1: x, y, c, s, v, w, gx, gy, goal_count, haz[8][2], vase[2], v_prev
+// state, level 2: x, y, c, s, v, w, gx, gy, goal_count, v_prev
+template <bool CAR, int LEVEL>
+struct NavGoal {
+    static constexpr int D = 60, A = 2, S = LEVEL == 1 ? 28 : 10, T = 1000;
+    static constexpr int VPREV = S - 1;
+    static_assert(S <= ENV_MAX_S, "env state too large");
+
+    // f(vase, x, y) for every hazard, then every vase.  Reset draws them with counters 1, 2, ... of
+    // its Philox stream, two (x, y) pairs per draw.
+    template <typename F>
+    __device__ static void layout(const float* st, uint32_t seed, uint32_t env, uint32_t ep, F&& f) {
+        using namespace pgoal;
+        if constexpr (LEVEL == 1) {
+#pragma unroll
+            for (int h = 0; h < NHAZ; ++h) f(false, st[9 + 2 * h], st[10 + 2 * h]);
+            f(true, st[25], st[26]);
+        } else {
+#pragma unroll
+            for (int h = 0; h < 10; ++h) {   // draws 0-4: 10 hazards, draws 5-9: 10 vases
+                uint32_t q[4];
+                Philox::gen(env, ep, 1u + h, 0u, seed, KEY_RESET, q);
+                f(h >= 5, xm(usym(q[0]), ARENA), xm(usym(q[1]), ARENA));
+                f(h >= 5, xm(usym(q[2]), ARENA), xm(usym(q[3]), ARENA));
+            }
+        }
+    }
+    __device__ static void sample_goal(float* st, uint32_t seed, uint32_t env, uint32_t ep, uint32_t k) {
+        uint32_t r[4];
+        Philox::gen(env, ep, k, 0u, seed, KEY_GOAL, r);
+        st[6] = xm(usym(r[0]), pgoal::ARENA);
+        st[7] = xm(usym(r[1]), pgoal::ARENA);
+    }
+    __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
+        using namespace pgoal;
+        uint32_t r[4];
+        Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
+        st[0] = xm(usym(r[0]), 0.5f);
+        st[1] = xm(usym(r[1]), 0.5f);
+        heading_from_box(usym(r[2]), usym(r[3]), st[2], st[3]);
+        st[4] = 0.0f; st[5] = 0.0f;
+        sample_goal(st, seed, env, ep, 0u);
+        st[8] = 0.0f;
+        if constexpr (LEVEL == 1) {
+#pragma unroll
+            for (int h = 0; h < 5; ++h) {   // 5 Philox calls -> 10 (x, y) pairs: 8 hazards, vase, spare
+                uint32_t q[4];
+                Philox::gen(env, ep, 1u + h, 0u, seed, KEY_RESET, q);
+                if (h < 4) {
+                    st[9 + 4 * h] = xm(usym(q[0]), ARENA); st[10 + 4 * h] = xm(usym(q[1]), ARENA);
+                    st[11 + 4 * h] = xm(usym(q[2]), ARENA); st[12 + 4 * h] = xm(usym(q[3]), ARENA);
+                } else {
+                    st[25] = xm(usym(q[0]), ARENA); st[26] = xm(usym(q[1]), ARENA);
+                }
+            }
+        }
+        st[VPREV] = 0.0f;
+    }
+    __device__ static void observe(const float* st, float* o, uint32_t seed, uint32_t env, uint32_t ep) {
+        const float x = st[0], y = st[1], c = st[2], s = st[3];
+        nav_sensors(o, st[4], st[5], st[VPREV], c, s);
+        float* gl = o + 12; float* hl = o + 28; float* vl = o + 44;
+#pragma unroll
+        for (int k = 0; k < 16; ++k) { gl[k] = 0.0f; hl[k] = 0.0f; vl[k] = 0.0f; }
+        lidar_world(gl, st[6], st[7], x, y, c, s);
+        layout(st, seed, env, ep, [&](bool vase, float ox, float oy) { lidar_world(vase ? vl : hl, ox, oy, x, y, c, s); });
+    }
+    __device__ static void step(float* st, const float* a, uint32_t seed, uint32_t env, uint32_t ep,
+                                float& rew, float& cost, bool& term) {
+        using namespace pgoal;
+        const float dxo = xs(st[6], st[0]), dyo = xs(st[7], st[1]);
+        const float dist_old = xq(xa(xm(dxo, dxo), xm(dyo, dyo)));
+        st[VPREV] = st[4];
+        nav_advance<CAR>(st, a);
+        st[0] = fminf(ARENA, fmaxf(-ARENA, st[0]));
+        st[1] = fminf(ARENA, fmaxf(-ARENA, st[1]));
+        const float dxn = xs(st[6], st[0]), dyn = xs(st[7], st[1]);
+        const float dist = xq(xa(xm(dxn, dxn), xm(dyn, dyn)));
+        rew = xs(dist_old, dist);
+        if (dist <= GOAL_R) {
+            rew = xa(rew, 1.0f);
+            st[8] = xa(st[8], 1.0f);
+            sample_goal(st, seed, env, ep, 16u + (uint32_t)st[8]);
+        }
+        float c = 0.0f;
+        layout(st, seed, env, ep, [&](bool vase, float ox, float oy) {
+            const float dx = xs(ox, st[0]), dy = xs(oy, st[1]);
+            const float d2 = xa(xm(dx, dx), xm(dy, dy));
+            if (vase ? (LEVEL == 2 && d2 <= nav::VASE_R * nav::VASE_R) : d2 <= HAZ_R * HAZ_R) c = 1.0f;
+        });
+        cost = c;
+        term = false;
+    }
+};
+
+template <> struct Env<ENV_POINT_GOAL> : NavGoal<false, 1> {};
+template <> struct Env<ENV_POINT_CIRCLE1> : NavCircle<false, 1> {};
+template <> struct Env<ENV_POINT_CIRCLE2> : NavCircle<false, 2> {};
+template <> struct Env<ENV_CAR_CIRCLE1> : NavCircle<true, 1> {};
+template <> struct Env<ENV_CAR_CIRCLE2> : NavCircle<true, 2> {};
+template <> struct Env<ENV_POINT_GOAL2> : NavGoal<false, 2> {};
+template <> struct Env<ENV_CAR_GOAL1> : NavGoal<true, 1> {};
+template <> struct Env<ENV_CAR_GOAL2> : NavGoal<true, 2> {};
 
 }  // namespace fsrl

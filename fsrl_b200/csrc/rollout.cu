@@ -44,7 +44,7 @@ __device__ __forceinline__ void collect_step_tail(const fsrl_rollout_t& a, int e
     const bool trunc = (t_new >= a.max_steps) && !term;
     const bool done = term || trunc;
     float on[D];
-    E_::observe(s, on);
+    E_::observe(s, on, a.seed_env, (uint32_t)e, ep);
 
     // ---- buffer.add (env-major sub-buffer ring; reserved keys of tianshou's buffer) -----------
     if (a.b_obs) {
@@ -290,7 +290,7 @@ __global__ void __launch_bounds__(1024) rollout_resolve_kernel(const fsrl_rollou
                 E_::reset(s, a.seed_env, (uint32_t)e, ep);
                 a.ep_idx[e] = ep + 1u;
                 a.env_t[e] = 0;
-                E_::observe(s, o);
+                E_::observe(s, o, a.seed_env, (uint32_t)e, ep);
                 for (int i = 0; i < S; ++i) a.env_state[(size_t)i * a.E + e] = s[i];
                 for (int k = 0; k < D; ++k) a.obs_cur[(size_t)e * D + k] = o[k];
             }
@@ -317,7 +317,7 @@ __device__ __forceinline__ void env_reset_one(const fsrl_rollout_t& a, int e, fl
     a.ep_idx[e] = ep + 1u;
     a.env_t[e] = 0;
     a.ep_rew[e] = 0.0; a.ep_len[e] = 0; a.done_now[e] = 0;
-    E_::observe(s, o);
+    E_::observe(s, o, a.seed_env, (uint32_t)e, ep);
     for (int i = 0; i < S; ++i) a.env_state[(size_t)i * a.E + e] = s[i];
     for (int k = 0; k < D; ++k) a.obs_cur[(size_t)e * D + k] = o[k];
 }
@@ -379,11 +379,12 @@ __global__ void __launch_bounds__(128) env_step_ids_kernel(const fsrl_rollout_t 
     for (int c = 0; c < S; ++c) s[c] = a.env_state[(size_t)c * a.E + e];
     float rew, cost;
     bool term;
-    E_::step(s, aenv, a.seed_env, (uint32_t)e, a.ep_idx[e] - 1u, rew, cost, term);
+    const uint32_t ep = a.ep_idx[e] - 1u;
+    E_::step(s, aenv, a.seed_env, (uint32_t)e, ep, rew, cost, term);
     const int t_new = a.env_t[e] + 1;
     const bool trunc = (t_new >= a.max_steps) && !term;
     float on[D];
-    E_::observe(s, on);
+    E_::observe(s, on, a.seed_env, (uint32_t)e, ep);
     a.ep_rew[e] += (double)rew;
     a.ep_len[e] += 1;
     a.env_t[e] = t_new;
@@ -494,7 +495,7 @@ using namespace fsrl;
 // the env half of the descriptor (what every entry point touches)
 static int check_env_state(const fsrl_rollout_t* a) {
     FSRL_REQUIRE(a != nullptr, "rollout: null descriptor");
-    FSRL_REQUIRE(a->kind >= 0 && a->kind < ENV_KIND_COUNT, "rollout: unknown env kind %d", a->kind);
+    FSRL_REQUIRE(env_kind_known(a->kind), "rollout: unknown env kind %d", a->kind);
     FSRL_REQUIRE(a->E > 0, "rollout: E must be positive");
     FSRL_REQUIRE(a->env_state && a->obs_cur && a->env_t && a->ep_idx && a->act_ctr && a->active &&
                  a->ep_rew && a->ep_len && a->done_now && a->stats, "rollout: null state pointer");
@@ -530,11 +531,18 @@ static int check_ids(const char* fn, const fsrl_rollout_t* a, const int32_t* ids
         case ENV_ANT_RUN: { constexpr int K = ENV_ANT_RUN; CALL; } break;            \
         case ENV_DRONE_CIRCLE: { constexpr int K = ENV_DRONE_CIRCLE; CALL; } break;  \
         case ENV_DRONE_RUN: { constexpr int K = ENV_DRONE_RUN; CALL; } break;        \
+        case ENV_POINT_CIRCLE1: { constexpr int K = ENV_POINT_CIRCLE1; CALL; } break;\
+        case ENV_POINT_CIRCLE2: { constexpr int K = ENV_POINT_CIRCLE2; CALL; } break;\
+        case ENV_CAR_CIRCLE1: { constexpr int K = ENV_CAR_CIRCLE1; CALL; } break;    \
+        case ENV_CAR_CIRCLE2: { constexpr int K = ENV_CAR_CIRCLE2; CALL; } break;    \
+        case ENV_POINT_GOAL2: { constexpr int K = ENV_POINT_GOAL2; CALL; } break;    \
+        case ENV_CAR_GOAL1: { constexpr int K = ENV_CAR_GOAL1; CALL; } break;        \
+        case ENV_CAR_GOAL2: { constexpr int K = ENV_CAR_GOAL2; CALL; } break;        \
         default: set_error("unknown env kind %d", kind); return FSRL_EINVAL;         \
     }
 
 extern "C" int fsrl_env_dims(int kind, int* D, int* A, int* S, int* T) {
-    FSRL_REQUIRE(kind >= 0 && kind < ENV_KIND_COUNT, "fsrl_env_dims: unknown env kind %d", kind);
+    FSRL_REQUIRE(env_kind_known(kind), "fsrl_env_dims: unknown env kind %d", kind);
     const EnvDims d = env_dims(kind);
     if (D) *D = d.D; if (A) *A = d.A; if (S) *S = d.S; if (T) *T = d.T;
     return FSRL_OK;

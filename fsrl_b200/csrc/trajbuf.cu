@@ -128,7 +128,7 @@ using namespace fsrl;
 
 static int check_ring(const fsrl_rollout_t* r) {
     FSRL_REQUIRE(r != nullptr, "trajectory harvest: null rollout descriptor");
-    FSRL_REQUIRE(r->kind >= 0 && r->kind < ENV_KIND_COUNT, "trajectory harvest: unknown env kind %d", r->kind);
+    FSRL_REQUIRE(env_kind_known(r->kind), "trajectory harvest: unknown env kind %d", r->kind);
     FSRL_REQUIRE(r->E > 0 && r->cap > 0, "trajectory harvest: E and cap must be positive");
     FSRL_REQUIRE(r->b_obs && r->b_obs_next && r->b_act && r->b_rew && r->b_cost && r->b_term && r->b_trunc &&
                  r->b_ptr, "trajectory harvest: the rollout has no transition ring");

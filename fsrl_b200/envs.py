@@ -25,6 +25,9 @@ KINDS = {
     "SafetyCarCircle-v0": 0, "SafetyCarRun-v0": 1, "SafetyBallCircle-v0": 2, "SafetyBallRun-v0": 3,
     "SafetyAntCircle-v0": 4, "SafetyPointGoal1Gymnasium-v0": 5, "SafetyPointGoal1-v0": 5,
     "SafetyAntRun-v0": 6, "SafetyDroneCircle-v0": 7, "SafetyDroneRun-v0": 8,
+    "SafetyPointCircle1Gymnasium-v0": 16, "SafetyPointCircle2Gymnasium-v0": 17,
+    "SafetyCarCircle1Gymnasium-v0": 18, "SafetyCarCircle2Gymnasium-v0": 19,
+    "SafetyPointGoal2Gymnasium-v0": 20, "SafetyCarGoal1Gymnasium-v0": 21, "SafetyCarGoal2Gymnasium-v0": 22,
 }
 
 

@@ -84,7 +84,10 @@ enum { FSRL_HEAD_GAUSS_INDEP = 0, FSRL_HEAD_GAUSS_COND = 1, FSRL_HEAD_DETERMINIS
 enum { FSRL_BOUND_NONE = 0, FSRL_BOUND_CLIP = 1, FSRL_BOUND_TANH = 2 };
 enum { FSRL_ENV_CAR_CIRCLE = 0, FSRL_ENV_CAR_RUN = 1, FSRL_ENV_BALL_CIRCLE = 2,
        FSRL_ENV_BALL_RUN = 3, FSRL_ENV_ANT_CIRCLE = 4, FSRL_ENV_POINT_GOAL = 5,
-       FSRL_ENV_ANT_RUN = 6, FSRL_ENV_DRONE_CIRCLE = 7, FSRL_ENV_DRONE_RUN = 8 };
+       FSRL_ENV_ANT_RUN = 6, FSRL_ENV_DRONE_CIRCLE = 7, FSRL_ENV_DRONE_RUN = 8,
+       /* Safety-Gymnasium navigation family; 9-15 are unassigned */
+       FSRL_ENV_POINT_CIRCLE1 = 16, FSRL_ENV_POINT_CIRCLE2 = 17, FSRL_ENV_CAR_CIRCLE1 = 18,
+       FSRL_ENV_CAR_CIRCLE2 = 19, FSRL_ENV_POINT_GOAL2 = 20, FSRL_ENV_CAR_GOAL1 = 21, FSRL_ENV_CAR_GOAL2 = 22 };
 
 /* per-collect statistics, device resident; the keys of collect()'s result dict
  * (fast_collector.py:399-408) are derived from it on the host */

@@ -1,6 +1,6 @@
 """Time collect-only env-steps/s of every device environment.
 
-For each of the nine tasks a PPO-Lagrangian actor 2x256 (2 x --hidden) collects one episode in each of 2048 envs
+For each of the sixteen tasks a PPO-Lagrangian actor 2x256 (2 x --hidden) collects one episode in each of 2048 envs
 (FastCollector.collect(n_episode=2048), the inline path); the collect is timed with CUDA events after a
 warm-up collect, the best of --reps.  An env-step is one stored transition (the collect's ``n/st``), so
 the Drone tasks, whose episodes end early on a crash, report the rate of the steps actually taken.  The
@@ -19,7 +19,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 TASKS = ["SafetyCarCircle-v0", "SafetyCarRun-v0", "SafetyBallCircle-v0", "SafetyBallRun-v0", "SafetyAntCircle-v0",
-         "SafetyPointGoal1Gymnasium-v0", "SafetyAntRun-v0", "SafetyDroneCircle-v0", "SafetyDroneRun-v0"]
+         "SafetyPointGoal1Gymnasium-v0", "SafetyAntRun-v0", "SafetyDroneCircle-v0", "SafetyDroneRun-v0",
+         "SafetyPointCircle1Gymnasium-v0", "SafetyPointCircle2Gymnasium-v0", "SafetyCarCircle1Gymnasium-v0",
+         "SafetyCarCircle2Gymnasium-v0", "SafetyPointGoal2Gymnasium-v0", "SafetyCarGoal1Gymnasium-v0",
+         "SafetyCarGoal2Gymnasium-v0"]
 
 
 def _card():
