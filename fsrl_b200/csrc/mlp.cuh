@@ -93,8 +93,8 @@ __device__ __forceinline__ void stage_load(const float* mat, int K, float* wst, 
 // (row stride lda, Kp a multiple of 8), W a row-major [K][H] global matrix streamed through
 // `wst`.  All threads must call; contains __syncthreads (the first one also orders the
 // caller's earlier shared-memory stores to A).
-template <int H>
-__device__ __forceinline__ void tc_gemm(float (&c)[MlpTile<H>::MT][MlpTile<H>::NT][4], const float* A,
+template <int H, int MT = MlpTile<H>::MT>
+__device__ __forceinline__ void tc_gemm(float (&c)[MT][MlpTile<H>::NT][4], const float* A,
                                         int lda, int K, const float* W, float* wst,
                                         bool stage0_in_flight) {
     using TT = MlpTile<H>;
@@ -127,7 +127,7 @@ __device__ __forceinline__ void tc_gemm(float (&c)[MlpTile<H>::MT][MlpTile<H>::N
                     split_tf32(w[(size_t)(ks + t + 4) * TT::LDW + n0 + 8 * nt + g], bh[nt][1], bl[nt][1]);
                 }
 #pragma unroll
-                for (int mt = 0; mt < TT::MT; ++mt) {
+                for (int mt = 0; mt < MT; ++mt) {
                     uint32_t ah[4], al[4];
                     const float* a = A + (size_t)(16 * mt + g) * lda + k0 + t;
                     split_tf32(a[0], ah[0], al[0]);
@@ -148,13 +148,13 @@ __device__ __forceinline__ void tc_gemm(float (&c)[MlpTile<H>::MT][MlpTile<H>::N
 }
 
 // visit every accumulator pair of this thread: f(row, col, v0, v1) with (row, col), (row, col+1)
-template <int H, class F>
-__device__ __forceinline__ void tc_foreach(float (&c)[MlpTile<H>::MT][MlpTile<H>::NT][4], F f) {
+template <int H, int MT = MlpTile<H>::MT, class F>
+__device__ __forceinline__ void tc_foreach(float (&c)[MT][MlpTile<H>::NT][4], F f) {
     using TT = MlpTile<H>;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int g = lane >> 2, t = lane & 3;
 #pragma unroll
-    for (int mt = 0; mt < TT::MT; ++mt)
+    for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
         for (int nt = 0; nt < TT::NT; ++nt) {
             const int col = warp * TT::WN + 8 * nt + 2 * t;
@@ -163,8 +163,8 @@ __device__ __forceinline__ void tc_foreach(float (&c)[MlpTile<H>::MT][MlpTile<H>
         }
 }
 
-template <int H>
-__device__ __forceinline__ void tc_init_bias(float (&c)[MlpTile<H>::MT][MlpTile<H>::NT][4], const float* bias) {
+template <int H, int MT = MlpTile<H>::MT>
+__device__ __forceinline__ void tc_init_bias(float (&c)[MT][MlpTile<H>::NT][4], const float* bias) {
     using TT = MlpTile<H>;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int t = lane & 3;
@@ -173,7 +173,7 @@ __device__ __forceinline__ void tc_init_bias(float (&c)[MlpTile<H>::MT][MlpTile<
         const int col = warp * TT::WN + 8 * nt + 2 * t;
         const float b0 = bias ? __ldg(bias + col) : 0.f, b1 = bias ? __ldg(bias + col + 1) : 0.f;
 #pragma unroll
-        for (int mt = 0; mt < TT::MT; ++mt) { c[mt][nt][0] = b0; c[mt][nt][1] = b1; c[mt][nt][2] = b0; c[mt][nt][3] = b1; }
+        for (int mt = 0; mt < MT; ++mt) { c[mt][nt][0] = b0; c[mt][nt][1] = b1; c[mt][nt][2] = b0; c[mt][nt][3] = b1; }
     }
 }
 
@@ -350,8 +350,9 @@ __device__ __forceinline__ void mlp_hidden_forward(const Mlp3& m, const MlpSmem<
 
 // Layer 3 (H -> out <= 16): PARTS lanes cooperate on each row, shuffle-reduce; on return the
 // lane with part == 0 of row r (thread r*PARTS) holds out[0..out) for that row.
+// h2: the R rows of this pass (row stride LDA); w3s: W3t staged in shared memory.
 template <int H>
-__device__ __forceinline__ void mlp_head_forward(const Mlp3& m, const MlpSmem<H>& s, float* out) {
+__device__ __forceinline__ void mlp_head_forward(const Mlp3& m, const float* h2, const float* w3s, float* out) {
     using TT = MlpTile<H>;
     const int tid = threadIdx.x;
     const int r = tid / TT::PARTS, part = tid % TT::PARTS;
@@ -359,8 +360,8 @@ __device__ __forceinline__ void mlp_head_forward(const Mlp3& m, const MlpSmem<H>
 #pragma unroll
     for (int j = 0; j < MLP_MAX_OUT; ++j) out[j] = 0.f;
     for (int k = part; k < H; k += TT::PARTS) {
-        const float x = s.h2[(size_t)r * TT::LDA + k];
-        const float* w = s.w3s + (size_t)k * no;
+        const float x = h2[(size_t)r * TT::LDA + k];
+        const float* w = w3s + (size_t)k * no;
 #pragma unroll
         for (int j = 0; j < MLP_MAX_OUT; ++j)
             if (j < no) out[j] = fmaf(x, w[j], out[j]);
@@ -374,6 +375,11 @@ __device__ __forceinline__ void mlp_head_forward(const Mlp3& m, const MlpSmem<H>
             out[j] = v + __ldg(m.b3 + j);
         }
     }
+}
+
+template <int H>
+__device__ __forceinline__ void mlp_head_forward(const Mlp3& m, const MlpSmem<H>& s, float* out) {
+    mlp_head_forward<H>(m, s.h2, s.w3s, out);
 }
 
 // stage R rows of x (optionally gathered) into s.x, zero-padding columns >= in

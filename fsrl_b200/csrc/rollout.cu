@@ -1,4 +1,4 @@
-// Rollout collection on the device: one launch == one vector step of
+// Rollout collection on the device: one loop iteration of rollout_step_kernel == one vector step of
 // FastCollector.collect (reference: /root/reference/fsrl/data/fast_collector.py:252-368):
 //   policy forward      (:267-269 -> base_policy.py:178-190, tianshou ActorProb/Actor)
 //   exploration noise   (:279-280 -> ddpg_lag.py:225-231)
@@ -6,12 +6,15 @@
 //   env.step            (:286)    -> envs.cuh (our analytic models)
 //   cost / buffer.add   (:325-335) -> SoA transition buffers, env-major, per-env ring
 //   done bookkeeping    (:340-363) -> inline when n_episode <= n_env, else rollout_resolve
-// fused into a single kernel per step: the actor MLP forward for a tile of envs (mlp.cuh),
-// Gaussian sampling from a Philox stream, log-prob, clip/scale, the env step and the SoA
-// stores, so no observation or action ever leaves the GPU.
+// fused into a single kernel: the actor MLP forward for a tile of envs (mlp.cuh), Gaussian
+// sampling from a Philox stream, log-prob, clip/scale, the env step and the SoA stores, so no
+// observation or action ever leaves the GPU.  With inline bookkeeping a whole collect is one
+// launch; the resolve path launches one step at a time (FSRL_ROLLOUT_PER_STEP=1 forces that
+// everywhere, for A/B runs and the tests).
 #include "envs.cuh"
 #include "mlp.cuh"
 #include "fsrl_b200.h"
+#include <cstdlib>
 
 namespace fsrl {
 
@@ -91,52 +94,11 @@ __device__ __forceinline__ void collect_step_tail(const fsrl_rollout_t& a, int e
     for (int k = 0; k < D; ++k) a.obs_cur[(size_t)e * D + k] = on[k];
 }
 
-template <int KIND, int H>
-__global__ void __launch_bounds__(MLP_TPB)
-rollout_step_kernel(const fsrl_rollout_t a) {
-    using E_ = Env<KIND>;
-    using TT = MlpTile<H>;
-    constexpr int D = E_::D, A = E_::A;
-    extern __shared__ __align__(16) float smem[];
-    fsrl_collect_stats_t* st = a.stats;
-    if (st->finished) return;
-
-    const int tid = threadIdx.x;
-    const int e0 = blockIdx.x * TT::R;
-    const Mlp3& actor = *reinterpret_cast<const Mlp3*>(&a.actor);
-    const MlpSmem<H> sm(smem, D, actor.out);
-    constexpr int INP = TT::in_pad(D);
-    float* xtile = sm.x;
-
-    // tile-level early out: nothing active in this tile
-    __shared__ int s_any;
-    if (tid == 0) s_any = 0;
-    __syncthreads();
-    if (tid < TT::R) {
-        const int e = e0 + tid;
-        if (e < a.E && a.active[e]) s_any = 1;
-    }
-    __syncthreads();
-    if (!s_any) return;
-
-    // ---- stage the observation tile ---------------------------------------------------------
-    mlp_stage_rows<H>(sm, D, [&](int r) -> const float* {
-        const int e = e0 + r;
-        return e < a.E ? a.obs_cur + (size_t)e * D : nullptr;
-    });
-    __syncthreads();
-
-    float out[MLP_MAX_OUT];
-    if (a.mode != FSRL_MODE_RANDOM) {
-        mlp_hidden_forward<H>(actor, sm);
-        mlp_head_forward<H>(actor, sm, out);
-    }
-
-    // ---- one thread per env: sample, log-prob, map, step, store ------------------------------
-    const int r = tid / TT::PARTS, part = tid % TT::PARTS;
-    const int e = e0 + r;
-    if (part != 0 || e >= a.E || !a.active[e]) return;
-
+// The policy's action for env e from the actor's head output `out` (Philox sampling, the heads, log-prob and
+// DDPG noise), then collect_step_tail.  obs: the observation the actor saw.
+template <int KIND>
+__device__ __forceinline__ void fused_step_env(const fsrl_rollout_t& a, int e, const float* out, const float* obs) {
+    constexpr int A = Env<KIND>::A;
     float act[A], mu[A], sig[A];
     float logp = 0.f;
     const uint32_t ctr = a.act_ctr[e];
@@ -207,7 +169,64 @@ rollout_step_kernel(const fsrl_rollout_t a) {
 #pragma unroll
         for (int j = 0; j < A; ++j) act[j] = fmaf(a.expl_sigma, eps[j], act[j]);
     }
-    collect_step_tail<KIND>(a, e, xtile + r * INP, act, logp);
+    collect_step_tail<KIND>(a, e, obs, act, logp);
+}
+
+// n_steps collect steps of the fused path in one launch: a CTA owns a tile of R envs and steps it n_steps
+// times, or until none of its envs is active.  Envs of different tiles never interact within a step, so
+// this equals n_steps single-step launches when nothing between the steps changes which envs are active:
+// the inline path, where a finished env retires.  The resolve path launches it with n_steps = 1, followed
+// by rollout_resolve_kernel after every step.
+template <int KIND, int H>
+__global__ void __launch_bounds__(MLP_TPB, 1)
+rollout_step_kernel(const fsrl_rollout_t a, int n_steps) {
+    using E_ = Env<KIND>;
+    using TT = MlpTile<H>;
+    constexpr int D = E_::D;
+    extern __shared__ __align__(16) float smem[];
+    fsrl_collect_stats_t* st = a.stats;
+    if (st->finished) return;
+
+    const int tid = threadIdx.x;
+    const int e0 = blockIdx.x * TT::R;
+    const Mlp3& actor = *reinterpret_cast<const Mlp3*>(&a.actor);
+    const MlpSmem<H> sm(smem, D, actor.out);
+    constexpr int INP = TT::in_pad(D);
+    float* xtile = sm.x;
+    const int r = tid / TT::PARTS, part = tid % TT::PARTS;
+    const int e = e0 + r;
+
+    __shared__ int s_any;
+    for (int step = 0; step < n_steps; ++step) {
+        // tile-level early out: nothing active in this tile (the previous step's last barrier orders the
+        // reads of s_any before this store)
+        if (tid == 0) s_any = 0;
+        __syncthreads();
+        if (tid < TT::R) {
+            const int et = e0 + tid;
+            if (et < a.E && a.active[et]) s_any = 1;
+        }
+        __syncthreads();
+        if (!s_any) return;
+
+        // ---- stage the observation tile -----------------------------------------------------
+        mlp_stage_rows<H>(sm, D, [&](int rr) -> const float* {
+            const int et = e0 + rr;
+            return et < a.E ? a.obs_cur + (size_t)et * D : nullptr;
+        });
+        __syncthreads();
+
+        float out[MLP_MAX_OUT];
+        if (a.mode != FSRL_MODE_RANDOM) {
+            mlp_hidden_forward<H>(actor, sm);
+            mlp_head_forward<H>(actor, sm, out);
+        }
+
+        // ---- one thread per env: sample, log-prob, map, step, store --------------------------
+        if (part == 0 && e < a.E && a.active[e]) fused_step_env<KIND>(a, e, out, xtile + r * INP);
+        // this step's stores to obs_cur / active are read by other threads of the tile in the next one
+        __syncthreads();
+    }
 }
 
 // One collect step with the caller's actions act[E][A] (the generic FastCollector path: any torch
@@ -412,8 +431,10 @@ __global__ void collect_begin_kernel(const fsrl_rollout_t a, int n_episode) {
     }
 }
 
+// n_steps steps of the fused kernel, each followed by the resolve kernel; or, with `one_launch`, all of them
+// in one launch followed by one resolve (which turns finished_next into finished)
 template <int KIND>
-static int launch_step_h(const fsrl_rollout_t& a, cudaStream_t s) {
+static int launch_steps_h(const fsrl_rollout_t& a, int n_steps, bool one_launch, cudaStream_t s) {
     const int H = a.actor.H;
 #define GO(HH)                                                                                   \
     {                                                                                            \
@@ -426,7 +447,19 @@ static int launch_step_h(const fsrl_rollout_t& a, cudaStream_t s) {
             attr_done = true;                                                                    \
         }                                                                                        \
         const int grid = (a.E + TT::R - 1) / TT::R;                                              \
-        rollout_step_kernel<KIND, HH><<<grid, MLP_TPB, smem, s>>>(a);                            \
+        if (one_launch) {                                                                        \
+            rollout_step_kernel<KIND, HH><<<grid, MLP_TPB, smem, s>>>(a, n_steps);               \
+            FSRL_LAUNCH_CHECK();                                                                 \
+            rollout_resolve_kernel<KIND><<<1, 1024, 0, s>>>(a);                                  \
+            FSRL_LAUNCH_CHECK();                                                                 \
+        } else {                                                                                 \
+            for (int i = 0; i < n_steps; ++i) {                                                  \
+                rollout_step_kernel<KIND, HH><<<grid, MLP_TPB, smem, s>>>(a, 1);                 \
+                FSRL_LAUNCH_CHECK();                                                             \
+                rollout_resolve_kernel<KIND><<<1, 1024, 0, s>>>(a);                              \
+                FSRL_LAUNCH_CHECK();                                                             \
+            }                                                                                    \
+        }                                                                                        \
     }
     switch (H) {
         case 64: GO(64) break;
@@ -436,9 +469,6 @@ static int launch_step_h(const fsrl_rollout_t& a, cudaStream_t s) {
         default: set_error("rollout: hidden width %d unsupported (64/128/256/512)", H); return FSRL_EINVAL;
     }
 #undef GO
-    FSRL_LAUNCH_CHECK();
-    rollout_resolve_kernel<KIND><<<1, 1024, 0, s>>>(a);
-    FSRL_LAUNCH_CHECK();
     return FSRL_OK;
 }
 
@@ -574,11 +604,13 @@ extern "C" int fsrl_rollout_steps(const fsrl_rollout_t* a, int n_steps, void* st
     FSRL_REQUIRE(a->mode == FSRL_MODE_RANDOM || (a->actor.w1t && a->actor.w2t && a->actor.w3t),
                  "rollout: null actor weights");
     FSRL_REQUIRE(a->actor.out <= MLP_MAX_OUT, "rollout: actor out dim %d > %d", a->actor.out, MLP_MAX_OUT);
+    if (n_steps == 0) return FSRL_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    for (int i = 0; i < n_steps; ++i) {
-        DISPATCH_KIND(a->kind, { int r2 = launch_step_h<K>(*a, s); if (r2) return r2; });
-    }
-    return FSRL_OK;
+    // inline bookkeeping: no env's step depends on another env's, so all steps run in one launch
+    const char* per_step = getenv("FSRL_ROLLOUT_PER_STEP");
+    const bool one_launch = a->inline_done && !(per_step && atoi(per_step) != 0);
+    DISPATCH_KIND(a->kind, rc = launch_steps_h<K>(*a, n_steps, one_launch, s));
+    return rc;
 }
 
 extern "C" int fsrl_rollout_steps_act(const fsrl_rollout_t* a, const float* act, void* stream) {

@@ -44,6 +44,8 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--hidden", type=int, default=256)
     ap.add_argument("--tasks", default=",".join(TASKS))
+    ap.add_argument("--episodes", type=int, default=0,
+                    help="n_episode of each collect (default: --envs, one episode per env; more takes the resolve path)")
     a = ap.parse_args()
     import torch
     from helpers import build_ppo
@@ -52,20 +54,21 @@ def main():
     E = a.envs
     for task in a.tasks.split(","):
         policy, venv, buf, col = build_ppo(task, hidden=(a.hidden, a.hidden), n_env=E)
-        col.collect(n_episode=E)                    # warm-up
+        n_ep = a.episodes or E
+        col.collect(n_episode=n_ep)                 # warm-up
         times, steps = [], []
         for _ in range(a.reps):
             buf.reset()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             torch.cuda.synchronize()
             e0.record()
-            st = col.collect(n_episode=E)
+            st = col.collect(n_episode=n_ep)
             e1.record()
             torch.cuda.synchronize()
             times.append(e0.elapsed_time(e1))
             steps.append(int(st["n/st"]))
         i = min(range(len(times)), key=lambda k: times[k] / steps[k])
-        print(json.dumps(dict(task=task, envs=E, hidden=a.hidden, horizon=venv.max_episode_steps, D=venv.D, A=venv.A,
+        print(json.dumps(dict(task=task, envs=E, episodes=n_ep, hidden=a.hidden, horizon=venv.max_episode_steps, D=venv.D, A=venv.A,
                               env_steps=steps[i], ms=round(times[i], 3),
                               env_steps_per_s=round(steps[i] / (times[i] / 1e3)), terminated=st["terminated"],
                               ms_all=[round(t, 3) for t in times], gpu=name, power_limit=plimit)), flush=True)
