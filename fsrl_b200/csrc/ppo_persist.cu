@@ -19,9 +19,11 @@
 //       epilogue threads' registers for the whole launch, the updated tile is re-published as images W2A / W2B
 //   small parameters (W1, b1, b2, W3, b3, log sigma): every CTA keeps the slices it consumes (+ their
 //       Adam moments) in shared memory and applies the identical update to them (deterministic
-//       replicas); gradients are fixed-order sums of per-row-block partials.
-//   global-norm clip: per-CTA sums of squares -> one device-wide counter hop -> every CTA adds the
-//       96 partials in the same order.
+//       replicas).  Column block b's gradient slice is reduced once, by its REDUCER CTA (a = b >> 2, b): fixed-order
+//       sums of the b2 / W3 / b3 row-block partials (L2, by warpgroup 1 during G2) and of the 8 dW1 / db1 partials that
+//       the G2 CTAs of k block b >> 1 -- same cluster -- keep in their operand rings (read over DSMEM).
+//   global-norm clip: sums of squares of the reducers' slices and the G3 tiles -> one device-wide counter hop (D2)
+//       -> every CTA adds the 96 slots in the same order and reads its column block's final slice.
 // All operand images are K-major no-swizzle plane images (wgmma.cuh); transposed copies are written by the producer
 // (wgmma reads tf32 operands K-major only).
 //
@@ -31,7 +33,8 @@
 // rows through shared memory behind one 64-thread barrier per warp pair (stage_acc).
 // The 8 CTAs of a row block form a thread-block cluster: operand chunks that several of them need are multicast
 // from L2 once into all of them (copy_operand), their head partials travel over distributed shared memory
-// (st.async + mbarrier complete_tx); all other hops are flag lines in L2.  The grid is launched as clusters only: the
+// (st.async + mbarrier complete_tx), and so do the dW1 / db1 partials (remote mbarrier arrival, ld.shared::cluster);
+// all other hops are flag lines in L2.  The grid is launched as clusters only: the
 // gate (ppo_persist_supported) admits a shape only when all 4 x n_nets clusters can be co-resident, and everything it
 // rejects runs on the three-launch chain of ppo.cu.  The cross terms of the 3-term split
 // accumulate in their own registers.  With world > 1 the <DP = true> instantiation exchanges gradients itself over peer
@@ -68,13 +71,14 @@ enum { I_H1A_HI, I_H1A_LO, I_H1T_HI, I_H1T_LO, I_DZA_HI, I_DZA_LO, I_DZT_HI, I_D
 constexpr int DB2P_OFF = N_IMG * IMG;                           // [4 a][H]
 constexpr int DW3P_OFF = DB2P_OFF + 4 * H_;                     // [4 a][H][OUTP]
 constexpr int DB3P_OFF = DW3P_OFF + 4 * H_ * OUTP;              // [4 a][16]
-constexpr int DW1P_OFF = DB3P_OFF + 4 * 16;                     // [4 rb][MAXD + 1][H]
 constexpr int MAXD = 40;
-constexpr int NET_WS = DW1P_OFF + 4 * WQ * (MAXD + 1) * H_;   // [row block 4][warp-in-subpartition WQ][MAXD + 1][H]
+constexpr int NSMAX = (MAXD + 1) * 32 + 32 + 32 * OUTP + 16;    // floats of the largest small-parameter slice (SliceMap)
+constexpr int SLICE_OFF = DB3P_OFF + 4 * 16;                    // [8 b][NSMAX]: final gradient slices, written by the reducers
+constexpr int NET_WS = SLICE_OFF + 8 * NSMAX;
 constexpr int SUMSQ_FLOATS = 128;                               // global tail: per-CTA sums of squares
-// flag lines (32 unsigned each): per net A, C, D1; global D2
+// flag lines (32 unsigned each): per net A, C; global D2
 constexpr int FLAG_LINE = 32;
-constexpr int F_A = 0, F_C = 1, F_D1 = 2, F_PER_NET = 3;
+constexpr int F_A = 0, F_C = 1, F_PER_NET = 2;
 // The two cross terms a_lo b_hi + a_hi b_lo accumulate in their OWN registers and meet the a_hi b_hi sum only in the
 // epilogue: the cross terms are 2^-11 of the main ones, and a tensor-core accumulator add may drop low bits of a small
 // addend.  Same MMA count, 8 more accumulator registers per instruction column.
@@ -87,7 +91,6 @@ constexpr int F_A = 0, F_C = 1, F_D1 = 2, F_PER_NET = 3;
 // The tag word is XORed with a hash of the three payload words: a 16-byte vector store does NOT become visible atomically
 // to a concurrent 16-byte load on the receiving GPU (a torn packet would show the new tag next to a stale payload
 // word, i.e. one diverging parameter update; tools/dp_identity_check.py), so the receiver accepts a packet only if tag AND payload agree and simply polls again otherwise.
-constexpr int NSMAX = (MAXD + 1) * 32 + 32 + 32 * OUTP + 16;
 constexpr int TILE_PK = (64 * 64 / NEPI + 2) / 3;                // packets per thread of a 64 x 64 tile (16 floats -> 6)
 constexpr int TILE_FLOATS = TILE_PK * NEPI * 4;                  // [packet][thread][4]
 constexpr int SLICE_PK = (NSMAX + 2) / 3;
@@ -196,6 +199,16 @@ __device__ __forceinline__ void st_cluster4(uint32_t raddr, float4 v) {
 __device__ __forceinline__ void st_async4(uint32_t raddr, float4 v, uint32_t rbar) {
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.f32 [%0], {%1,%2,%3,%4}, [%5];"
                  ::"r"(raddr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "r"(rbar) : "memory");
+}
+__device__ __forceinline__ float ld_cluster(uint32_t raddr) {
+    float v;
+    asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(raddr) : "memory");
+    return v;
+}
+// remote mbarrier arrival with cluster-scope release: the CTA's shared-memory stores before it (ordered by a CTA barrier)
+// are visible to a peer that acquires the phase (mbar_wait_cluster) -- once per step, so the fence it implies is cheap
+__device__ __forceinline__ void mbar_arrive_release_cluster(uint32_t raddr) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
 }
 __device__ __forceinline__ bool mbar_wait_cluster(uint64_t* bar, uint32_t parity, long long timeout_cycles) {
     const long long t0 = clock64();
@@ -502,15 +515,15 @@ __device__ __noinline__ float dp_tile_finish(DpCtx d, size_t off, float* accs, i
     acc_st<C2>(accs, trow, cb2, g);
     return sq;
 }
-// small-parameter slices of one column block (n floats in shared memory): row block 0 pushes them to every rank, every
-// CTA of the column block replaces them by the rank-ordered mean (one hop: this exchange is on the step's critical path)
-__device__ __noinline__ void dp_slices(DpCtx d, size_t off_s, float* sp_g, int n, int et, bool push) {
+// small-parameter slice of one column block (n floats in shared memory), called by its reducer only: pushes the slice to
+// every rank and replaces it by the rank-ordered mean (one hop: this exchange is on the step's critical path); the other
+// CTAs of the column block read the mean from the reducer's published slice after hop D2
+__device__ __noinline__ void dp_slices(DpCtx d, size_t off_s, float* sp_g, int n, int et) {
     const int n3 = (n + 2) / 3;
     const float inv_world = 1.0f / (float)d.world;
-    if (push)
-        for (int i = et; i < n3; i += NEPI)
-            dp_push_all(d.xg, (size_t)d.me * d.region + off_s + 4 * (size_t)i, d.me, d.world,
-                        sp_g[3 * i], 3 * i + 1 < n ? sp_g[3 * i + 1] : 0.f, 3 * i + 2 < n ? sp_g[3 * i + 2] : 0.f, d.tag);
+    for (int i = et; i < n3; i += NEPI)
+        dp_push_all(d.xg, (size_t)d.me * d.region + off_s + 4 * (size_t)i, d.me, d.world,
+                    sp_g[3 * i], 3 * i + 1 < n ? sp_g[3 * i + 1] : 0.f, 3 * i + 2 < n ? sp_g[3 * i + 2] : 0.f, d.tag);
     const float* loc = d.xg[d.me];
     for (int i = et; i < n3; i += NEPI) {
         const float3 s3 = dp_gather(loc + off_s + 4 * (size_t)i, d.region, d.me, d.world, d.tag, sp_g[3 * i],
@@ -521,11 +534,27 @@ __device__ __noinline__ void dp_slices(DpCtx d, size_t off_s, float* sp_g, int n
     }
 }
 
+// Reducer of column block b's small-parameter gradient (CTA c = 8 a + b with a = b >> 2): the CTA of that column block
+// in the cluster whose G2 CTAs (k block b >> 1, CTAs 4 (b >> 1) .. + 3) produce its dW1 / db1 partials -- CTAs 0-3 and
+// 12-15 of each network.  Re-derived from blockIdx at each use rather than kept in a register: in <DP = true> a value
+// live across the exchange calls costs spill traffic.
+__device__ __forceinline__ bool red_cta() { return ((blockIdx.x >> 3) & 3) == ((blockIdx.x & 7) >> 2); }
+
+// the exchange part of the step tail behind one call site: G3 CTAs complete their W2 gradient tile with the ranks'
+// mean (returns its sum of squares), reducers replace their slice by the ranks' mean
+__device__ __noinline__ float dp_tail(DpCtx d, size_t off_t, size_t off_s, float* accs, float* sp_g, int n, int trow, int cb2,
+                                      int et, bool tile, bool slice) {
+    if (tile && !d.direct) dp_tile_reduce(d, off_t, accs, trow, cb2, et);
+    if (slice) dp_slices(d, off_s, sp_g, n, et);
+    __syncwarp();
+    return tile ? dp_tile_finish(d, off_t, accs, trow, cb2, et) : 0.f;
+}
+
 // DP = false: single-GPU instantiation without any of the exchange code (smaller instruction footprint)
 template <bool DP>
 __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    __shared__ __align__(8) uint64_t bar_full[NSLOT], bar_empty[NSLOT], bar_b;
+    __shared__ __align__(8) uint64_t bar_full[NSLOT], bar_empty[NSLOT], bar_b, bar_w1;
     __shared__ float s_red[4][320];          // cross-subpartition partial sums
     __shared__ float s_misc[32];
     __shared__ AdamS s_adam;
@@ -535,6 +564,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     const int net = blockIdx.x >> 5, c = blockIdx.x & 31, a = c >> 3, b = c & 7;
     const bool is_g2 = c < 16;
     const int ka = (c & 15) >> 2, q4 = c & 3;      // G2: (k block, row block) ; G3: (k block, o block)
+
     const int D = u.D, A = u.A, C = u.C, H = H_;
     const int out = (net == 0) ? A : 1;
     const int n_cta = 32 * u.n_nets;
@@ -556,6 +586,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
     if (tid == 0) {
         for (int i = 0; i < NSLOT; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 4 * 8); }
         mbar_init(&bar_b, 1);                // per step: one local expect_tx arrival + 16 KB of remote st.async bytes
+        mbar_init(&bar_w1, 4);               // reducers, per step: one arrival of each of the 4 G2 CTAs of k block b >> 1
         fence_mbar_init();
     }
     __syncthreads();
@@ -632,7 +663,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
         // W2 tiles travel in two hops (reduce-scatter + all-gather, 2 (W - 1) / W tile volumes per rank instead of W - 1):
         // packet q of epilogue warp w is OWNED by rank (6 w + q) mod W -- every rank sends it there, the owner sums the
         // ranks' packets in rank order and pushes the mean into everybody's result region (region 8).  Both hops are
-        // hidden behind the dW1 hop / slice reduction of the same step; the result is bit-identical on every rank.
+        // hidden behind the dW1 / slice reduction of the same step; the result is bit-identical on every rank.
         auto dp_ctx = [&](int t_) {
             DpCtx d;
             const unsigned long long id = (unsigned long long)(P.adam_t0 + t_ + 1);
@@ -974,6 +1005,52 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                     if (q < nx && e < 64 * D) { const int r = e / D; land[e + (r >> 5)] = xr[q]; }
                 }
             }
+            // reducers: warpgroup 1 would only wait for warpgroup 0's GEMM -- it sums the b2 / W3 / b3 / log sigma
+            // partials of slice b (complete since flag C) into sp_g meanwhile.  Each element: its 4 row-block partials
+            // in order a = 0 .. 3, starting from 0.
+            if (red_cta() && wq == 1) {
+                const int tw = et - 128;
+                if (tw == 0) {
+                    if (!flag_wait_ge(fl_net + F_C * FLAG_LINE, 32u * (t + 1), WAIT_CYCLES)) fail(P.err, 35);
+                    STAMP(15);
+                }
+                asm volatile("bar.sync 6, 128;" ::: "memory");
+                for (int i0 = sm.b2 + tw; i0 < sm.n; i0 += 4 * 128) {     // 4 elements x 4 partials in flight per thread
+                    float pv[4][4];
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int i = i0 + e * 128;
+                        const float* src = wsn;
+                        size_t stride = 0;
+                        bool real = false;
+                        if (i < sm.n) {
+                            if (i < sm.w3) { src = wsn + DB2P_OFF + 32 * b + (i - sm.b2); stride = H; real = true; }
+                            else if (i < sm.b3) {
+                                const int oo = (i - sm.w3) / OUTP, jj = (i - sm.w3) % OUTP;
+                                real = jj < out;
+                                src = wsn + DW3P_OFF + ((size_t)32 * b + oo) * OUTP + jj; stride = (size_t)H * OUTP;
+                            } else {
+                                const int jj = i - sm.b3;
+                                real = (jj < out) || (net == 0 && jj >= 8 && jj < 8 + A);
+                                src = wsn + DB3P_OFF + jj; stride = 16;
+                            }
+                        }
+#pragma unroll
+                        for (int q = 0; q < 4; ++q) pv[e][q] = real ? __ldcg(src + q * stride) : 0.f;
+                    }
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int i = i0 + e * 128;
+                        if (i < sm.n) {
+                            float gsum = 0.f;
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) gsum += pv[e][q];          // fixed order
+                            sp_g[i] = gsum;
+                        }
+                    }
+                }
+                if (tw == 0) STAMP(16);
+            }
             {
                 float dm[32], dc[32];
                 if (wq == 0) gemm_phase<64>(ring, qq, bar_full, empty_r, dm, dc, P.err, 32, lane);
@@ -983,31 +1060,36 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             if (et == 0) STAMP(6);
             float sq = 0.f;
             if (is_g2) {
-                // lane: k = 64 ka + trow ; rows cb2 + j of row block q4; partial set 2 q4 + wq (WQ sets per row block)
+                // lane: k = 64 ka + trow ; rows cb2 + j of row block q4; partial set 2 q4 + wq (WQ sets per row block).
+                // The partials stay in this CTA's operand ring, [wq][D + 1][64 k]: every chunk of this step's G2 has
+                // landed and been consumed, and no peer copies into the ring again before flag A of the next step.
                 float v[C2];
                 acc_ld<C2>(accs, trow, cb2, v);
-                const int k = 64 * ka + trow;
 #pragma unroll
                 for (int jq = 0; jq < C2; ++jq) v[jq] = ((mbits >> jq) & 1u) ? v[jq] : 0.f;
                 epi_bar();
                 if (et == 0) STAMP(22);
                 const float* xh = land + (size_t)cb2 * D + half;
-                float* dst = wsn + DW1P_OFF + (size_t)(WQ * q4 + wq) * (MAXD + 1) * H + k;
+                float* dst = reinterpret_cast<float*>(ring) + (size_t)wq * (D + 1) * 64 + trow;
                 for (int d = 0; d < D; ++d) {
                     float sacc = 0.f;
 #pragma unroll
                     for (int jq = 0; jq < C2; ++jq) sacc = fmaf(xh[jq * D + d], v[jq], sacc);
                     sacc += __shfl_xor_sync(0xffffffffu, sacc, 16);
-                    if (half == 0) dst[(size_t)d * H] = sacc;
+                    if (half == 0) dst[d * 64] = sacc;
                 }
                 float sb1 = 0.f;
 #pragma unroll
                 for (int jq = 0; jq < C2; ++jq) sb1 += v[jq];
                 sb1 += __shfl_xor_sync(0xffffffffu, sb1, 16);
-                if (half == 0) dst[(size_t)D * H] = sb1;          // db1
+                if (half == 0) dst[D * 64] = sb1;                 // db1
                 if (et == 0) STAMP(23);
                 epi_bar();
-                if (et == 0) flag_add_release(fl_net + F_D1 * FLAG_LINE);
+                // the reducers of column blocks 2 ka and 2 ka + 1 (cluster ranks = column blocks) may read them now
+                if (et == 0) {
+                    mbar_arrive_release_cluster(mapa_u32(smem_u32(&bar_w1), 2 * ka));
+                    mbar_arrive_release_cluster(mapa_u32(smem_u32(&bar_w1), 2 * ka + 1));
+                }
             } else {
                 float g[C2];
                 acc_ld<C2>(accs, trow, cb2, g);
@@ -1019,40 +1101,32 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                     for (int jq = 0; jq < C2; ++jq) sq = fmaf(g[jq], g[jq], sq);
                 }
             }
-            // ---- small-parameter gradients: fixed-order sums of the row-block partials.  The b2 / W3 / b3 partials
-            // are complete since flag C: they are summed while flag D1 (the dW1 partials) is still on its way.
-            auto reduce_slices = [&](int lo, int hi) {
-                for (int i0 = lo + et; i0 < hi; i0 += 4 * NEPI) {    // 4 elements x 4 partials in flight per thread
-                    float pv[4][4 * WQ];
-                    bool real[4];
-                    int np[4];
+            if (et == 0) STAMP(7);
+            // ---- small-parameter gradients (reducers): W1 / b1 = fixed-order sums of the 8 partials q = WQ rb + wq in the
+            // rings of the G2 CTAs 4 (b >> 1) + rb (cluster ranks (4 (b >> 1) + rb) & 7), read over distributed shared memory
+            if (red_cta()) {
+                if (!mbar_wait_cluster(&bar_w1, t & 1, WAIT_CYCLES)) fail(P.err, 33);
+                if (et == 0) STAMP(8);
+                const uint32_t ring_s = smem_u32(ring);
+                const int kb = 32 * (b & 1);                           // the slice's first k inside k block b >> 1
+                for (int i0 = et; i0 < sm.b2; i0 += 2 * NEPI) {       // 2 elements x 8 partials in flight per thread
+                    float pv[2][4 * WQ];
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) {
+                    for (int e = 0; e < 2; ++e) {
                         const int i = i0 + e * NEPI;
-                        const float* src = wsn;
-                        size_t stride = 0;
-                        real[e] = false;
-                        np[e] = 4;
-                        if (i < hi) {
-                            if (i < sm.b2) { src = wsn + DW1P_OFF + (size_t)(i / 32) * H + 32 * b + (i % 32); stride = (size_t)(MAXD + 1) * H; real[e] = true; np[e] = 4 * WQ; }
-                            else if (i < sm.w3) { src = wsn + DB2P_OFF + 32 * b + (i - sm.b2); stride = H; real[e] = true; }
-                            else if (i < sm.b3) {
-                                const int oo = (i - sm.w3) / OUTP, jj = (i - sm.w3) % OUTP;
-                                real[e] = jj < out;
-                                src = wsn + DW3P_OFF + ((size_t)32 * b + oo) * OUTP + jj; stride = (size_t)H * OUTP;
-                            } else {
-                                const int jj = i - sm.b3;
-                                real[e] = (jj < out) || (net == 0 && jj >= 8 && jj < 8 + A);
-                                src = wsn + DB3P_OFF + jj; stride = 16;
-                            }
-                        }
+                        const uint32_t off = 4u * (uint32_t)((i / 32) * 64 + kb + (i % 32));
 #pragma unroll
-                        for (int q = 0; q < 4 * WQ; ++q) pv[e][q] = (real[e] && q < np[e]) ? __ldcg(src + q * stride) : 0.f;
+                        for (int rb = 0; rb < 4; ++rb) {
+                            const uint32_t src = mapa_u32(ring_s + off, (uint32_t)((4 * (b >> 1) + rb) & 7));
+#pragma unroll
+                            for (int w = 0; w < WQ; ++w)
+                                pv[e][WQ * rb + w] = i < sm.b2 ? ld_cluster(src + 4u * (uint32_t)(w * (D + 1) * 64)) : 0.f;
+                        }
                     }
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) {
+                    for (int e = 0; e < 2; ++e) {
                         const int i = i0 + e * NEPI;
-                        if (i < hi) {
+                        if (i < sm.b2) {
                             float gsum = 0.f;
 #pragma unroll
                             for (int q = 0; q < 4 * WQ; ++q) gsum += pv[e][q];          // fixed order
@@ -1060,50 +1134,57 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                         }
                     }
                 }
-            };
-            reduce_slices(sm.b2, sm.n);
-            if (et == 0) { STAMP(7); if (!flag_wait_ge(fl_net + F_D1 * FLAG_LINE, 16u * (t + 1), WAIT_CYCLES)) fail(P.err, 33); STAMP(8); }
-            epi_bar();
-            reduce_slices(0, sm.b2);
+                epi_bar();                                    // sp_g complete (warpgroup 1 summed b2 .. n before the G2 epilogue)
+                if (et == 0) STAMP(17);
+            }
             if (DP) {
                 const DpCtx d = dp_ctx(t);
                 const size_t off_t = (size_t)(net * 16 + (c - 16)) * TILE_FLOATS + (size_t)et * 4;
-                epi_bar();                                    // sp_g complete
-                if (!is_g2 && !d.direct) { dp_tile_reduce(d, off_t, accs, trow, cb2, et); if (et == 0) STAMP(33); }
-                dp_slices(d, (size_t)u.n_nets * 16 * TILE_FLOATS + (size_t)(net * 8 + b) * SLICE_PK * 4, sp_g, sm.n, et, a == 0);
-                __syncwarp();
-                if (et == 0) STAMP(38);
-                if (!is_g2) { sq += dp_tile_finish(d, off_t, accs, trow, cb2, et); if (et == 0) STAMP(41); }
-                epi_bar();                                    // sp_g holds the global mean before the norm / Adam read it
+                sq += dp_tail(d, off_t, (size_t)u.n_nets * 16 * TILE_FLOATS + (size_t)(net * 8 + b) * SLICE_PK * 4, accs, sp_g, sm.n,
+                              trow, cb2, et, !is_g2, red_cta());
+                if (et == 0) STAMP(41);
+                epi_bar();                                    // sp_g holds the ranks' mean before the norm reads it
             }
-            // every small parameter is counted once in the norm: W1/b1/b2/W3 slices by row block 0, b3 / log sigma by CTA 0.
-            // (each thread re-reads only elements it wrote itself: same i = et + k NEPI mapping)
-            if (a == 0) {
+            if (red_cta()) {
+                // every small parameter is counted once in the norm: the W1/b1/b2/W3 slices by their reducers, b3 / log sigma
+                // by the reducer of b = 0.  The slice goes out to the other CTAs of the column block with it.
                 for (int i = et; i < sm.n; i += NEPI) {
                     bool real = true;
                     if (i >= sm.w3 && i < sm.b3) real = ((i - sm.w3) % OUTP) < out;
                     else if (i >= sm.b3) { const int jj = i - sm.b3; real = (jj < out) || (net == 0 && jj >= 8 && jj < 8 + A); }
                     if (real && (i < sm.b3 || b == 0)) sq = fmaf(sp_g[i], sp_g[i], sq);
+                    wsn[SLICE_OFF + (size_t)b * NSMAX + i] = sp_g[i];   // final gradient slice of column block b
                 }
             }
-            // ---- global gradient norm: per-CTA partial -> device-wide hop -> same summation order everywhere --
-            sq = warp_sum(sq);
-            if (lane == 0) s_misc[warp] = sq;
-            epi_bar();
-            if (et == 0) {
-                float tot = 0.f;
+            // ---- global gradient norm: per-CTA partials -> device-wide hop -> same summation order everywhere.  Slot
+            // 32 net + b holds column block b's slice (written by its reducer), slots 32 net + 16 .. 31 the W2 tiles; slots
+            // 32 net + 8 .. 15 stay +0 (zeroed at launch), so only 24 CTAs per network arrive.
+            if (red_cta() || !is_g2) {
+                sq = warp_sum(sq);
+                if (lane == 0) s_misc[warp] = sq;
+                epi_bar();
+                if (et == 0) {
+                    float tot = 0.f;
 #pragma unroll
-                for (int w2 = 0; w2 < NEPI / 32; ++w2) tot += s_misc[w2];
-                sumsq_g[blockIdx.x] = tot;
-                STAMP(9);
-                flag_add_release(fl_d2);
-                if (!flag_wait_ge(fl_d2, (unsigned)n_cta * (t + 1), WAIT_CYCLES)) fail(P.err, 34);
+                    for (int w2 = 0; w2 < NEPI / 32; ++w2) tot += s_misc[w2];
+                    sumsq_g[blockIdx.x - (red_cta() ? 8 * a : 0)] = tot;
+                    STAMP(9);
+                    flag_add_release(fl_d2);
+                }
+            }
+            if (et == 0) {
+                if (!flag_wait_ge(fl_d2, 24u * (unsigned)u.n_nets * (t + 1), WAIT_CYCLES)) fail(P.err, 34);
                 STAMP(10);
             }
             epi_bar();
             float nq[4];
 #pragma unroll
             for (int q = 0; q < 4; ++q) nq[q] = (lane + 32 * q < n_cta) ? __ldcg(sumsq_g + lane + 32 * q) : 0.f;
+            // the other CTAs of the column block fetch its final slice in the same round trip (each thread the elements
+            // it steps below: same i = et + k NEPI mapping, no barrier needed).  <DP = true> reads it inside the Adam loop
+            // instead: a separate pass there raises the register pressure of the whole step and with it the spills.
+            if (!DP && !red_cta())
+                for (int i = et; i < sm.n; i += NEPI) sp_g[i] = __ldcg(wsn + SLICE_OFF + (size_t)b * NSMAX + i);
             float nsq = ((nq[0] + nq[1]) + nq[2]) + nq[3];                          // identical order in every warp of the grid
             nsq = warp_sum(nsq);
             float gscale = 1.0f;
@@ -1114,7 +1195,8 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             // ---- clip + Adam: replicated small slices, then the owned W2 tile (registers) ------------------------
             for (int i = et; i < sm.n; i += NEPI) {
                 float m = sp_m[i], v = sp_v[i];
-                sp_p[i] = adam_one(sp_p[i], sp_g[i] * gscale, m, v, ad);
+                const float g = (DP && !red_cta()) ? __ldcg(wsn + SLICE_OFF + (size_t)b * NSMAX + i) : sp_g[i];
+                sp_p[i] = adam_one(sp_p[i], g * gscale, m, v, ad);
                 sp_m[i] = m; sp_v[i] = v;
             }
             if (et == 0) STAMP(25);
@@ -1220,7 +1302,8 @@ int ppo_persist_run(const fsrl_ppo_update_t& ug, int n_mb, int stats_slot0, long
     a.flags = reinterpret_cast<unsigned*>(ug.persist_ws + fl_off);
     const size_t n_flag_words = (size_t)(ug.n_nets * pp::F_PER_NET + 1) * pp::FLAG_LINE;
     a.err = reinterpret_cast<int*>(a.flags + n_flag_words);
-    FSRL_CUDA(cudaMemsetAsync(a.flags, 0, (n_flag_words + 32) * sizeof(unsigned), s));
+    // the per-CTA sums of squares (slots no CTA writes read +0), the flag lines and the error word
+    FSRL_CUDA(cudaMemsetAsync(ug.persist_ws + fl_off - pp::SUMSQ_FLOATS, 0, (pp::SUMSQ_FLOATS + n_flag_words + 32) * sizeof(float), s));
     // Adam bias corrections of every step, computed like torch.optim.Adam does (python doubles)
     float* tab_dev = reinterpret_cast<float*>(a.err + 32);
     static std::vector<float> tab;

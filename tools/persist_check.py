@@ -85,7 +85,7 @@ def main():
     # decode the images (they hold the operands of the LAST step = the only step)
     ws = policy._persist_ws.detach().cpu().numpy()
     from fsrl_b200 import _lib as _fl
-    lib_net_ws = int(_fl.lib.fsrl_ppo_persist_ws_floats(2, 8, 256)) - int(_fl.lib.fsrl_ppo_persist_ws_floats(1, 8, 256)) - 3 * 32 - 2 * 32 * 48
+    lib_net_ws = int(_fl.lib.fsrl_ppo_persist_ws_floats(2, 8, 256)) - int(_fl.lib.fsrl_ppo_persist_ws_floats(1, 8, 256)) - 2 * 32 - 2 * 32 * 48   # minus one network's flag lines (A, C) and stamp rows
     x = sub.obs.cpu().double().numpy()
     perm = None
     for net in range(3):
@@ -138,27 +138,34 @@ def main():
             print("  c2 epoch (2400 steps) %s: %.1f ms -> %.2f us / step" % ("persistent" if persist else "chain", dt * 1e3, dt * 1e6 / 2400))
         # per-phase clock stamps of one step in the middle of the epoch (FSRL_PPO_PERSIST_DBG=<step>)
         os.environ["FSRL_PPO_PERSIST_DBG"] = "1000"
+        policy2._persist_ws[-2 * 96 * 48:].zero_()          # stamps a CTA does not take stay 0 and are left out below
         run(policy2, batch2, 256, True, seed=5)
         del os.environ["FSRL_PPO_PERSIST_DBG"]
         ws = policy2._persist_ws.detach().cpu().numpy()
         dbg = ws[-2 * 96 * 48:].view(np.int64).reshape(96, 48)
         names = {1: "S done (h1 tile + W2 images)", 2: "G1 accumulators ready", 3: "head partial written", 4: "hop B passed",
-                 5: "dz2 + partials written", 6: "G2/G3 accumulators ready", 7: "G2/G3 epilogue done", 8: "flag D1 passed",
-                 9: "slices reduced, sumsq out", 10: "flag D2 passed", 11: "Adam done (step end)", 12: "[producer] flag A passed",
-                 13: "[producer] G1 copies issued", 14: "[producer] flag C passed", 22: "G2: mask applied",
-                 23: "G2: dW1 partial stored",
-                 24: "norm known", 25: "small slices stepped", 26: "head gathered, loss gradient", 27: "dz2 images stored",
-                 28: "partial sums exchanged"}
+                 5: "dz2 + partials written", 6: "G2/G3 accumulators ready", 7: "G2/G3 epilogue done",
+                 8: "[reducer] dW1 partials arrived", 9: "sumsq (+ slice) out", 10: "flag D2 passed",
+                 11: "Adam done (step end)", 12: "[producer] flag A passed", 13: "[producer] G1 copies issued",
+                 14: "[producer] flag C passed", 15: "[reducer wg1] flag C passed", 16: "[reducer wg1] b2/W3/b3 reduced",
+                 17: "[reducer] W1/b1 reduced (DSMEM)", 22: "G2: mask applied", 23: "G2: dW1 partial in smem",
+                 24: "norm known (+ slice read)", 25: "small slices stepped", 26: "head gathered, loss gradient",
+                 27: "dz2 images stored", 28: "partial sums exchanged"}
         rel = dbg - dbg[:, :1]
-        for grp, sel in (("G2 CTAs", [i for i in range(96) if i % 32 < 16]), ("G3 CTAs", [i for i in range(96) if i % 32 >= 16])):
+        red = lambda i: i % 32 < 16 and (i % 32) // 8 == (i % 8) // 4      # reducers: CTAs 0-3 and 12-15 of a network
+        for grp, sel in (("G2 reducer CTAs", [i for i in range(96) if red(i)]),
+                         ("other G2 CTAs", [i for i in range(96) if i % 32 < 16 and not red(i)]),
+                         ("G3 CTAs", [i for i in range(96) if i % 32 >= 16])):
             print("  --- %s: cycles since step start (mean / min / max over CTAs) ---" % grp)
             for i in sorted(names):
-                v = rel[sel, i]
-                print("    %2d %-34s %8.0f %8d %8d" % (i, names[i], v.mean(), v.min(), v.max()))
+                v = rel[sel, i][dbg[sel, i] != 0]
+                if len(v):
+                    print("    %2d %-34s %8.0f %8d %8d" % (i, names[i], v.mean(), v.min(), v.max()))
         for net in range(3):
             sel = list(range(32 * net, 32 * net + 32))
-            print("  net %d: dz2 done %6.0f  slices reduced %6.0f  step end %6.0f (mean cycles since step start)" % (
-                net, rel[sel, 5].mean(), rel[sel, 9].mean(), rel[sel, 11].mean()))
+            s9 = [i for i in sel if dbg[i, 9] != 0]
+            print("  net %d: dz2 done %6.0f  sumsq out %6.0f  step end %6.0f (mean cycles since step start)" % (
+                net, rel[sel, 5].mean(), rel[s9, 9].mean(), rel[sel, 11].mean()))
             print("         G1 ready %6.0f | head out %6.0f | B passed %6.0f | loss %6.0f | images %6.0f | sums %6.0f | C arrive %6.0f" % tuple(
                 rel[sel, i].mean() for i in (2, 3, 4, 26, 27, 28, 5)))
             b0 = [i for i in sel if i % 8 == 0]

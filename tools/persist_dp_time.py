@@ -26,6 +26,7 @@ def main():
         bench.one_cycle(trainer)
     torch.cuda.synchronize()
     os.environ["FSRL_PPO_PERSIST_DBG"] = "1000"
+    agent.policy._persist_ws[-2 * 96 * 48:].zero_()      # stamps a CTA does not take stay 0 and are left out below
     bench.one_cycle(trainer)
     torch.cuda.synchronize()
     del os.environ["FSRL_PPO_PERSIST_DBG"]
@@ -33,18 +34,21 @@ def main():
     dbg = ws[-2 * 96 * 48:].view(np.int64).reshape(96, 48)
     rel = dbg - dbg[:, :1]
     names = {1: "S done", 2: "G1 accumulators ready", 4: "hop B passed", 5: "dz2 + partials written", 6: "G2/G3 accumulators ready",
-             7: "G2/G3 epilogue done (own slices summed)", 8: "flag D1 passed", 32: "W2 tile pushed", 35: "slices pushed",
-             38: "slices summed (peers' packets in)", 41: "W2 tile summed (peers' packets in)", 9: "sumsq out",
+             7: "G2/G3 epilogue done", 8: "[reducer] dW1 partials arrived",
+             17: "[reducer] W1/b1 reduced (DSMEM)", 32: "W2 tile pushed",
+             41: "exchange done (W2 tile / slice: ranks' mean in)", 9: "sumsq (+ slice) out",
              10: "flag D2 passed", 11: "Adam done (step end)"}
+    red = lambda i: i % 32 < 16 and (i % 32) // 8 == (i % 8) // 4      # reducers: CTAs 0-3 and 12-15 of a network
     for r in range(world):
         if r == rank:
             print("=== rank %d ===" % rank)
-            for grp, sel in (("G2 CTAs, a == 0", [i for i in range(96) if i % 32 < 8]), ("G2 CTAs, a == 1", [i for i in range(96) if 8 <= i % 32 < 16]),
+            for grp, sel in (("G2 reducer CTAs", [i for i in range(96) if red(i)]),
+                             ("other G2 CTAs", [i for i in range(96) if i % 32 < 16 and not red(i)]),
                              ("G3 CTAs", [i for i in range(96) if i % 32 >= 16])):
                 print("  --- %s: cycles since step start (mean / min / max over CTAs) ---" % grp)
                 for i in names:
-                    v = rel[sel, i]
-                    if (np.abs(v) > 10 ** 9).any():
+                    v = rel[sel, i][dbg[sel, i] != 0]
+                    if len(v) == 0:
                         continue
                     print("    %2d %-40s %8.0f %8d %8d" % (i, names[i], v.mean(), v.min(), v.max()))
             cyc = (dbg[:, 29] - dbg[:, 0]) / 64.0
