@@ -204,6 +204,7 @@ SIGNATURES = {
     "fsrl_traj_gather": (c_int, [ctypes.POINTER(TrajArena), ctypes.POINTER(TrajArena), c_vp, c_int, c_vp]),
     "fsrl_mlp_forward": (c_int, [ctypes.POINTER(Mlp3), c_vp, c_vp, ctypes.c_longlong, c_vp, c_vp]),
     "fsrl_engine_slot_floats": (c_size, [c_int, c_int]),
+    "fsrl_engine_dx_ld": (c_int, []),
     "fsrl_engine_forward": (c_int, [ctypes.POINTER(Engine), ctypes.POINTER(NetList), ctypes.POINTER(EngInput), c_int, c_int, c_vp]),
     "fsrl_engine_backward": (c_int, [ctypes.POINTER(Engine), ctypes.POINTER(NetList), c_int, c_int, c_vp]),
     "fsrl_engine_wgrad": (c_int, [ctypes.POINTER(Engine), ctypes.POINTER(NetList), ctypes.POINTER(EngInput), c_int, c_int, c_vp, c_vp]),

@@ -443,6 +443,7 @@ static_assert(FSRL_ENG_MAX_NETS <= W2_MIRROR_MAX_NETS, "one mirror launch must c
 using namespace fsrl;
 
 extern "C" size_t fsrl_engine_slot_floats(int H, int bmax) { return eng_slot_floats(H, bmax); }
+extern "C" int fsrl_engine_dx_ld(void) { return FSRL_ENG_DX_LD; }
 
 extern "C" int fsrl_engine_forward(const fsrl_engine_t* e, const fsrl_netlist_t* nl,
                                    const fsrl_eng_input_t* in, int B, int save, void* stream) {

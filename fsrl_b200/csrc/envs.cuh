@@ -3,7 +3,7 @@
 //
 // The reference's physics engines are absent and irreproducible (SURVEY.md F5), so these are
 // OUR documented analytic models with the task structure of Bullet-Safety-Gym's Circle / Run
-// tasks and Safety-Gymnasium's Point / Car Circle and Goal tasks (dense reward, binary cost, fixed
+// tasks and Safety-Gymnasium's Point / Car Circle, Goal, Button and Push tasks (dense reward, binary cost, fixed
 // horizon; the Drone tasks also terminate on a crash or a flip, every other task is truncation
 // only).  Every arithmetic step
 // uses only IEEE-exact operations (+ - * / sqrt, no FMA contraction, polynomial sin/cos), so
@@ -18,13 +18,14 @@
 namespace fsrl {
 
 // Kinds 0-8 are the Bullet-Safety-Gym tasks and PointGoal1; the Safety-Gymnasium navigation family
-// starts at 16.  Ids 9-15 are unassigned.
+// starts at 16.  Ids 9-15 and 23 are unassigned.
 enum EnvKind { ENV_CAR_CIRCLE = 0, ENV_CAR_RUN = 1, ENV_BALL_CIRCLE = 2, ENV_BALL_RUN = 3,
                ENV_ANT_CIRCLE = 4, ENV_POINT_GOAL = 5, ENV_ANT_RUN = 6, ENV_DRONE_CIRCLE = 7,
                ENV_DRONE_RUN = 8, ENV_POINT_CIRCLE1 = 16, ENV_POINT_CIRCLE2 = 17, ENV_CAR_CIRCLE1 = 18,
-               ENV_CAR_CIRCLE2 = 19, ENV_POINT_GOAL2 = 20, ENV_CAR_GOAL1 = 21, ENV_CAR_GOAL2 = 22 };
+               ENV_CAR_CIRCLE2 = 19, ENV_POINT_GOAL2 = 20, ENV_CAR_GOAL1 = 21, ENV_CAR_GOAL2 = 22,
+               ENV_POINT_BUTTON1 = 24, ENV_POINT_BUTTON2 = 25, ENV_CAR_BUTTON1 = 26, ENV_CAR_BUTTON2 = 27,
+               ENV_POINT_PUSH1 = 28, ENV_POINT_PUSH2 = 29, ENV_CAR_PUSH1 = 30, ENV_CAR_PUSH2 = 31 };
 
-constexpr int ENV_MAX_D = 64;
 constexpr int ENV_MAX_A = 8;
 constexpr int ENV_MAX_S = 32;
 
@@ -99,6 +100,16 @@ constexpr float CAR_VW = 1.0f, CAR_AL = 0.2f, TRACK = 0.5f;    // Car: top wheel
 constexpr float CIRC_R = 1.5f, WALL = 1.125f, START = 0.8f;    // Circle: circle radius, walls, reset box
 constexpr float VASE_R = 0.25f;                                // Goal2: robot-vase contact distance
 }
+namespace button {   // Button1 / Button2; hazards use pgoal::HAZ_R
+constexpr float BUTTON_R = 0.2f, GREM_R = 0.2f;     // robot-button and robot-gremlin contact distances
+constexpr float GREM_W = 1.0f, GREM_TRAVEL = 0.35f; // gremlin orbit: angular speed (rad/s) and radius
+constexpr int DELAY = 10;                           // steps the buttons stay hidden and inert after a press
+}
+namespace push {     // Push1 / Push2; the goal uses pgoal::GOAL_R
+constexpr float PUSH_D = 0.3f;                      // robot-box centre distance on contact (robot + box radius)
+constexpr float HAZ_R = 0.3f, PILLAR_R = 0.4f;      // robot-hazard and robot-pillar contact distances
+constexpr float BOX_START = 1.0f;                   // the box starts in [-BOX_START, BOX_START]^2
+}
 
 struct EnvDims { int D, A, S, T; };
 
@@ -117,6 +128,10 @@ __host__ __device__ inline EnvDims env_dims(int kind) {
             return {28, 2, 7, 500};
         case ENV_POINT_GOAL2: case ENV_CAR_GOAL2: return {60, 2, 10, 1000};
         case ENV_CAR_GOAL1: return {60, 2, 28, 1000};
+        case ENV_POINT_BUTTON1: case ENV_POINT_BUTTON2: case ENV_CAR_BUTTON1: case ENV_CAR_BUTTON2:
+            return {76, 2, 12, 1000};
+        case ENV_POINT_PUSH1: case ENV_CAR_PUSH1: return {76, 2, 18, 1000};
+        case ENV_POINT_PUSH2: case ENV_CAR_PUSH2: return {76, 2, 28, 1000};
         default: return {0, 0, 0, 0};
     }
 }
@@ -631,6 +646,23 @@ __device__ __forceinline__ void lidar_world(float* bins, float ox, float oy, flo
     lidar_add(bins, xa(xm(c, dx), xm(s, dy)), xs(xm(c, dy), xm(s, dx)));
 }
 
+// the robot's pose at reset on the Goal, Button and Push tasks: position in [-0.5, 0.5]^2, heading towards a
+// point of the square, at rest (x, y, c, s, v, w = draw 0 of the reset's Philox stream)
+__device__ __forceinline__ void nav_reset_pose(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
+    uint32_t r[4];
+    Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
+    st[0] = xm(usym(r[0]), 0.5f);
+    st[1] = xm(usym(r[1]), 0.5f);
+    heading_from_box(usym(r[2]), usym(r[3]), st[2], st[3]);
+    st[4] = 0.0f; st[5] = 0.0f;
+}
+
+// the squared distance from the robot (x, y) to the point (ox, oy)
+__device__ __forceinline__ float nav_dist2(float ox, float oy, float x, float y) {
+    const float dx = xs(ox, x), dy = xs(oy, y);
+    return xa(xm(dx, dx), xm(dy, dy));
+}
+
 // Circle (D = 28, A = 2, T = 500): the 12 channels, then a 16-bin lidar towards the circle's centre.
 // Reward is Safety-Gymnasium's 0.1 * (x*vy - y*vx) / (r * (1 + |r - R|)), with r kept away from 0.
 // Cost 1 outside the walls: |x| > WALL at level 1, |x| or |y| > WALL at level 2.  The walls do not
@@ -712,12 +744,7 @@ struct NavGoal {
     }
     __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
         using namespace pgoal;
-        uint32_t r[4];
-        Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
-        st[0] = xm(usym(r[0]), 0.5f);
-        st[1] = xm(usym(r[1]), 0.5f);
-        heading_from_box(usym(r[2]), usym(r[3]), st[2], st[3]);
-        st[4] = 0.0f; st[5] = 0.0f;
+        nav_reset_pose(st, seed, env, ep);
         sample_goal(st, seed, env, ep, 0u);
         st[8] = 0.0f;
         if constexpr (LEVEL == 1) {
@@ -772,6 +799,221 @@ struct NavGoal {
     }
 };
 
+// Button (D = 76, A = 2, T = 1000): 4 buttons, one of them the goal; hazards and gremlins (level 1: 4 and 4,
+// level 2: 8 and 6), all drawn in the arena at reset.  The layout does not fit ENV_MAX_S beside the dynamic
+// state, so step / observe regenerate it from the reset's Philox stream at both levels: draws 1-2 hold the
+// buttons, draws 3, 4, ... the hazards and then the gremlins' orbit centres, two (x, y) pairs per draw.
+//   Gremlins orbit their centre at radius GREM_TRAVEL.  One unit phase (pc, ps) advances by GREM_W * DT per step
+//   (rotate_heading); gremlin k sits at the phase turned by (k mod 4) quarter-turns, gremlins 4-5 use the
+//   mirrored phase (pc, -ps) and orbit the other way.
+//   Step: reward = the distance progress towards the goal button.  A live step (timer 0) with the robot within
+//   BUTTON_R of the goal presses it: +1, the count goes up, the buttons go hidden and inert for DELAY steps and
+//   the goal moves to one of the other three buttons, (goal + 1 + r % 3) % 4 with r from the goal stream at
+//   16 + count.  While the timer runs it counts down and nothing presses.  Then the gremlins move.
+//   Cost 1 within pgoal::HAZ_R of a hazard, within GREM_R of a gremlin, or, on a live step, within BUTTON_R
+//   of a button other than the step's goal.
+//   Observation: the 12 channels, then 16-bin lidars of the goal button | all buttons (zero while the timer
+//   runs) | gremlins | hazards.  The arena walls clamp the robot; gremlins may orbit past them.
+// state: x, y, c, s, v, w, v_prev, goal, count, timer, pc, ps
+template <bool CAR, int LEVEL>
+struct NavButton {
+    static constexpr int D = 76, A = 2, S = 12, T = 1000;
+    static constexpr int NHAZ = LEVEL == 1 ? 4 : 8, NGREM = LEVEL == 1 ? 4 : 6;
+    static_assert((NHAZ + NGREM) % 2 == 0, "two objects per Philox draw");
+
+    __device__ static void buttons(uint32_t seed, uint32_t env, uint32_t ep, float (&bx)[4], float (&by)[4]) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            uint32_t q[4];
+            Philox::gen(env, ep, 1u + h, 0u, seed, KEY_RESET, q);
+            bx[2 * h] = xm(usym(q[0]), pgoal::ARENA); by[2 * h] = xm(usym(q[1]), pgoal::ARENA);
+            bx[2 * h + 1] = xm(usym(q[2]), pgoal::ARENA); by[2 * h + 1] = xm(usym(q[3]), pgoal::ARENA);
+        }
+    }
+    // f(gremlin, x, y) for every hazard, then every gremlin at the phase held in the state
+    template <typename F>
+    __device__ static void hazards_gremlins(const float* st, uint32_t seed, uint32_t env, uint32_t ep, F&& f) {
+        const float pc = st[10], ps = st[11];
+#pragma unroll
+        for (int h = 0; h < (NHAZ + NGREM) / 2; ++h) {
+            uint32_t q[4];
+            Philox::gen(env, ep, 3u + h, 0u, seed, KEY_RESET, q);
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const int k = 2 * h + j;
+                const float ox = xm(usym(q[2 * j]), pgoal::ARENA), oy = xm(usym(q[2 * j + 1]), pgoal::ARENA);
+                if (k < NHAZ) {
+                    f(false, ox, oy);
+                    continue;
+                }
+                const int g = k - NHAZ;
+                const float qs = g >= 4 ? -ps : ps;
+                const float ux = (g & 3) == 0 ? pc : (g & 3) == 1 ? -qs : (g & 3) == 2 ? -pc : qs;
+                const float uy = (g & 3) == 0 ? qs : (g & 3) == 1 ? pc : (g & 3) == 2 ? -qs : -pc;
+                f(true, xa(ox, xm(button::GREM_TRAVEL, ux)), xa(oy, xm(button::GREM_TRAVEL, uy)));
+            }
+        }
+    }
+    __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
+        nav_reset_pose(st, seed, env, ep);
+        st[6] = 0.0f;
+        uint32_t g[4];
+        Philox::gen(env, ep, 0u, 0u, seed, KEY_GOAL, g);
+        st[7] = (float)(g[0] % 4u);
+        st[8] = 0.0f; st[9] = 0.0f;
+        heading_from_box(usym(g[1]), usym(g[2]), st[10], st[11]);
+    }
+    __device__ static void observe(const float* st, float* o, uint32_t seed, uint32_t env, uint32_t ep) {
+        const float x = st[0], y = st[1], c = st[2], s = st[3];
+        nav_sensors(o, st[4], st[5], st[6], c, s);
+        float* gl = o + 12; float* bl = o + 28; float* ml = o + 44; float* hl = o + 60;
+#pragma unroll
+        for (int k = 0; k < 16; ++k) { gl[k] = 0.0f; bl[k] = 0.0f; ml[k] = 0.0f; hl[k] = 0.0f; }
+        float bx[4], by[4];
+        buttons(seed, env, ep, bx, by);
+        const int goal = (int)st[7];
+        const bool live = st[9] == 0.0f;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+            if (b == goal) lidar_world(gl, bx[b], by[b], x, y, c, s);
+            if (live) lidar_world(bl, bx[b], by[b], x, y, c, s);
+        }
+        hazards_gremlins(st, seed, env, ep, [&](bool grem, float ox, float oy) { lidar_world(grem ? ml : hl, ox, oy, x, y, c, s); });
+    }
+    __device__ static void step(float* st, const float* a, uint32_t seed, uint32_t env, uint32_t ep,
+                                float& rew, float& cost, bool& term) {
+        using namespace button;
+        float bx[4], by[4];
+        buttons(seed, env, ep, bx, by);
+        const int goal = (int)st[7];
+        float gx = bx[0], gy = by[0];
+#pragma unroll
+        for (int b = 1; b < 4; ++b)
+            if (b == goal) { gx = bx[b]; gy = by[b]; }
+        const float dist_old = xq(nav_dist2(gx, gy, st[0], st[1]));
+        st[6] = st[4];
+        nav_advance<CAR>(st, a);
+        st[0] = fminf(pgoal::ARENA, fmaxf(-pgoal::ARENA, st[0]));
+        st[1] = fminf(pgoal::ARENA, fmaxf(-pgoal::ARENA, st[1]));
+        const float dist = xq(nav_dist2(gx, gy, st[0], st[1]));
+        rew = xs(dist_old, dist);
+        const bool live = st[9] == 0.0f;
+        if (!live) {
+            st[9] = xs(st[9], 1.0f);
+        } else if (dist <= BUTTON_R) {
+            rew = xa(rew, 1.0f);
+            st[8] = xa(st[8], 1.0f);
+            st[9] = (float)DELAY;
+            uint32_t r[4];
+            Philox::gen(env, ep, 16u + (uint32_t)st[8], 0u, seed, KEY_GOAL, r);
+            st[7] = (float)((goal + 1 + (int)(r[0] % 3u)) & 3);
+        }
+        rotate_heading(st[10], st[11], GREM_W * pgoal::DT);
+        float c = 0.0f;
+#pragma unroll
+        for (int b = 0; b < 4; ++b)
+            if (live && b != goal && nav_dist2(bx[b], by[b], st[0], st[1]) <= BUTTON_R * BUTTON_R) c = 1.0f;
+        hazards_gremlins(st, seed, env, ep, [&](bool grem, float ox, float oy) {
+            const float d2 = nav_dist2(ox, oy, st[0], st[1]);
+            if (grem ? d2 <= GREM_R * GREM_R : d2 <= pgoal::HAZ_R * pgoal::HAZ_R) c = 1.0f;
+        });
+        cost = c;
+        term = false;
+    }
+};
+
+// Push (D = 76, A = 2, T = 1000): one box, one goal, hazards and pillars (level 1: 2 and 1, level 2: 4 and 4).
+// The layout fits the state: reset draws the box in [-BOX_START, BOX_START]^2 and the hazards and pillars in
+// the arena from draws 1, 2, ... of its Philox stream, two (x, y) pairs per draw; the goal comes from the goal
+// stream as on the Goal tasks.
+//   The box is pushed kinematically: after the robot moves (and is clamped), a box closer than PUSH_D to it
+//   moves along the unit vector robot -> box (the robot's heading at zero distance) until it is PUSH_D away,
+//   then is clamped to the arena.  The robot is not slowed; pillars block neither the robot nor the box.
+//   Reward = the robot-box distance progress + the box-goal distance progress; a box centre within
+//   pgoal::GOAL_R of the goal adds +1 and re-draws the goal (goal stream, 16 + count).
+//   Cost 1 within HAZ_R of a hazard and, at level 2 only, within PILLAR_R of a pillar.
+//   Observation: the 12 channels, then 16-bin lidars of the goal | box | hazards | pillars.
+// state: x, y, c, s, v, w, gx, gy, goal_count, bx, by, haz[NHAZ][2], pillar[NPIL][2], v_prev
+template <bool CAR, int LEVEL>
+struct NavPush {
+    static constexpr int NHAZ = LEVEL == 1 ? 2 : 4, NPIL = LEVEL == 1 ? 1 : 4;
+    static constexpr int HAZ0 = 11, PIL0 = HAZ0 + 2 * NHAZ, VPREV = PIL0 + 2 * NPIL;
+    static constexpr int D = 76, A = 2, S = VPREV + 1, T = 1000;
+    static_assert(S <= ENV_MAX_S, "env state too large");
+
+    __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
+        nav_reset_pose(st, seed, env, ep);
+        NavGoal<CAR, LEVEL>::sample_goal(st, seed, env, ep, 0u);
+        st[8] = 0.0f;
+        // object k (0: the box, then the hazards, then the pillars) at st[9 + 2k], st[10 + 2k]
+        constexpr int NOBJ = 1 + NHAZ + NPIL;
+#pragma unroll
+        for (int h = 0; h < (NOBJ + 1) / 2; ++h) {
+            uint32_t q[4];
+            Philox::gen(env, ep, 1u + h, 0u, seed, KEY_RESET, q);
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const int k = 2 * h + j;
+                if (k >= NOBJ) continue;
+                const float sc = k == 0 ? push::BOX_START : pgoal::ARENA;
+                st[9 + 2 * k] = xm(usym(q[2 * j]), sc);
+                st[10 + 2 * k] = xm(usym(q[2 * j + 1]), sc);
+            }
+        }
+        st[VPREV] = 0.0f;
+    }
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
+        const float x = st[0], y = st[1], c = st[2], s = st[3];
+        nav_sensors(o, st[4], st[5], st[VPREV], c, s);
+        float* gl = o + 12; float* bl = o + 28; float* hl = o + 44; float* pl = o + 60;
+#pragma unroll
+        for (int k = 0; k < 16; ++k) { gl[k] = 0.0f; bl[k] = 0.0f; hl[k] = 0.0f; pl[k] = 0.0f; }
+        lidar_world(gl, st[6], st[7], x, y, c, s);
+        lidar_world(bl, st[9], st[10], x, y, c, s);
+#pragma unroll
+        for (int h = 0; h < NHAZ; ++h) lidar_world(hl, st[HAZ0 + 2 * h], st[HAZ0 + 2 * h + 1], x, y, c, s);
+#pragma unroll
+        for (int p = 0; p < NPIL; ++p) lidar_world(pl, st[PIL0 + 2 * p], st[PIL0 + 2 * p + 1], x, y, c, s);
+    }
+    __device__ static void step(float* st, const float* a, uint32_t seed, uint32_t env, uint32_t ep,
+                                float& rew, float& cost, bool& term) {
+        using namespace push;
+        const float rb_old = xq(nav_dist2(st[9], st[10], st[0], st[1]));
+        const float bg_old = xq(nav_dist2(st[6], st[7], st[9], st[10]));
+        st[VPREV] = st[4];
+        nav_advance<CAR>(st, a);
+        const float x = fminf(pgoal::ARENA, fmaxf(-pgoal::ARENA, st[0]));
+        const float y = fminf(pgoal::ARENA, fmaxf(-pgoal::ARENA, st[1]));
+        st[0] = x; st[1] = y;
+        const float dx = xs(st[9], x), dy = xs(st[10], y);
+        const float d = xq(xa(xm(dx, dx), xm(dy, dy)));
+        if (d < PUSH_D) {
+            const float ux = d == 0.0f ? st[2] : xd(dx, d), uy = d == 0.0f ? st[3] : xd(dy, d);
+            st[9] = fminf(pgoal::ARENA, fmaxf(-pgoal::ARENA, xa(x, xm(PUSH_D, ux))));
+            st[10] = fminf(pgoal::ARENA, fmaxf(-pgoal::ARENA, xa(y, xm(PUSH_D, uy))));
+        }
+        const float rb = xq(nav_dist2(st[9], st[10], x, y));
+        const float bg = xq(nav_dist2(st[6], st[7], st[9], st[10]));
+        rew = xa(xs(rb_old, rb), xs(bg_old, bg));
+        if (bg <= pgoal::GOAL_R) {
+            rew = xa(rew, 1.0f);
+            st[8] = xa(st[8], 1.0f);
+            NavGoal<CAR, LEVEL>::sample_goal(st, seed, env, ep, 16u + (uint32_t)st[8]);
+        }
+        float c = 0.0f;
+#pragma unroll
+        for (int h = 0; h < NHAZ; ++h)
+            if (nav_dist2(st[HAZ0 + 2 * h], st[HAZ0 + 2 * h + 1], x, y) <= HAZ_R * HAZ_R) c = 1.0f;
+        if constexpr (LEVEL == 2) {
+#pragma unroll
+            for (int p = 0; p < NPIL; ++p)
+                if (nav_dist2(st[PIL0 + 2 * p], st[PIL0 + 2 * p + 1], x, y) <= PILLAR_R * PILLAR_R) c = 1.0f;
+        }
+        cost = c;
+        term = false;
+    }
+};
+
 template <> struct Env<ENV_POINT_GOAL> : NavGoal<false, 1> {};
 template <> struct Env<ENV_POINT_CIRCLE1> : NavCircle<false, 1> {};
 template <> struct Env<ENV_POINT_CIRCLE2> : NavCircle<false, 2> {};
@@ -780,5 +1022,13 @@ template <> struct Env<ENV_CAR_CIRCLE2> : NavCircle<true, 2> {};
 template <> struct Env<ENV_POINT_GOAL2> : NavGoal<false, 2> {};
 template <> struct Env<ENV_CAR_GOAL1> : NavGoal<true, 1> {};
 template <> struct Env<ENV_CAR_GOAL2> : NavGoal<true, 2> {};
+template <> struct Env<ENV_POINT_BUTTON1> : NavButton<false, 1> {};
+template <> struct Env<ENV_POINT_BUTTON2> : NavButton<false, 2> {};
+template <> struct Env<ENV_CAR_BUTTON1> : NavButton<true, 1> {};
+template <> struct Env<ENV_CAR_BUTTON2> : NavButton<true, 2> {};
+template <> struct Env<ENV_POINT_PUSH1> : NavPush<false, 1> {};
+template <> struct Env<ENV_POINT_PUSH2> : NavPush<false, 2> {};
+template <> struct Env<ENV_CAR_PUSH1> : NavPush<true, 1> {};
+template <> struct Env<ENV_CAR_PUSH2> : NavPush<true, 2> {};
 
 }  // namespace fsrl

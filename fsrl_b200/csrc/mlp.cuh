@@ -32,7 +32,6 @@ constexpr int MLP_TPB = 256;
 constexpr int MLP_KC = 16;          // k-rows of a weight matrix per pipeline stage
 constexpr int MLP_NST = 4;          // pipeline stages in flight (L2 latency x bandwidth ~ 64 KB per SM)
 constexpr int MLP_MAX_OUT = 16;
-constexpr int MLP_MAX_IN = 64;
 
 template <int H>
 struct MlpTile {

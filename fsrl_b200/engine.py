@@ -10,6 +10,8 @@ import torch
 from . import _lib
 from .nets import Arena, NetSlot
 
+DX_LD = _lib.lib.fsrl_engine_dx_ld()   # row stride of the 'dx' region, and the widest input a net may have
+
 
 class EngineCtx:
     def __init__(self, arena: Arena, bmax: int, extra_slots: int = 0):
@@ -55,14 +57,14 @@ class EngineCtx:
         return nl
 
     def slot_view(self, s: NetSlot, what: str) -> torch.Tensor:
-        """torch view of a scratch region: 'out' / 'dout' [bmax,16], 'dx' [bmax,64],
+        """torch view of a scratch region: 'out' / 'dout' [bmax,16], 'dx' [bmax,FSRL_ENG_DX_LD],
         'h1','h2','dz1','dz2' [bmax,H]."""
         i = self._index[id(s)]
         base = i * self.slot_floats
         bh = self.bmax * self.H
         offs = {"h1": 0, "h2": bh, "dz1": 2 * bh, "dz2": 3 * bh, "out": 4 * bh,
                 "dout": 4 * bh + self.bmax * 16, "dx": 4 * bh + 2 * self.bmax * 16}
-        width = {"out": 16, "dout": 16, "dx": 64}.get(what, self.H)
+        width = {"out": 16, "dout": 16, "dx": DX_LD}.get(what, self.H)
         o = base + offs[what]
         return self.scratch[o:o + self.bmax * width].view(self.bmax, width)
 

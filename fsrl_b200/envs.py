@@ -28,6 +28,10 @@ KINDS = {
     "SafetyPointCircle1Gymnasium-v0": 16, "SafetyPointCircle2Gymnasium-v0": 17,
     "SafetyCarCircle1Gymnasium-v0": 18, "SafetyCarCircle2Gymnasium-v0": 19,
     "SafetyPointGoal2Gymnasium-v0": 20, "SafetyCarGoal1Gymnasium-v0": 21, "SafetyCarGoal2Gymnasium-v0": 22,
+    "SafetyPointButton1Gymnasium-v0": 24, "SafetyPointButton2Gymnasium-v0": 25,
+    "SafetyCarButton1Gymnasium-v0": 26, "SafetyCarButton2Gymnasium-v0": 27,
+    "SafetyPointPush1Gymnasium-v0": 28, "SafetyPointPush2Gymnasium-v0": 29,
+    "SafetyCarPush1Gymnasium-v0": 30, "SafetyCarPush2Gymnasium-v0": 31,
 }
 
 

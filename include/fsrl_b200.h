@@ -85,9 +85,12 @@ enum { FSRL_BOUND_NONE = 0, FSRL_BOUND_CLIP = 1, FSRL_BOUND_TANH = 2 };
 enum { FSRL_ENV_CAR_CIRCLE = 0, FSRL_ENV_CAR_RUN = 1, FSRL_ENV_BALL_CIRCLE = 2,
        FSRL_ENV_BALL_RUN = 3, FSRL_ENV_ANT_CIRCLE = 4, FSRL_ENV_POINT_GOAL = 5,
        FSRL_ENV_ANT_RUN = 6, FSRL_ENV_DRONE_CIRCLE = 7, FSRL_ENV_DRONE_RUN = 8,
-       /* Safety-Gymnasium navigation family; 9-15 are unassigned */
+       /* Safety-Gymnasium navigation family; 9-15 and 23 are unassigned */
        FSRL_ENV_POINT_CIRCLE1 = 16, FSRL_ENV_POINT_CIRCLE2 = 17, FSRL_ENV_CAR_CIRCLE1 = 18,
-       FSRL_ENV_CAR_CIRCLE2 = 19, FSRL_ENV_POINT_GOAL2 = 20, FSRL_ENV_CAR_GOAL1 = 21, FSRL_ENV_CAR_GOAL2 = 22 };
+       FSRL_ENV_CAR_CIRCLE2 = 19, FSRL_ENV_POINT_GOAL2 = 20, FSRL_ENV_CAR_GOAL1 = 21, FSRL_ENV_CAR_GOAL2 = 22,
+       FSRL_ENV_POINT_BUTTON1 = 24, FSRL_ENV_POINT_BUTTON2 = 25, FSRL_ENV_CAR_BUTTON1 = 26,
+       FSRL_ENV_CAR_BUTTON2 = 27, FSRL_ENV_POINT_PUSH1 = 28, FSRL_ENV_POINT_PUSH2 = 29, FSRL_ENV_CAR_PUSH1 = 30,
+       FSRL_ENV_CAR_PUSH2 = 31 };
 
 /* per-collect statistics, device resident; the keys of collect()'s result dict
  * (fast_collector.py:399-408) are derived from it on the host */
@@ -298,12 +301,12 @@ int fsrl_mlp_forward(const fsrl_mlp3_t* net, const float* x, const int* idx, lon
  * (fsrl/policy/sac_lag.py:185-258, ddpg_lag.py:165-213, cpo.py:147-162) and soft_update
  * (fsrl/policy/base_policy.py:220-224).  Networks live in the flat arena (layout as for
  * fsrl_ppo_update_t); each has a scratch slot of fsrl_engine_slot_floats(H, bmax) floats:
- *   h1 | h2 | dz1 | dz2 : [bmax][H],  out | dout : [bmax][16],  dx : [bmax][64]
+ *   h1 | h2 | dz1 | dz2 : [bmax][H],  out | dout : [bmax][16],  dx : [bmax][FSRL_ENG_DX_LD]
  * forward writes `out` (+ h1, h2 when save != 0); the caller fills `dout` (d loss / d head
  * output, columns [out, out+n_extra) = d loss / d extra parameters); backward produces dz1,
  * dz2 (+ dx = d loss / d input); wgrad reduces them into `grad`; adam applies them. */
 #define FSRL_ENG_MAX_NETS 8
-#define FSRL_ENG_DX_LD 64
+#define FSRL_ENG_DX_LD 80   /* the widest input a net may have (obs + act of the widest task: 76 + 2) */
 typedef struct fsrl_netref {
     long long off;      /* start of the net inside theta / grad / adam_m / adam_v */
     long long w2n_off;  /* start of its W2 mirror inside w2n */
@@ -328,6 +331,7 @@ typedef struct fsrl_eng_input {
 } fsrl_eng_input_t;
 
 size_t fsrl_engine_slot_floats(int H, int bmax);
+int fsrl_engine_dx_ld(void); /* FSRL_ENG_DX_LD: the row stride of dx, and the widest input */
 int fsrl_engine_forward(const fsrl_engine_t* e, const fsrl_netlist_t* nets, const fsrl_eng_input_t* in,
                         int B, int save, void* stream);
 int fsrl_engine_backward(const fsrl_engine_t* e, const fsrl_netlist_t* nets, int B, int want_dx, void* stream);

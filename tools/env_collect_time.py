@@ -1,6 +1,6 @@
 """Time collect-only env-steps/s of every device environment.
 
-For each of the sixteen tasks a PPO-Lagrangian actor 2x256 (2 x --hidden) collects one episode in each of 2048 envs
+For each task (every device environment by default) a PPO-Lagrangian actor 2x256 (2 x --hidden) collects one episode in each of 2048 envs
 (FastCollector.collect(n_episode=2048), the inline path); the collect is timed with CUDA events after a
 warm-up collect, the best of --reps.  An env-step is one stored transition (the collect's ``n/st``), so
 the Drone tasks, whose episodes end early on a crash, report the rate of the steps actually taken.  The
@@ -22,7 +22,9 @@ TASKS = ["SafetyCarCircle-v0", "SafetyCarRun-v0", "SafetyBallCircle-v0", "Safety
          "SafetyPointGoal1Gymnasium-v0", "SafetyAntRun-v0", "SafetyDroneCircle-v0", "SafetyDroneRun-v0",
          "SafetyPointCircle1Gymnasium-v0", "SafetyPointCircle2Gymnasium-v0", "SafetyCarCircle1Gymnasium-v0",
          "SafetyCarCircle2Gymnasium-v0", "SafetyPointGoal2Gymnasium-v0", "SafetyCarGoal1Gymnasium-v0",
-         "SafetyCarGoal2Gymnasium-v0"]
+         "SafetyCarGoal2Gymnasium-v0", "SafetyPointButton1Gymnasium-v0", "SafetyPointButton2Gymnasium-v0",
+         "SafetyCarButton1Gymnasium-v0", "SafetyCarButton2Gymnasium-v0", "SafetyPointPush1Gymnasium-v0",
+         "SafetyPointPush2Gymnasium-v0", "SafetyCarPush1Gymnasium-v0", "SafetyCarPush2Gymnasium-v0"]
 
 
 def _card():
