@@ -3,9 +3,9 @@
 //
 // The reference's physics engines are absent and irreproducible (SURVEY.md F5), so these are
 // OUR documented analytic models with the task structure of Bullet-Safety-Gym's Circle / Run
-// tasks and Safety-Gymnasium's Point / Car Circle, Goal, Button and Push tasks (dense reward, binary cost, fixed
-// horizon; the Drone tasks also terminate on a crash or a flip, every other task is truncation
-// only).  Every arithmetic step
+// tasks and Safety-Gymnasium's Point / Car Circle, Goal, Button and Push tasks and its velocity tasks (dense
+// reward, binary cost, fixed horizon; the Drone tasks also terminate on a crash or a flip, Hopper, Walker2d and
+// Ant on an unhealthy pose, every other task is truncation only).  Every arithmetic step
 // uses only IEEE-exact operations (+ - * / sqrt, no FMA contraction, polynomial sin/cos), so
 // the CPU twin in oracle/envs.py reproduces trajectories BIT-EXACTLY from the same actions.
 //
@@ -18,13 +18,15 @@
 namespace fsrl {
 
 // Kinds 0-8 are the Bullet-Safety-Gym tasks and PointGoal1; the Safety-Gymnasium navigation family
-// starts at 16.  Ids 9-15 and 23 are unassigned.
+// starts at 16, its velocity family at 33.  Ids 9-15, 23 and 32 are unassigned.
 enum EnvKind { ENV_CAR_CIRCLE = 0, ENV_CAR_RUN = 1, ENV_BALL_CIRCLE = 2, ENV_BALL_RUN = 3,
                ENV_ANT_CIRCLE = 4, ENV_POINT_GOAL = 5, ENV_ANT_RUN = 6, ENV_DRONE_CIRCLE = 7,
                ENV_DRONE_RUN = 8, ENV_POINT_CIRCLE1 = 16, ENV_POINT_CIRCLE2 = 17, ENV_CAR_CIRCLE1 = 18,
                ENV_CAR_CIRCLE2 = 19, ENV_POINT_GOAL2 = 20, ENV_CAR_GOAL1 = 21, ENV_CAR_GOAL2 = 22,
                ENV_POINT_BUTTON1 = 24, ENV_POINT_BUTTON2 = 25, ENV_CAR_BUTTON1 = 26, ENV_CAR_BUTTON2 = 27,
-               ENV_POINT_PUSH1 = 28, ENV_POINT_PUSH2 = 29, ENV_CAR_PUSH1 = 30, ENV_CAR_PUSH2 = 31 };
+               ENV_POINT_PUSH1 = 28, ENV_POINT_PUSH2 = 29, ENV_CAR_PUSH1 = 30, ENV_CAR_PUSH2 = 31,
+               ENV_HALF_CHEETAH_VEL = 33, ENV_HOPPER_VEL = 34, ENV_SWIMMER_VEL = 35, ENV_WALKER2D_VEL = 36,
+               ENV_ANT_VEL = 37 };
 
 constexpr int ENV_MAX_A = 8;
 constexpr int ENV_MAX_S = 32;
@@ -132,6 +134,10 @@ __host__ __device__ inline EnvDims env_dims(int kind) {
             return {76, 2, 12, 1000};
         case ENV_POINT_PUSH1: case ENV_CAR_PUSH1: return {76, 2, 18, 1000};
         case ENV_POINT_PUSH2: case ENV_CAR_PUSH2: return {76, 2, 28, 1000};
+        case ENV_HALF_CHEETAH_VEL: case ENV_WALKER2D_VEL: return {17, 6, 17, 1000};
+        case ENV_HOPPER_VEL: return {11, 3, 11, 1000};
+        case ENV_SWIMMER_VEL: return {8, 2, 9, 1000};
+        case ENV_ANT_VEL: return {27, 8, 26, 1000};
         default: return {0, 0, 0, 0};
     }
 }
@@ -1013,6 +1019,247 @@ struct NavPush {
         term = false;
     }
 };
+
+// ---------------------------------------------------------------------------------------------
+// Safety-Gymnasium velocity tasks (T = 1000): HalfCheetah, Hopper, Swimmer, Walker2d and Ant, with the observation
+// widths of gymnasium's MuJoCo v4 robots minus the x (x, y) position.  Our models, not MuJoCo:
+//   Joints   N damped, driven joints: qd += (KA*a - KQ*q - KD*qd) * DT ; q += qd * DT  (vel_joints).
+//   Gait     forward force F = clamp(GK * sum over the robot's joint pairs (i, k) of q_i*qd_k - q_k*qd_i, -1, 1):
+//            the signed area the pairs sweep.  A constant action (qd -> 0) or in-phase motion sweeps none; two
+//            joints driven by sinusoids a quarter period apart sweep a constant area.  The forward speed moves the
+//            fraction RDT of the way to VMAX * F per step (linear drag).
+//   Pitch    (HalfCheetah, Hopper, Walker2d) wd += (PU*th - PT*tq - PD*wd) * DT ; th += wd * DT, with tq the
+//            thigh angle (Hopper q0, Walker2d (q0 + q3) / 2, HalfCheetah q0 - q3).  PU > 0 (Hopper, Walker2d)
+//            is an inverted pendulum that only thigh feedback holds up; HalfCheetah's PU < 0 is a restoring
+//            spring, and the model has no flips.  |th| is clamped to FALL (lying on the ground).
+//   Height   z follows zt through a spring-damper (ZK, ZD): planar zt = (Z0 - ZQ * sum knee^2) * cos th, Ant
+//            zt = Z0 + ANT_ZA * (sum of the 4 ankles).
+//   Swimmer  the plane with a heading: the yaw rate follows SW_KW * (q0 + q1) (the body's bend).
+//   Ant      Ant-Circle's joint layout; the gait pairs are (hip j, ankle j + 4), the speed runs along the heading,
+//            the yaw rate follows ANT_KW * (area of legs 0-1 - area of legs 2-3), small roll / pitch angles with
+//            spring-dampers are driven by the hips, and the quaternion observation is built from half-angles.
+//   Reward   vx + HEALTHY - WCTRL * |a|^2 (a: the action the env receives).  Cost 1 when the speed (vx; the
+//            planar speed for Ant) exceeds VCOST.  Terminated, checked after the step: Hopper z <= 0.7 or
+//            |th| >= 0.2; Walker2d z <= 0.8, z >= 2 or |th| >= 1; Ant z < 0.2 or z > 1.
+//   Reset    from the reset's Philox stream: draw 0 the body, draws 1-2 the joint angles (4 per draw, +-0.05).
+// observation  HalfCheetah / Hopper / Walker2d: z, th, q[N], vx, vz, wd, qd[N]
+//              Swimmer: th, q0, q1, vx, vy, wd, qd0, qd1
+//              Ant: z, quaternion (w, x, y, z), q[8], vx, vy, vz, roll rate, pitch rate, yaw rate, qd[8]
+// state        planar: z, vz, th, wd, vx, q[N], qd[N];  Swimmer: th, c, s, u, wd, q[2], qd[2]
+//              Ant: z, vz, c, s, u, w, roll, roll rate, pitch, pitch rate, q[8], qd[8]
+// ---------------------------------------------------------------------------------------------
+namespace vel {
+constexpr float DT = 0.05f, KA = 20.0f, KQ = 10.0f, KD = 4.0f;   // joints
+constexpr float RDT = 0.1f;                                       // forward-speed relaxation per step
+constexpr float ZK = 40.0f, ZD = 10.0f, ZQ = 0.05f, FALL = 1.5f;  // height spring-damper, knee crouch, pitch clamp
+constexpr float SW_KW = 0.5f, SW_YD = 2.0f;                       // Swimmer yaw
+constexpr float ANT_KW = 0.02f, ANT_YD = 2.0f;                    // Ant yaw
+constexpr float ANT_AT = 0.5f, ANT_AS = 20.0f, ANT_AD = 6.0f;     // Ant roll / pitch: hip drive, spring, damping
+constexpr float ANT_ZA = 0.1f;                                    // Ant height per unit of ankle angle
+}
+
+// per robot: N joints, state offset of q, the saturated speed, gait gain, cost threshold, control weight, healthy
+// reward, standing height and pitch constants
+template <int KIND> struct VelCfg;
+template <> struct VelCfg<ENV_HALF_CHEETAH_VEL> {
+    static constexpr int N = 6, Q0 = 5, D = 17, S = 17;
+    static constexpr float VMAX = 4.0f, GK = 0.05f, VCOST = 2.8f, WCTRL = 0.1f, HEALTHY = 0.0f, Z0 = 0.6f;
+    static constexpr float PU = -20.0f, PT = 0.5f, PD = 2.0f;
+};
+template <> struct VelCfg<ENV_HOPPER_VEL> {
+    static constexpr int N = 3, Q0 = 5, D = 11, S = 11;
+    static constexpr float VMAX = 0.5f, GK = 0.2f, VCOST = 0.35f, WCTRL = 1e-3f, HEALTHY = 1.0f, Z0 = 1.25f;
+    static constexpr float PU = 2.0f, PT = 2.0f, PD = 1.0f;
+};
+template <> struct VelCfg<ENV_SWIMMER_VEL> {
+    static constexpr int N = 2, Q0 = 5, D = 8, S = 9;
+    static constexpr float VMAX = 0.07f, GK = 0.2f, VCOST = 0.05f, WCTRL = 1e-4f, HEALTHY = 0.0f;
+};
+template <> struct VelCfg<ENV_WALKER2D_VEL> {
+    static constexpr int N = 6, Q0 = 5, D = 17, S = 17;
+    static constexpr float VMAX = 2.5f, GK = 0.1f, VCOST = 1.7f, WCTRL = 1e-3f, HEALTHY = 1.0f, Z0 = 1.25f;
+    static constexpr float PU = 2.0f, PT = 2.0f, PD = 1.0f;
+};
+template <> struct VelCfg<ENV_ANT_VEL> {
+    static constexpr int N = 8, Q0 = 10, D = 27, S = 26;
+    static constexpr float VMAX = 3.5f, GK = 0.05f, VCOST = 2.5f, WCTRL = 0.5f, HEALTHY = 1.0f, Z0 = 0.6f;
+};
+
+// the N joints q = st[0..N), qd = st[N..2N), integrated in place; returns sum a_j^2
+template <int N>
+__device__ __forceinline__ float vel_joints(float* st, const float* a) {
+    using namespace vel;
+    float ctrl = 0.0f;
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+        const float q = st[j];
+        const float qd = xa(st[N + j], xm(xs(xs(xm(KA, a[j]), xm(KQ, q)), xm(KD, st[N + j])), DT));
+        st[j] = xa(q, xm(qd, DT));
+        st[N + j] = qd;
+        ctrl = xa(ctrl, xm(a[j], a[j]));
+    }
+    return ctrl;
+}
+
+// the area joints i and k sweep per unit time: q_i * qd_k - q_k * qd_i (q = st[0..N), qd = st[N..2N))
+template <int N>
+__device__ __forceinline__ float vel_area(const float* st, int i, int k) {
+    return xs(xm(st[i], st[N + k]), xm(st[k], st[N + i]));
+}
+
+template <int KIND>
+struct Velocity {
+    using C = VelCfg<KIND>;
+    static constexpr int N = C::N, Q0 = C::Q0, D = C::D, A = N, S = C::S, T = 1000;
+    static constexpr bool PLANAR = KIND != ENV_SWIMMER_VEL && KIND != ENV_ANT_VEL;
+    static_assert(S <= ENV_MAX_S && A <= ENV_MAX_A, "env too large");
+
+    // the saturated gait force of the joints q = st[0..N), qd = st[N..2N)
+    __device__ static float gait(const float* j) {
+        float g = 0.0f;
+        if constexpr (KIND == ENV_HOPPER_VEL) {
+            g = xa(g, vel_area<N>(j, 0, 1)); g = xa(g, vel_area<N>(j, 1, 2));
+        } else if constexpr (KIND == ENV_SWIMMER_VEL) {
+            g = xa(g, vel_area<N>(j, 0, 1));
+        } else if constexpr (KIND == ENV_ANT_VEL) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) g = xa(g, vel_area<N>(j, k, k + 4));
+        } else {
+            g = xa(g, vel_area<N>(j, 0, 1)); g = xa(g, vel_area<N>(j, 1, 2));
+            g = xa(g, vel_area<N>(j, 3, 4)); g = xa(g, vel_area<N>(j, 4, 5));
+        }
+        return fminf(1.0f, fmaxf(-1.0f, xm(g, C::GK)));
+    }
+    __device__ static void reset(float* st, uint32_t seed, uint32_t env, uint32_t ep) {
+        uint32_t r[4];
+        Philox::gen(env, ep, 0u, 0u, seed, KEY_RESET, r);
+#pragma unroll
+        for (int i = 0; i < S; ++i) st[i] = 0.0f;
+        if constexpr (PLANAR) {
+            st[0] = xa(C::Z0, xm(usym(r[0]), 0.005f));
+            st[2] = xm(usym(r[1]), 0.02f);
+            st[3] = xm(usym(r[2]), 0.02f);
+        } else if constexpr (KIND == ENV_SWIMMER_VEL) {
+            st[0] = xm(usym(r[0]), 0.05f);
+            poly_sincos(st[0], st[2], st[1]);
+        } else {
+            st[0] = xa(C::Z0, xm(usym(r[0]), 0.005f));
+            float sn, cs;
+            poly_sincos(xm(usym(r[1]), 0.05f), sn, cs);
+            const float n = xq(xa(xm(cs, cs), xm(sn, sn)));
+            st[2] = xd(cs, n); st[3] = xd(sn, n);
+            st[6] = xm(usym(r[2]), 0.02f);
+            st[8] = xm(usym(r[3]), 0.02f);
+        }
+#pragma unroll
+        for (int h = 0; h < (N + 3) / 4; ++h) {
+            uint32_t q[4];
+            Philox::gen(env, ep, 1u + h, 0u, seed, KEY_RESET, q);
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (4 * h + j < N) st[Q0 + 4 * h + j] = xm(usym(q[j]), 0.05f);
+        }
+    }
+    __device__ static void observe(const float* st, float* o, uint32_t, uint32_t, uint32_t) {
+        if constexpr (PLANAR) {
+            o[0] = st[0]; o[1] = st[2];
+#pragma unroll
+            for (int j = 0; j < N; ++j) { o[2 + j] = st[Q0 + j]; o[5 + N + j] = st[Q0 + N + j]; }
+            o[2 + N] = st[4]; o[3 + N] = st[1]; o[4 + N] = st[3];
+        } else if constexpr (KIND == ENV_SWIMMER_VEL) {
+            o[0] = st[0]; o[1] = st[5]; o[2] = st[6];
+            o[3] = xm(st[3], st[1]); o[4] = xm(st[3], st[2]); o[5] = st[4];
+            o[6] = st[7]; o[7] = st[8];
+        } else {
+            const float c = st[2], s = st[3];
+            const float ch = xq(fmaxf(0.0f, xm(xa(1.0f, c), 0.5f)));
+            float sh = xq(fmaxf(0.0f, xm(xs(1.0f, c), 0.5f)));
+            if (s < 0.0f) sh = -sh;
+            float sr, cr, sp, cp;
+            poly_sincos(xm(st[6], 0.5f), sr, cr);
+            poly_sincos(xm(st[8], 0.5f), sp, cp);
+            o[0] = st[0];
+            o[1] = xa(xm(xm(ch, cp), cr), xm(xm(sh, sp), sr));
+            o[2] = xs(xm(xm(ch, cp), sr), xm(xm(sh, sp), cr));
+            o[3] = xa(xm(xm(ch, sp), cr), xm(xm(sh, cp), sr));
+            o[4] = xs(xm(xm(sh, cp), cr), xm(xm(ch, sp), sr));
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { o[5 + j] = st[Q0 + j]; o[19 + j] = st[Q0 + 8 + j]; }
+            o[13] = xm(st[4], c); o[14] = xm(st[4], s); o[15] = st[1];
+            o[16] = st[7]; o[17] = st[9]; o[18] = st[5];
+        }
+    }
+    __device__ static void step(float* st, const float* a, uint32_t, uint32_t, uint32_t,
+                                float& rew, float& cost, bool& term) {
+        using namespace vel;
+        float* j = st + Q0;
+        const float ctrl = vel_joints<N>(j, a);
+        const float F = gait(j);
+        float vx, speed;
+        term = false;
+        if constexpr (PLANAR) {
+            st[4] = xa(st[4], xm(xs(xm(C::VMAX, F), st[4]), RDT));
+            float tq, kn;
+            if constexpr (KIND == ENV_HOPPER_VEL) {
+                tq = j[0]; kn = xm(j[1], j[1]);
+            } else if constexpr (KIND == ENV_WALKER2D_VEL) {
+                tq = xm(xa(j[0], j[3]), 0.5f); kn = xa(xm(j[1], j[1]), xm(j[4], j[4]));
+            } else {
+                tq = xs(j[0], j[3]); kn = xa(xm(j[1], j[1]), xm(j[4], j[4]));
+            }
+            float th = st[2], wd = st[3];
+            wd = xa(wd, xm(xs(xs(xm(C::PU, th), xm(C::PT, tq)), xm(C::PD, wd)), DT));
+            th = xa(th, xm(wd, DT));
+            if (fabsf(th) > FALL) { th = th > 0.0f ? FALL : -FALL; wd = 0.0f; }
+            st[2] = th; st[3] = wd;
+            float sth, cth;
+            poly_sincos(th, sth, cth);
+            const float zt = xm(xs(C::Z0, xm(ZQ, kn)), cth);
+            st[1] = xa(st[1], xm(xs(xm(ZK, xs(zt, st[0])), xm(ZD, st[1])), DT));
+            st[0] = xa(st[0], xm(st[1], DT));
+            vx = st[4];
+            speed = vx;
+            const float z = st[0];
+            if constexpr (KIND == ENV_HOPPER_VEL) term = z <= 0.7f || fabsf(th) >= 0.2f;
+            if constexpr (KIND == ENV_WALKER2D_VEL) term = z <= 0.8f || z >= 2.0f || fabsf(th) >= 1.0f;
+        } else if constexpr (KIND == ENV_SWIMMER_VEL) {
+            st[3] = xa(st[3], xm(xs(xm(C::VMAX, F), st[3]), RDT));
+            st[4] = xa(st[4], xm(xs(xm(SW_KW, xa(j[0], j[1])), xm(SW_YD, st[4])), DT));
+            const float d = xm(st[4], DT);
+            st[0] = xa(st[0], d);
+            rotate_heading(st[1], st[2], d);
+            vx = xm(st[3], st[1]);
+            speed = vx;
+        } else {
+            st[4] = xa(st[4], xm(xs(xm(C::VMAX, F), st[4]), RDT));
+            const float lft = xa(vel_area<N>(j, 0, 4), vel_area<N>(j, 1, 5));
+            const float rgt = xa(vel_area<N>(j, 2, 6), vel_area<N>(j, 3, 7));
+            st[5] = xa(st[5], xm(xs(xm(ANT_KW, xs(lft, rgt)), xm(ANT_YD, st[5])), DT));
+            rotate_heading(st[2], st[3], xm(st[5], DT));
+            st[7] = xa(st[7], xm(xs(xs(xm(ANT_AT, xs(xa(j[0], j[1]), xa(j[2], j[3]))), xm(ANT_AS, st[6])),
+                                    xm(ANT_AD, st[7])), DT));
+            st[6] = xa(st[6], xm(st[7], DT));
+            st[9] = xa(st[9], xm(xs(xs(xm(ANT_AT, xs(xa(j[0], j[3]), xa(j[1], j[2]))), xm(ANT_AS, st[8])),
+                                    xm(ANT_AD, st[9])), DT));
+            st[8] = xa(st[8], xm(st[9], DT));
+            const float zt = xa(C::Z0, xm(ANT_ZA, xa(xa(j[4], j[5]), xa(j[6], j[7]))));
+            st[1] = xa(st[1], xm(xs(xm(ZK, xs(zt, st[0])), xm(ZD, st[1])), DT));
+            st[0] = xa(st[0], xm(st[1], DT));
+            vx = xm(st[4], st[2]);
+            const float vy = xm(st[4], st[3]);
+            speed = xq(xa(xm(vx, vx), xm(vy, vy)));
+            term = st[0] < 0.2f || st[0] > 1.0f;
+        }
+        rew = xs(xa(vx, C::HEALTHY), xm(C::WCTRL, ctrl));
+        cost = speed > C::VCOST ? 1.0f : 0.0f;
+    }
+};
+
+template <> struct Env<ENV_HALF_CHEETAH_VEL> : Velocity<ENV_HALF_CHEETAH_VEL> {};
+template <> struct Env<ENV_HOPPER_VEL> : Velocity<ENV_HOPPER_VEL> {};
+template <> struct Env<ENV_SWIMMER_VEL> : Velocity<ENV_SWIMMER_VEL> {};
+template <> struct Env<ENV_WALKER2D_VEL> : Velocity<ENV_WALKER2D_VEL> {};
+template <> struct Env<ENV_ANT_VEL> : Velocity<ENV_ANT_VEL> {};
 
 template <> struct Env<ENV_POINT_GOAL> : NavGoal<false, 1> {};
 template <> struct Env<ENV_POINT_CIRCLE1> : NavCircle<false, 1> {};

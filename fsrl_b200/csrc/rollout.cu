@@ -86,6 +86,11 @@ static int check_ids(const char* fn, const fsrl_rollout_t* a, const int32_t* ids
         case ENV_POINT_PUSH2: { constexpr int K = ENV_POINT_PUSH2; CALL; } break;    \
         case ENV_CAR_PUSH1: { constexpr int K = ENV_CAR_PUSH1; CALL; } break;        \
         case ENV_CAR_PUSH2: { constexpr int K = ENV_CAR_PUSH2; CALL; } break;        \
+        case ENV_HALF_CHEETAH_VEL: { constexpr int K = ENV_HALF_CHEETAH_VEL; CALL; } break; \
+        case ENV_HOPPER_VEL: { constexpr int K = ENV_HOPPER_VEL; CALL; } break;      \
+        case ENV_SWIMMER_VEL: { constexpr int K = ENV_SWIMMER_VEL; CALL; } break;    \
+        case ENV_WALKER2D_VEL: { constexpr int K = ENV_WALKER2D_VEL; CALL; } break;  \
+        case ENV_ANT_VEL: { constexpr int K = ENV_ANT_VEL; CALL; } break;            \
         default: set_error("unknown env kind %d", kind); return FSRL_EINVAL;         \
     }
 

@@ -505,7 +505,8 @@ int launch_env_reset_ids(const fsrl_rollout_t& a, const int32_t* ids, int n, flo
 
 // Every entry point reaches a kind through these five launchers.  ROLLOUT_LAUNCHERS(extern, K) declares the
 // instantiations of kind K that another translation unit defines, ROLLOUT_LAUNCHERS(, K) defines them: the
-// Button and Push kinds are compiled in rollout_bp.cu, in parallel with the rest of rollout.cu.
+// Button and Push kinds are compiled in rollout_bp.cu and the velocity kinds in rollout_vel.cu, in parallel with the
+// rest of rollout.cu.
 #define ROLLOUT_LAUNCHERS(EXT, K)                                                                          \
     EXT template int launch_env_reset_all<K>(const fsrl_rollout_t&, cudaStream_t);                         \
     EXT template int launch_steps_h<K>(const fsrl_rollout_t&, int, bool, cudaStream_t);                    \
@@ -518,6 +519,11 @@ int launch_env_reset_ids(const fsrl_rollout_t& a, const int32_t* ids, int n, flo
     X(EXT, ENV_POINT_BUTTON1) X(EXT, ENV_POINT_BUTTON2) X(EXT, ENV_CAR_BUTTON1) X(EXT, ENV_CAR_BUTTON2) \
     X(EXT, ENV_POINT_PUSH1) X(EXT, ENV_POINT_PUSH2) X(EXT, ENV_CAR_PUSH1) X(EXT, ENV_CAR_PUSH2)
 
+#define ROLLOUT_VEL_KINDS(X, EXT)                                                                        \
+    X(EXT, ENV_HALF_CHEETAH_VEL) X(EXT, ENV_HOPPER_VEL) X(EXT, ENV_SWIMMER_VEL) X(EXT, ENV_WALKER2D_VEL) \
+    X(EXT, ENV_ANT_VEL)
+
 ROLLOUT_BP_KINDS(ROLLOUT_LAUNCHERS, extern)
+ROLLOUT_VEL_KINDS(ROLLOUT_LAUNCHERS, extern)
 
 }  // namespace fsrl

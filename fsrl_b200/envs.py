@@ -32,6 +32,9 @@ KINDS = {
     "SafetyCarButton1Gymnasium-v0": 26, "SafetyCarButton2Gymnasium-v0": 27,
     "SafetyPointPush1Gymnasium-v0": 28, "SafetyPointPush2Gymnasium-v0": 29,
     "SafetyCarPush1Gymnasium-v0": 30, "SafetyCarPush2Gymnasium-v0": 31,
+    "SafetyHalfCheetahVelocityGymnasium-v1": 33, "SafetyHopperVelocityGymnasium-v1": 34,
+    "SafetySwimmerVelocityGymnasium-v1": 35, "SafetyWalker2dVelocityGymnasium-v1": 36,
+    "SafetyAntVelocityGymnasium-v1": 37,
 }
 
 

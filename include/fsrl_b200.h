@@ -90,7 +90,10 @@ enum { FSRL_ENV_CAR_CIRCLE = 0, FSRL_ENV_CAR_RUN = 1, FSRL_ENV_BALL_CIRCLE = 2,
        FSRL_ENV_CAR_CIRCLE2 = 19, FSRL_ENV_POINT_GOAL2 = 20, FSRL_ENV_CAR_GOAL1 = 21, FSRL_ENV_CAR_GOAL2 = 22,
        FSRL_ENV_POINT_BUTTON1 = 24, FSRL_ENV_POINT_BUTTON2 = 25, FSRL_ENV_CAR_BUTTON1 = 26,
        FSRL_ENV_CAR_BUTTON2 = 27, FSRL_ENV_POINT_PUSH1 = 28, FSRL_ENV_POINT_PUSH2 = 29, FSRL_ENV_CAR_PUSH1 = 30,
-       FSRL_ENV_CAR_PUSH2 = 31 };
+       FSRL_ENV_CAR_PUSH2 = 31,
+       /* Safety-Gymnasium velocity family; 32 is unassigned */
+       FSRL_ENV_HALF_CHEETAH_VEL = 33, FSRL_ENV_HOPPER_VEL = 34, FSRL_ENV_SWIMMER_VEL = 35,
+       FSRL_ENV_WALKER2D_VEL = 36, FSRL_ENV_ANT_VEL = 37 };
 
 /* per-collect statistics, device resident; the keys of collect()'s result dict
  * (fast_collector.py:399-408) are derived from it on the host */

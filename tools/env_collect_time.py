@@ -24,7 +24,9 @@ TASKS = ["SafetyCarCircle-v0", "SafetyCarRun-v0", "SafetyBallCircle-v0", "Safety
          "SafetyCarCircle2Gymnasium-v0", "SafetyPointGoal2Gymnasium-v0", "SafetyCarGoal1Gymnasium-v0",
          "SafetyCarGoal2Gymnasium-v0", "SafetyPointButton1Gymnasium-v0", "SafetyPointButton2Gymnasium-v0",
          "SafetyCarButton1Gymnasium-v0", "SafetyCarButton2Gymnasium-v0", "SafetyPointPush1Gymnasium-v0",
-         "SafetyPointPush2Gymnasium-v0", "SafetyCarPush1Gymnasium-v0", "SafetyCarPush2Gymnasium-v0"]
+         "SafetyPointPush2Gymnasium-v0", "SafetyCarPush1Gymnasium-v0", "SafetyCarPush2Gymnasium-v0",
+         "SafetyHalfCheetahVelocityGymnasium-v1", "SafetyHopperVelocityGymnasium-v1",
+         "SafetySwimmerVelocityGymnasium-v1", "SafetyWalker2dVelocityGymnasium-v1", "SafetyAntVelocityGymnasium-v1"]
 
 
 def _card():
