@@ -79,6 +79,10 @@ def gae_dual(v: torch.Tensor, vnext: torch.Tensor, rew: torch.Tensor,
     else:
         adv, ret = out
         _req(adv, torch.float32, "adv"); _req(ret, torch.float32, "ret")
+        # the kernel writes C rows of N elements at stride N: a smaller buffer would be written past its end
+        for nm, t in (("adv", adv), ("ret", ret)):
+            if t.shape != v.shape:
+                raise ValueError(f"out {nm} has shape {tuple(t.shape)}, expected {tuple(v.shape)}")
     need = lib.fsrl_gae_dual_workspace_bytes(N)
     ws = workspace(need, v.device, "gae")
     with torch.cuda.device(v.device):
