@@ -172,6 +172,11 @@ class TrajArena(ctypes.Structure):
                 ("D", c_int), ("A", c_int)]
 
 
+class HostStep(ctypes.Structure):
+    _fields_ = [("D", c_int), ("A", c_int), ("n_store", c_int), ("n_act", c_int), ("parity", c_int), ("pad", c_int),
+                ("pack_host", c_vp), ("pack_dev", c_vp), ("scratch", c_vp), ("act_dev", c_vp), ("act_host", c_vp)]
+
+
 ALGO_SAC, ALGO_DDPG = 0, 1
 OFF_STATS = 8
 CVPO_STATS = 16
@@ -198,6 +203,8 @@ SIGNATURES = {
     "fsrl_rollout_steps_act": (c_int, [ctypes.POINTER(Rollout), c_f32p, c_vp]),
     "fsrl_env_step": (c_int, [ctypes.POINTER(Rollout), c_f32p, c_vp, c_int, c_f32p, c_f32p, c_f32p, c_u8p, c_u8p, c_vp]),
     "fsrl_env_reset_ids": (c_int, [ctypes.POINTER(Rollout), c_vp, c_int, c_f32p, c_vp]),
+    "fsrl_host_pack_bytes": (c_size, [c_int, c_int, c_int]),
+    "fsrl_host_collect_step": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(HostStep), c_vp]),
     "fsrl_traj_begin": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_vp]),
     "fsrl_traj_scan": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_int, c_vp]),
     "fsrl_traj_copy": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajArena), c_vp, c_int, c_vp]),
@@ -270,7 +277,7 @@ def _check_abi_sizes():
     lib.fsrl_abi_sizeof.restype = c_size
     lib.fsrl_abi_sizeof.argtypes = [c_int]
     for which, cls in enumerate((Mlp3, CollectStats, Rollout, PpoUpdate, NetRef, NetList, Engine, EngInput,
-                                 OffPolicy, Cpo, Cvpo, TrajRow, TrajScan, TrajArena)):
+                                 OffPolicy, Cpo, Cvpo, TrajRow, TrajScan, TrajArena, HostStep)):
         want = lib.fsrl_abi_sizeof(which)
         if want != ctypes.sizeof(cls):
             raise ImportError(f"ABI mismatch: {cls.__name__} is {ctypes.sizeof(cls)} bytes in python, "

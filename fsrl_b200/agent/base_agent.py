@@ -7,14 +7,19 @@ from abc import ABC, abstractmethod
 from typing import Optional, Tuple
 
 from ..data import FastCollector, VectorReplayBuffer
-from ..envs import DeviceEnv, DeviceVectorEnv
+from ..envs import DeviceEnv, DeviceVectorEnv, HostVectorEnv
+from ..host_envs import is_vector_env
 from ..trainer import OffpolicyTrainer, OnpolicyTrainer
 from ..utils.logger import BaseLogger, DummyLogger
 
 
 def _as_vector(envs, device, seed=0):
+    """A device env as a one-env DeviceVectorEnv; any other vector-protocol object (a tianshou vector env of
+    host envs) as a HostVectorEnv, so that the replay buffer and the collectors see one env object."""
     if isinstance(envs, DeviceEnv):
         return DeviceVectorEnv(envs.task, 1, device=device, seed=seed)
+    if not isinstance(envs, (DeviceVectorEnv, HostVectorEnv)) and is_vector_env(envs):
+        return HostVectorEnv.from_vector_env(envs, device=device, seed=seed)
     return envs
 
 

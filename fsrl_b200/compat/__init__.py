@@ -37,15 +37,22 @@ def _missing(name: str) -> bool:
 
 # ---- vector-env factories with tianshou's constructor (a list of env constructors) ------------------
 def _vector_env_class(cls_name: str):
-    from ..envs import DeviceEnv, DeviceVectorEnv
+    """Registered tasks (DeviceEnv prototypes) become a DeviceVectorEnv; any other env constructor a
+    HostVectorEnv stepping those envs in this process."""
+    from ..envs import DeviceEnv, DeviceVectorEnv, HostVectorEnv
 
     class _Vec(DeviceVectorEnv):
-        def __init__(self, env_fns: List[Callable[[], Any]], **kwargs):
+        def __new__(cls, env_fns: List[Callable[[], Any]], **kwargs):
             proto = env_fns[0]()
-            if not isinstance(proto, DeviceEnv):
-                raise TypeError("the device engine steps its own registered tasks "
-                                f"(got {type(proto).__name__} from the env constructor)")
-            super().__init__(proto.task, len(env_fns), device=kwargs.get("device", "cuda"),
+            if isinstance(proto, DeviceEnv):
+                self = super().__new__(cls)
+                self._proto = proto         # the constructor runs once: __init__ reads the task from it
+                return self
+            return HostVectorEnv._from_envs([proto] + [fn() for fn in env_fns[1:]],
+                                            device=kwargs.get("device", "cuda"), seed=kwargs.get("seed", 0))
+
+        def __init__(self, env_fns: List[Callable[[], Any]], **kwargs):
+            super().__init__(self._proto.task, len(env_fns), device=kwargs.get("device", "cuda"),
                              seed=kwargs.get("seed", 0))
 
     _Vec.__name__ = _Vec.__qualname__ = cls_name

@@ -65,6 +65,7 @@ extern "C" size_t fsrl_abi_sizeof(int which) {
         case 11: return sizeof(fsrl_traj_row_t);
         case 12: return sizeof(fsrl_traj_scan_t);
         case 13: return sizeof(fsrl_traj_arena_t);
+        case 14: return sizeof(fsrl_host_step_t);
         default: return 0;
     }
 }

@@ -12,6 +12,31 @@ namespace fsrl {
 static_assert(sizeof(fsrl_mlp3_t) == sizeof(Mlp3), "ABI struct mismatch");
 static_assert(FSRL_BOUND_CLIP == 1 && FSRL_BOUND_TANH == 2, "map_action() codes");
 
+// buffer.add of one transition of env e (env-major sub-buffer ring; reserved keys of tianshou's buffer);
+// a no-op when the collect stores nothing.  DC is the observation width when it is known at compile time
+// (the device envs), else 0 and d gives it (host-stepped envs).  Every collect path stores through here.
+template <int DC, int A>
+__device__ __forceinline__ void ring_store(const fsrl_rollout_t& a, int e, int d, const float* obs, const float* on,
+                                           const float* act, float logp, float rew, float cost, bool term, bool trunc) {
+    const int D = DC ? DC : d;
+    if (a.b_obs) {
+        const int ptr = a.b_ptr[e];
+        const size_t p = (size_t)e * a.cap + ptr;
+#pragma unroll
+        for (int k = 0; k < D; ++k) {
+            a.b_obs[p * D + k] = obs[k];
+            a.b_obs_next[p * D + k] = on[k];
+        }
+#pragma unroll
+        for (int j = 0; j < A; ++j) a.b_act[p * A + j] = act[j];
+        a.b_rew[p] = rew; a.b_cost[p] = cost; a.b_logp[p] = logp;
+        a.b_term[p] = term ? 1 : 0; a.b_trunc[p] = trunc ? 1 : 0;
+        a.b_ptr[e] = (ptr + 1 == a.cap) ? 0 : ptr + 1;
+        const int len = a.b_len[e];
+        if (len < a.cap) a.b_len[e] = len + 1;
+    }
+}
+
 // Everything of one collect step that follows the policy's action, for env e: map_action, env.step,
 // buffer.add of (obs, act, logp), statistics and the done bookkeeping.  The fused step and the
 // caller-action step both end here, so the two collect paths apply the same episode rules.
@@ -40,23 +65,7 @@ __device__ __forceinline__ void collect_step_tail(const fsrl_rollout_t& a, int e
     float on[D];
     E_::observe(s, on, a.seed_env, (uint32_t)e, ep);
 
-    // ---- buffer.add (env-major sub-buffer ring; reserved keys of tianshou's buffer) -----------
-    if (a.b_obs) {
-        const int ptr = a.b_ptr[e];
-        const size_t p = (size_t)e * a.cap + ptr;
-#pragma unroll
-        for (int k = 0; k < D; ++k) {
-            a.b_obs[p * D + k] = obs[k];
-            a.b_obs_next[p * D + k] = on[k];
-        }
-#pragma unroll
-        for (int j = 0; j < A; ++j) a.b_act[p * A + j] = act[j];
-        a.b_rew[p] = rew; a.b_cost[p] = cost; a.b_logp[p] = logp;
-        a.b_term[p] = term ? 1 : 0; a.b_trunc[p] = trunc ? 1 : 0;
-        a.b_ptr[e] = (ptr + 1 == a.cap) ? 0 : ptr + 1;
-        const int len = a.b_len[e];
-        if (len < a.cap) a.b_len[e] = len + 1;
-    }
+    ring_store<D, A>(a, e, D, obs, on, act, logp, rew, cost, term, trunc);
     // ---- statistics (:326, :338-348) --------------------------------------------------------------
     atomicAdd(&st->step_count, 1ull);
     if (cost != 0.f) atomicAdd(&st->total_cost, (double)cost);
@@ -85,12 +94,12 @@ __device__ __forceinline__ void collect_step_tail(const fsrl_rollout_t& a, int e
     for (int k = 0; k < D; ++k) a.obs_cur[(size_t)e * D + k] = on[k];
 }
 
-// The policy's action for env e from the actor's head output `out` (Philox sampling, the heads, log-prob and
-// DDPG noise), then collect_step_tail.  obs: the observation the actor saw.
-template <int KIND>
-__device__ __forceinline__ void fused_step_env(const fsrl_rollout_t& a, int e, const float* out, const float* obs) {
-    constexpr int A = Env<KIND>::A;
-    float act[A], mu[A], sig[A];
+// The policy's raw action act[A] for env e from the actor's head output `out` (Philox sampling keyed by
+// (e, act_ctr[e]), the heads, log-prob and DDPG noise; random mode draws uniform actions instead); returns
+// its log-prob.  Both fused paths sample through here: the device-env step and the host-env step.
+template <int A>
+__device__ __forceinline__ float policy_sample(const fsrl_rollout_t& a, int e, const float* out, float (&act)[A]) {
+    float mu[A], sig[A];
     float logp = 0.f;
     const uint32_t ctr = a.act_ctr[e];
     float eps[(A + 3) / 4 * 4];
@@ -160,6 +169,15 @@ __device__ __forceinline__ void fused_step_env(const fsrl_rollout_t& a, int e, c
 #pragma unroll
         for (int j = 0; j < A; ++j) act[j] = fmaf(a.expl_sigma, eps[j], act[j]);
     }
+    return logp;
+}
+
+// The policy's action for env e from the actor's head output `out`, then collect_step_tail.  obs: the
+// observation the actor saw.
+template <int KIND>
+__device__ __forceinline__ void fused_step_env(const fsrl_rollout_t& a, int e, const float* out, const float* obs) {
+    float act[Env<KIND>::A];
+    const float logp = policy_sample<Env<KIND>::A>(a, e, out, act);
     collect_step_tail<KIND>(a, e, obs, act, logp);
 }
 

@@ -14,18 +14,28 @@ A policy the rollout kernel cannot run (its own ``forward``, or an actor the par
 rejects) takes the generic path (``collector.fused == False``): per vector step the collector calls
 ``policy(batch)`` and ``exploration_noise`` in torch, then a step kernel with those actions runs the
 same map_action, env step, buffer store and episode bookkeeping as the fused kernel.
+
+A :class:`HostVectorEnv` (or any other object with tianshou's vector-env protocol, wrapped once by
+``HostVectorEnv.from_vector_env``) takes the host path: the reference's loop runs on the host around the
+envs' own ``step`` / ``reset``, and per vector step one launch (csrc/rollout_host.cu) stores the previous
+step's transitions into the same ring and computes this step's actions with the fused path's actor,
+sampling and noise stream.  Finished envs are reset, surplus ones retired without a reset, as on the
+device path; the statistics are summed on the host in float64, in step order.
 """
 from __future__ import annotations
 
 import contextlib
 import ctypes
 import time
+import types
 from typing import Any, Callable, Dict, Optional
 
+import numpy as np
 import torch
 
 from .. import _lib
 from ..envs import DeviceVectorEnv
+from ..host_envs import HostVectorEnv, is_vector_env
 from .batch import Batch
 from .buffer import DeviceVectorReplayBuffer
 from .traj_buf import TrajectoryBuffer, TrajectoryHarvest
@@ -55,11 +65,21 @@ class FastCollector(object):
                  preprocess_fn: Optional[Callable[..., Batch]] = None,
                  exploration_noise: bool = False, traj_buffer: Optional[TrajectoryBuffer] = None) -> None:
         super().__init__()
-        if not isinstance(env, DeviceVectorEnv):
-            raise TypeError("fsrl_b200.FastCollector steps DeviceVectorEnv instances on the GPU; "
-                            f"got {type(env).__name__}")
+        if not isinstance(env, (DeviceVectorEnv, HostVectorEnv)):
+            if not is_vector_env(env):
+                raise TypeError("fsrl_b200.FastCollector steps a DeviceVectorEnv, a HostVectorEnv or an object with "
+                                f"the vector-env protocol (len, step(action, id), reset(id)); got {type(env).__name__}")
+            env = HostVectorEnv.from_vector_env(env, device=getattr(policy, "device", "cuda"))
         if preprocess_fn is not None:
             raise NotImplementedError("preprocess_fn would need a host round trip per step")
+        # host path: the host steps the envs, one launch per vector step acts and stores
+        self.host = isinstance(env, HostVectorEnv)
+        if self.host and traj_buffer is not None:
+            raise NotImplementedError("traj_buffer harvests the ring of device envs only; host envs collect into "
+                                      "a VectorReplayBuffer")
+        if self.host and not _fused_policy(policy):
+            raise NotImplementedError("host envs need a policy whose actor the rollout kernel runs (a built-in "
+                                      "actor the parameter arena holds); this policy would take the generic path")
         self.env = env
         self.env_num = len(env)
         self.exploration_noise = exploration_noise
@@ -101,6 +121,9 @@ class FastCollector(object):
             self.buffer.reset(keep_statistics=keep_statistics)
 
     def reset_env(self, gym_reset_kwargs: Optional[Dict[str, Any]] = None) -> None:
+        if self.host:
+            self._obs = self.env.reset_obs(None, **(gym_reset_kwargs or {}))
+            return
         self.env.reset()
 
     def min_ring_capacity(self, n_episode: Optional[int] = None) -> int:
@@ -158,8 +181,82 @@ class FastCollector(object):
             raise TypeError("Please specify n_episode"
                             "in FastCollector.collect().")
         start_time = time.time()
-        env = self.env
         r = self._descriptor(random)
+        if self.host:
+            st = self._host_steps(r, int(n_episode), render, gym_reset_kwargs)
+        else:
+            st = self._device_steps(r, n_episode, no_grad, random)
+        step_count, episode_count = int(st.step_count), int(st.episode_count)
+        self.collect_step += step_count
+        self.collect_episode += episode_count
+        # a collect always ends with fresh resets of every env (:375-388)
+        self.reset_env()
+        self.collect_time += max(time.time() - start_time, 1e-9)
+
+        if episode_count > 0:
+            rew_mean = st.sum_ep_rew / episode_count
+            len_mean = st.sum_ep_len / episode_count
+        else:
+            rew_mean = len_mean = 0
+        done_count = st.term_count + st.trunc_count
+        return {
+            "n/ep": episode_count,
+            "n/st": step_count,
+            "rew": rew_mean,
+            "len": len_mean,
+            "total_cost": st.total_cost,
+            "cost": st.total_cost / episode_count,
+            "truncated": st.trunc_count / done_count,
+            "terminated": st.term_count / done_count,
+        }
+
+    def _host_steps(self, r, n_episode: int, render: bool, gym_reset_kwargs) -> types.SimpleNamespace:
+        """The reference's collect loop (:252-368) over host envs; the device acts and stores once per step."""
+        env = self.env
+        E = self.env_num
+        kw = gym_reset_kwargs or {}
+        obs = self._obs
+        ready = np.arange(min(E, n_episode))
+        ep_rew, ep_len = np.zeros(E, np.float64), np.zeros(E, np.int64)
+        st = types.SimpleNamespace(step_count=0, episode_count=0, total_cost=0.0, sum_ep_rew=0.0, sum_ep_len=0,
+                                   term_count=0, trunc_count=0)
+        stored = None                         # the previous step's transitions, stored by the next launch
+        while True:
+            act = env.device_step(r, ready, obs[ready], stored)
+            obs_next, rew, term, trunc, cost = env.step_envs(act, ready)
+            if render:
+                env.render()
+            if self.buffer is not None:
+                stored = (ready, obs_next, rew, cost, term, trunc)
+            st.total_cost += float(np.sum(cost, dtype=np.float64))
+            st.step_count += len(ready)
+            ep_rew[ready] += rew.astype(np.float64)
+            ep_len[ready] += 1
+            obs[ready] = obs_next
+            done = term | trunc
+            if done.any():
+                ids = ready[done]
+                st.episode_count += len(ids)
+                st.sum_ep_rew += float(np.sum(ep_rew[ids]))
+                st.sum_ep_len += int(np.sum(ep_len[ids]))
+                st.term_count += int(term.sum())
+                st.trunc_count += int(trunc.sum())
+                ep_rew[ids], ep_len[ids] = 0.0, 0
+                # the surplus rule (:357-363): the lowest finished ids retire, without a reset; the rest restart
+                surplus = min(max(len(ready) - (n_episode - st.episode_count), 0), len(ids))
+                if surplus < len(ids):
+                    restart = ids[surplus:]
+                    obs[restart] = env.reset_obs(restart, **kw)
+                if surplus:
+                    ready = ready[~np.isin(ready, ids[:surplus])]
+            if st.episode_count >= n_episode:
+                break
+        if stored is not None:
+            env.device_step(r, ready[:0], obs[:0], stored)
+        return st
+
+    def _device_steps(self, r, n_episode: int, no_grad: bool, random: bool):
+        env = self.env
         r.inline_done = 1 if n_episode <= self.env_num else 0
         T = env.max_episode_steps
         traj = self.traj_buffer
@@ -195,29 +292,7 @@ class FastCollector(object):
         if not st.finished:
             raise RuntimeError("rollout did not reach n_episode within the step bound "
                                f"(episodes {st.episode_count}/{n_episode})")
-        step_count, episode_count = int(st.step_count), int(st.episode_count)
-        self.collect_step += step_count
-        self.collect_episode += episode_count
-        # a collect always ends with fresh resets of every env (:375-388)
-        self.reset_env()
-        self.collect_time += max(time.time() - start_time, 1e-9)
-
-        if episode_count > 0:
-            rew_mean = st.sum_ep_rew / episode_count
-            len_mean = st.sum_ep_len / episode_count
-        else:
-            rew_mean = len_mean = 0
-        done_count = st.term_count + st.trunc_count
-        return {
-            "n/ep": episode_count,
-            "n/st": step_count,
-            "rew": rew_mean,
-            "len": len_mean,
-            "total_cost": st.total_cost,
-            "cost": st.total_cost / episode_count,
-            "truncated": st.trunc_count / done_count,
-            "terminated": st.term_count / done_count,
-        }
+        return st
 
     def _harvest_into(self, traj: TrajectoryBuffer, r, n_ready: int, window: int, stream: int) -> None:
         rows = self._harvest.scan(r, n_ready, window, stream)

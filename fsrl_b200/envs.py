@@ -6,6 +6,8 @@ The dynamics are the analytic models of csrc/envs.cuh (bullet_safety_gym / safet
 are absent and irreproducible; SURVEY.md F5).  All state lives in HBM as SoA tensors; the
 fused rollout kernel (csrc/rollout.cu) steps every env without host involvement.  ``step`` /
 ``reset(id)`` give the gym protocol on the same state, for loops that bring their own actions.
+Envs the device cannot run (gymnasium simulators, a user's own env) go behind :class:`HostVectorEnv`
+(host_envs.py).
 """
 from __future__ import annotations
 
@@ -16,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .host_envs import HostVectorEnv, _Spec  # noqa: F401
 from .spaces import Box
 
 # task id -> (kind, D, A, S, T).  Registry names follow the reference's examples
@@ -42,11 +45,6 @@ def env_dims(kind: int):
     D, A, S, T = (ctypes.c_int() for _ in range(4))
     _lib.check(_lib.lib.fsrl_env_dims(kind, ctypes.byref(D), ctypes.byref(A), ctypes.byref(S), ctypes.byref(T)))
     return D.value, A.value, S.value, T.value
-
-
-class _Spec:
-    def __init__(self, id, max_episode_steps):
-        self.id, self.max_episode_steps = id, max_episode_steps
 
 
 class DeviceEnv:

@@ -167,6 +167,39 @@ int fsrl_env_step(const fsrl_rollout_t* r, const float* act, const int32_t* ids,
                   float* rew, float* cost, uint8_t* term, uint8_t* trunc, void* stream);
 int fsrl_env_reset_ids(const fsrl_rollout_t* r, const int32_t* ids, int n, float* obs, void* stream);
 
+/* ---- host-stepped envs: one vector step of FastCollector.collect around a host env.step ----------
+ * The host steps its own envs (gymnasium / tianshou objects); the device keeps the actor, the noise
+ * stream and the ring.  One call per vector step enqueues, on `stream`: one H2D copy of the packed
+ * upload, one launch, one D2H copy of the actions.  The launch
+ *   store phase: buffer.add of the n_store transitions of the previous call (obs, raw act and logp from
+ *                that call's act phase, obs_next / rew / cost / flags from this upload); advances
+ *                b_ptr / b_len.  Skipped when r->b_obs is NULL (n_store must then be 0).
+ *   act phase:   the actor on the n_act uploaded observations, sampling keyed by (env id, act_ctr) as in
+ *                fsrl_rollout_steps (same heads, modes and noise), map_action; act_host[k][A] receives
+ *                the env-range action of row k.
+ * Per-env scratch [2][E][D + A + 1] (obs, raw act, logp) alternates by `parity` (0 / 1, flipped every
+ * call): the act phase writes half `parity`, the store phase reads the other half.  r->kind, the env
+ * state pointers and r->stats are unused; r->E, act_ctr, the actor, head / mode and the ring are read.
+ * pack_host (HOST, pinned) holds, in this order and without padding:
+ *   int32 store_ids[n_store] | int32 act_ids[n_act] | f32 obs[n_act][D] | f32 obs_next[n_store][D] |
+ *   f32 rew[n_store] | f32 cost[n_store] | u8 term[n_store] | u8 trunc[n_store]
+ * (fsrl_host_pack_bytes gives its size); pack_dev receives it.  Ids are in [0, E), each at most once per
+ * list.  Returns FSRL_EINVAL before touching the device when a count, an id or a pointer is invalid,
+ * D != r->actor.in (outside random mode), A is outside 1..8, D + A > FSRL_ENG_DX_LD or the actor's H
+ * is not 64 / 128 / 256 / 512.  The caller synchronises `stream` before reading act_host. */
+typedef struct fsrl_host_step {
+    int D, A;
+    int n_store, n_act;
+    int parity, pad;
+    const void* pack_host;
+    void* pack_dev;
+    float* scratch;        /* device [2][E][D + A + 1] */
+    float* act_dev;        /* device [E][A] */
+    float* act_host;       /* HOST, pinned [E][A] */
+} fsrl_host_step_t;
+size_t fsrl_host_pack_bytes(int D, int n_store, int n_act);
+int fsrl_host_collect_step(const fsrl_rollout_t* r, const fsrl_host_step_t* h, void* stream);
+
 /* ---- offline datasets: finished episodes of the rollout ring -> trajectory arena ----------------
  * Replaces the per-transition Batch.cat / return sums of TrajectoryBuffer.store
  * (fsrl/data/traj_buf.py:60-95), fed by BasicCollector (basic_collector.py:238-248), and the
