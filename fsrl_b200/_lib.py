@@ -177,6 +177,15 @@ class HostStep(ctypes.Structure):
                 ("pack_host", c_vp), ("pack_dev", c_vp), ("scratch", c_vp), ("act_dev", c_vp), ("act_host", c_vp)]
 
 
+class ObsRms(ctypes.Structure):
+    _fields_ = [("mean", c_vp), ("var", c_vp), ("count", c_vp), ("work", c_vp), ("D", c_int), ("update", c_int),
+                ("clip_max", c_f64), ("eps", c_f64)]
+
+
+class HostNorm(ctypes.Structure):
+    _fields_ = [("obs_rms", c_vp), ("obs_norm", c_vp), ("n_fresh", c_int), ("pad", c_int)]
+
+
 ALGO_SAC, ALGO_DDPG = 0, 1
 OFF_STATS = 8
 CVPO_STATS = 16
@@ -205,6 +214,11 @@ SIGNATURES = {
     "fsrl_env_reset_ids": (c_int, [ctypes.POINTER(Rollout), c_vp, c_int, c_f32p, c_vp]),
     "fsrl_host_pack_bytes": (c_size, [c_int, c_int, c_int]),
     "fsrl_host_collect_step": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(HostStep), c_vp]),
+    "fsrl_host_pack_norm_bytes": (c_size, [c_int, c_int, c_int, c_int]),
+    "fsrl_host_collect_step_norm": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(HostStep), ctypes.POINTER(HostNorm), c_vp]),
+    "fsrl_obs_rms_work_bytes": (c_size, [c_int, c_int]),
+    "fsrl_obs_rms_rows": (c_int, [ctypes.POINTER(ObsRms), c_f32p, c_int, c_vp, c_int, c_f32p, c_f32p, c_vp]),
+    "fsrl_rollout_norm_steps": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(ObsRms), c_int, c_f32p, c_vp]),
     "fsrl_traj_begin": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_vp]),
     "fsrl_traj_scan": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_int, c_vp]),
     "fsrl_traj_copy": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajArena), c_vp, c_int, c_vp]),
@@ -277,7 +291,7 @@ def _check_abi_sizes():
     lib.fsrl_abi_sizeof.restype = c_size
     lib.fsrl_abi_sizeof.argtypes = [c_int]
     for which, cls in enumerate((Mlp3, CollectStats, Rollout, PpoUpdate, NetRef, NetList, Engine, EngInput,
-                                 OffPolicy, Cpo, Cvpo, TrajRow, TrajScan, TrajArena, HostStep)):
+                                 OffPolicy, Cpo, Cvpo, TrajRow, TrajScan, TrajArena, HostStep, ObsRms, HostNorm)):
         want = lib.fsrl_abi_sizeof(which)
         if want != ctypes.sizeof(cls):
             raise ImportError(f"ABI mismatch: {cls.__name__} is {ctypes.sizeof(cls)} bytes in python, "

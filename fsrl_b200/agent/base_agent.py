@@ -3,19 +3,24 @@
 buffer, two FastCollectors and a trainer around a policy.  Host control code."""
 from __future__ import annotations
 
+import contextlib
 from abc import ABC, abstractmethod
 from typing import Optional, Tuple
 
 from ..data import FastCollector, VectorReplayBuffer
 from ..envs import DeviceEnv, DeviceVectorEnv, HostVectorEnv
 from ..host_envs import is_vector_env
+from ..obs_norm import VectorEnvNormObs
 from ..trainer import OffpolicyTrainer, OnpolicyTrainer
 from ..utils.logger import BaseLogger, DummyLogger
 
 
 def _as_vector(envs, device, seed=0):
     """A device env as a one-env DeviceVectorEnv; any other vector-protocol object (a tianshou vector env of
-    host envs) as a HostVectorEnv, so that the replay buffer and the collectors see one env object."""
+    host envs) as a HostVectorEnv, so that the replay buffer and the collectors see one env object.  A
+    VectorEnvNormObs passes through."""
+    if isinstance(envs, VectorEnvNormObs):
+        return envs
     if isinstance(envs, DeviceEnv):
         return DeviceVectorEnv(envs.task, 1, device=device, seed=seed)
     if not isinstance(envs, (DeviceVectorEnv, HostVectorEnv)) and is_vector_env(envs):
@@ -43,8 +48,11 @@ class BaseAgent(ABC):
             self.policy.load_state_dict(state_dict)
         self.policy.train() if train_mode else self.policy.eval()
         test_envs = _as_vector(test_envs, self.policy.device)
-        eval_collector = FastCollector(self.policy, test_envs)
-        result = eval_collector.collect(n_episode=eval_episodes, render=render)
+        # a normalizing wrapper only normalizes here: evaluation leaves its statistics as they are
+        frozen = test_envs.frozen() if isinstance(test_envs, VectorEnvNormObs) else contextlib.nullcontext()
+        with frozen:
+            eval_collector = FastCollector(self.policy, test_envs)
+            result = eval_collector.collect(n_episode=eval_episodes, render=render)
         return result["rew"], result["len"], result["cost"]
 
     @property
@@ -57,15 +65,25 @@ class BaseAgent(ABC):
         self.policy.train()
         dev = self.policy.device
         train_envs = _as_vector(train_envs, dev)
+        if test_envs is not None:
+            test_envs = _as_vector(test_envs, dev)
+            if isinstance(train_envs, VectorEnvNormObs) and not isinstance(test_envs, VectorEnvNormObs):
+                # tianshou's MuJoCo recipe: the test envs normalize with the training statistics, frozen
+                test_envs = VectorEnvNormObs(test_envs, update_obs_rms=False)
+                test_envs.set_obs_rms(train_envs.get_obs_rms())
         buffer = VectorReplayBuffer(buffer_size, len(train_envs), device=dev)
         train_collector = FastCollector(self.policy, train_envs, buffer, exploration_noise=True)
-        test_collector = FastCollector(self.policy, _as_vector(test_envs, dev)) if test_envs is not None else None
+        test_collector = FastCollector(self.policy, test_envs) if test_envs is not None else None
 
         def stop_fn(reward, cost):
             return reward > reward_threshold and cost < self.cost_limit
 
         if save_ckpt:
-            self.logger.setup_checkpoint_fn(lambda: {"model": self.state_dict})
+            if isinstance(train_envs, VectorEnvNormObs):
+                rms = train_envs.get_obs_rms()
+                self.logger.setup_checkpoint_fn(lambda: {"model": self.state_dict, "obs_rms": rms.state_dict()})
+            else:
+                self.logger.setup_checkpoint_fn(lambda: {"model": self.state_dict})
         return train_collector, test_collector, stop_fn
 
     def _run(self, trainer, verbose):

@@ -130,7 +130,7 @@ def install(force: bool = False) -> List[str]:
         _mod("pyrallis", wrap=_pyrallis_wrap)
     if want("tianshou"):
         vec = {n: _vector_env_class(n) for n in ("DummyVectorEnv", "ShmemVectorEnv", "SubprocVectorEnv")}
-        t_env = _mod("tianshou.env", BaseVectorEnv=_envs.DeviceVectorEnv, **vec)
+        t_env = _mod("tianshou.env", BaseVectorEnv=_envs.DeviceVectorEnv, VectorEnvNormObs=_envs.VectorEnvNormObs, **vec)
         t_data = _mod("tianshou.data", Batch=_data.Batch, ReplayBuffer=_data.ReplayBuffer,
                       ReplayBufferManager=_data.VectorReplayBuffer, VectorReplayBuffer=_data.VectorReplayBuffer,
                       to_numpy=_data.to_numpy, to_torch_as=_data.to_torch_as)

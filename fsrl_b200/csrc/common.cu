@@ -66,6 +66,8 @@ extern "C" size_t fsrl_abi_sizeof(int which) {
         case 12: return sizeof(fsrl_traj_scan_t);
         case 13: return sizeof(fsrl_traj_arena_t);
         case 14: return sizeof(fsrl_host_step_t);
+        case 15: return sizeof(fsrl_obs_rms_t);
+        case 16: return sizeof(fsrl_host_norm_t);
         default: return 0;
     }
 }

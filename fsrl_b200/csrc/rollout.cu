@@ -144,6 +144,25 @@ extern "C" int fsrl_rollout_steps_act(const fsrl_rollout_t* a, const float* act,
     return rc;
 }
 
+extern "C" int fsrl_rollout_norm_steps(const fsrl_rollout_t* a, const fsrl_obs_rms_t* n, int n_steps, const float* act,
+                                       void* stream) {
+    int rc = act ? check_env_state(a) : check_rollout(a);
+    if (rc) return rc;
+    rc = check_obs_rms("fsrl_rollout_norm_steps", n, a->E, env_dims(a->kind).D);
+    if (rc) return rc;
+    FSRL_REQUIRE(n_steps >= 0, "fsrl_rollout_norm_steps: n_steps < 0");
+    FSRL_REQUIRE(!act || n_steps == 1, "fsrl_rollout_norm_steps: caller actions cover one step (n_steps = %d)", n_steps);
+    if (!act) {
+        FSRL_REQUIRE(a->mode == FSRL_MODE_RANDOM || (a->actor.w1t && a->actor.w2t && a->actor.w3t),
+                     "rollout: null actor weights");
+        FSRL_REQUIRE(a->actor.out <= MLP_MAX_OUT, "rollout: actor out dim %d > %d", a->actor.out, MLP_MAX_OUT);
+    }
+    if (n_steps == 0) return FSRL_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    DISPATCH_KIND(a->kind, rc = launch_norm_steps<K>(*a, *n, n_steps, act, s));
+    return rc;
+}
+
 extern "C" int fsrl_env_step(const fsrl_rollout_t* a, const float* act, const int32_t* ids, int n, float* obs_next,
                              float* rew, float* cost, uint8_t* term, uint8_t* trunc, void* stream) {
     int rc = check_env_state(a);

@@ -4,6 +4,7 @@
 #pragma once
 #include "envs.cuh"
 #include "mlp.cuh"
+#include "obsnorm.cuh"
 #include "fsrl_b200.h"
 #include <cstdlib>
 
@@ -521,7 +522,56 @@ int launch_env_reset_ids(const fsrl_rollout_t& a, const int32_t* ids, int n, flo
     });
 }
 
-// Every entry point reaches a kind through these five launchers.  ROLLOUT_LAUNCHERS(extern, K) declares the
+// n_steps vector steps of a collect over an env wrapped by VectorEnvNormObs (fsrl_rollout_norm_steps): per step
+// the fused step kernel (act == NULL) or the caller-action one, the update + normalize pass over the envs that
+// stepped (the snapshot of active in the workspace mask), the resolve kernel, and the pass over the envs it
+// restarted, which also takes the snapshot for the next step.  The kernels are those of the unwrapped paths.
+template <int KIND>
+int launch_norm_steps(const fsrl_rollout_t& a, const fsrl_obs_rms_t& n, int n_steps, const float* act, cudaStream_t s) {
+    const int H = a.actor.H;
+    if (!act && H != 64 && H != 128 && H != 256 && H != 512) {
+        set_error("rollout: hidden width %d unsupported (64/128/256/512)", H);
+        return FSRL_EINVAL;
+    }
+    int rc = launch_obs_norm_snapshot(a, n, s);
+    if (rc) return rc;
+    const ObsNormPass stepped{&n, a.obs_cur, a.E, OBS_SEL_STEPPED, 1, &a};
+    const ObsNormPass restarted{&n, a.obs_cur, a.E, OBS_SEL_RESTARTED, 0, &a};
+#define GO(HH)                                                                                   \
+    {                                                                                            \
+        using TT = MlpTile<HH>;                                                                  \
+        const size_t smem = TT::smem_bytes(Env<KIND>::D);                                        \
+        static bool attr_done = false;                                                           \
+        if (!attr_done) {                                                                        \
+            FSRL_CUDA(cudaFuncSetAttribute(rollout_step_kernel<KIND, HH>,                        \
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            attr_done = true;                                                                    \
+        }                                                                                        \
+        rollout_step_kernel<KIND, HH><<<(a.E + TT::R - 1) / TT::R, MLP_TPB, smem, s>>>(a, 1);    \
+        FSRL_LAUNCH_CHECK();                                                                     \
+    }
+    for (int i = 0; i < n_steps; ++i) {
+        if (act) {
+            rollout_act_step_kernel<KIND><<<(a.E + 127) / 128, 128, 0, s>>>(a, act);
+            FSRL_LAUNCH_CHECK();
+        } else {
+            switch (H) {
+                case 64: GO(64) break;
+                case 128: GO(128) break;
+                case 256: GO(256) break;
+                default: GO(512) break;
+            }
+        }
+        if ((rc = launch_obs_norm(stepped, s))) return rc;
+        rollout_resolve_kernel<KIND><<<1, 1024, 0, s>>>(a);
+        FSRL_LAUNCH_CHECK();
+        if ((rc = launch_obs_norm(restarted, s))) return rc;
+    }
+#undef GO
+    return FSRL_OK;
+}
+
+// Every entry point reaches a kind through these six launchers.  ROLLOUT_LAUNCHERS(extern, K) declares the
 // instantiations of kind K that another translation unit defines, ROLLOUT_LAUNCHERS(, K) defines them: the
 // Button and Push kinds are compiled in rollout_bp.cu and the velocity kinds in rollout_vel.cu, in parallel with the
 // rest of rollout.cu.
@@ -531,7 +581,8 @@ int launch_env_reset_ids(const fsrl_rollout_t& a, const int32_t* ids, int n, flo
     EXT template int launch_act_step<K>(const fsrl_rollout_t&, const float*, cudaStream_t);                \
     EXT template int launch_env_step<K>(const fsrl_rollout_t&, const float*, const int32_t*, int, float*,  \
                                         float*, float*, uint8_t*, uint8_t*, cudaStream_t);                  \
-    EXT template int launch_env_reset_ids<K>(const fsrl_rollout_t&, const int32_t*, int, float*, cudaStream_t);
+    EXT template int launch_env_reset_ids<K>(const fsrl_rollout_t&, const int32_t*, int, float*, cudaStream_t);  \
+    EXT template int launch_norm_steps<K>(const fsrl_rollout_t&, const fsrl_obs_rms_t&, int, const float*, cudaStream_t);
 
 #define ROLLOUT_BP_KINDS(X, EXT)                                                           \
     X(EXT, ENV_POINT_BUTTON1) X(EXT, ENV_POINT_BUTTON2) X(EXT, ENV_CAR_BUTTON1) X(EXT, ENV_CAR_BUTTON2) \

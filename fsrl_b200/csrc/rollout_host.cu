@@ -10,6 +10,7 @@
 // rows of its tile, so a host env sees the action the device-env kernel would compute for the same
 // observation, key and counter, bit for bit.
 #include "rollout.cuh"
+#include "obsnorm.cuh"
 
 #include <vector>
 
@@ -116,6 +117,12 @@ extern "C" size_t fsrl_host_pack_bytes(int D, int n_store, int n_act) {
            2 * (size_t)n_store;
 }
 
+// the wrapped pack (obs_rms set): the unwrapped layout, then from a 16-byte boundary fresh_ids | fresh_obs
+extern "C" size_t fsrl_host_pack_norm_bytes(int D, int n_store, int n_act, int n_fresh) {
+    const size_t base = (fsrl_host_pack_bytes(D, n_store, n_act) + 15) & ~(size_t)15;
+    return base + sizeof(int32_t) * (size_t)n_fresh + sizeof(float) * (size_t)n_fresh * D;
+}
+
 // ids[0..n) each in [0, E) and listed once
 static int check_host_ids(const char* what, const int32_t* ids, int n, int E, std::vector<unsigned char>& seen) {
     seen.assign(E, 0);
@@ -127,7 +134,9 @@ static int check_host_ids(const char* what, const int32_t* ids, int n, int E, st
     return FSRL_OK;
 }
 
-extern "C" int fsrl_host_collect_step(const fsrl_rollout_t* r, const fsrl_host_step_t* h, void* stream) {
+// both entry points; nrm == NULL: no normalization
+static int host_collect_step(const fsrl_rollout_t* r, const fsrl_host_step_t* h, const fsrl_host_norm_t* nrm,
+                             void* stream) {
     FSRL_REQUIRE(r != nullptr && h != nullptr, "fsrl_host_collect_step: null descriptor");
     const int E = r->E, D = h->D, A = h->A;
     FSRL_REQUIRE(E > 0, "fsrl_host_collect_step: E must be positive");
@@ -153,7 +162,15 @@ extern "C" int fsrl_host_collect_step(const fsrl_rollout_t* r, const fsrl_host_s
                      r->actor.out, need, MLP_MAX_OUT, r->head, A);
         FSRL_REQUIRE(r->head != FSRL_HEAD_GAUSS_INDEP || r->log_sigma, "fsrl_host_collect_step: null log_sigma");
     }
-    if (h->n_store > 0)
+    const bool norm = nrm != nullptr;
+    const int n_fresh = norm ? nrm->n_fresh : 0;
+    if (norm) {
+        int rc = check_obs_rms("fsrl_host_collect_step", nrm->obs_rms, E, D);
+        if (rc) return rc;
+        FSRL_REQUIRE(nrm->obs_norm != nullptr, "fsrl_host_collect_step: null obs_norm");
+        FSRL_REQUIRE(n_fresh >= 0 && n_fresh <= E, "fsrl_host_collect_step: n_fresh = %d outside [0, E = %d]", n_fresh, E);
+    }
+    if (h->n_store > 0 && !norm)
         FSRL_REQUIRE(r->b_obs && r->b_obs_next && r->b_act && r->b_rew && r->b_cost && r->b_logp && r->b_term && r->b_trunc &&
                      r->b_ptr && r->b_len && r->cap > 0,
                      "fsrl_host_collect_step: n_store = %d without a complete ring", h->n_store);
@@ -163,7 +180,13 @@ extern "C" int fsrl_host_collect_step(const fsrl_rollout_t* r, const fsrl_host_s
     if (rc) return rc;
     rc = check_host_ids("act_ids", ids + h->n_store, h->n_act, E, seen);
     if (rc) return rc;
-    if (h->n_store == 0 && h->n_act == 0) return FSRL_OK;
+    const size_t fresh_off = (fsrl_host_pack_bytes(D, h->n_store, h->n_act) + 15) & ~(size_t)15;
+    if (norm) {
+        rc = check_host_ids("fresh_ids", reinterpret_cast<const int32_t*>(static_cast<const char*>(h->pack_host) + fresh_off),
+                            n_fresh, E, seen);
+        if (rc) return rc;
+    }
+    if (h->n_store == 0 && h->n_act == 0 && n_fresh == 0) return FSRL_OK;
 
     // resolve the packed layout on the device copy
     char* p = static_cast<char*>(h->pack_dev);
@@ -181,8 +204,24 @@ extern "C" int fsrl_host_collect_step(const fsrl_rollout_t* r, const fsrl_host_s
     g.D = D; g.n_store = h->n_store; g.n_act = h->n_act; g.parity = h->parity;
 
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    FSRL_CUDA(cudaMemcpyAsync(h->pack_dev, h->pack_host, fsrl_host_pack_bytes(D, h->n_store, h->n_act),
+    FSRL_CUDA(cudaMemcpyAsync(h->pack_dev, h->pack_host,
+                              norm ? fsrl_host_pack_norm_bytes(D, h->n_store, h->n_act, n_fresh)
+                                   : fsrl_host_pack_bytes(D, h->n_store, h->n_act),
                               cudaMemcpyHostToDevice, s));
+    if (norm) {
+        // the order of the device-env collect: the rows of the envs that stepped, then those restarted since;
+        // then every acting env's current normalized row into the pack
+        const int* fresh_ids = reinterpret_cast<const int*>(static_cast<char*>(h->pack_dev) + fresh_off);
+        const float* fresh_obs = reinterpret_cast<const float*>(fresh_ids + n_fresh);
+        float* obs_next = const_cast<float*>(g.obs_next);
+        rc = launch_obs_norm_rows(*nrm->obs_rms, nrm->obs_norm, E, g.store_ids, h->n_store, obs_next, obs_next, s);
+        if (rc) return rc;
+        rc = launch_obs_norm_rows(*nrm->obs_rms, nrm->obs_norm, E, fresh_ids, n_fresh, fresh_obs, nullptr, s);
+        if (rc) return rc;
+        rc = launch_obs_gather(nrm->obs_norm, D, g.act_ids, h->n_act, const_cast<float*>(g.obs), s);
+        if (rc) return rc;
+        if (h->n_store == 0 && h->n_act == 0) return FSRL_OK;
+    }
     switch (H) {
         case 64: rc = dispatch_a<64>(*r, g, A, s); break;
         case 128: rc = dispatch_a<128>(*r, g, A, s); break;
@@ -193,4 +232,14 @@ extern "C" int fsrl_host_collect_step(const fsrl_rollout_t* r, const fsrl_host_s
     if (h->n_act > 0)
         FSRL_CUDA(cudaMemcpyAsync(h->act_host, h->act_dev, sizeof(float) * (size_t)h->n_act * A, cudaMemcpyDeviceToHost, s));
     return FSRL_OK;
+}
+
+extern "C" int fsrl_host_collect_step(const fsrl_rollout_t* r, const fsrl_host_step_t* h, void* stream) {
+    return host_collect_step(r, h, nullptr, stream);
+}
+
+extern "C" int fsrl_host_collect_step_norm(const fsrl_rollout_t* r, const fsrl_host_step_t* h, const fsrl_host_norm_t* n,
+                                           void* stream) {
+    FSRL_REQUIRE(n != nullptr, "fsrl_host_collect_step_norm: null normalization descriptor");
+    return host_collect_step(r, h, n, stream);
 }

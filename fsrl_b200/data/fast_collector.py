@@ -21,6 +21,12 @@ envs' own ``step`` / ``reset``, and per vector step one launch (csrc/rollout_hos
 step's transitions into the same ring and computes this step's actions with the fused path's actor,
 sampling and noise stream.  Finished envs are reset, surplus ones retired without a reset, as on the
 device path; the statistics are summed on the host in float64, in step order.
+
+An env wrapped by :class:`~fsrl_b200.obs_norm.VectorEnvNormObs` collects normalized observations: per vector step
+the statistics take the ``obs_next`` of every env that stepped, then the reset observations of the envs that
+restarted, and the ring and the actor see the normalized rows.  Device envs then take one
+``fsrl_rollout_norm_steps`` per step (six launches) instead of the one-launch collect; host envs normalize inside
+their per-step ``fsrl_host_collect_step_norm``.
 """
 from __future__ import annotations
 
@@ -36,6 +42,7 @@ import torch
 from .. import _lib
 from ..envs import DeviceVectorEnv
 from ..host_envs import HostVectorEnv, is_vector_env
+from ..obs_norm import VectorEnvNormObs
 from .batch import Batch
 from .buffer import DeviceVectorReplayBuffer
 from .traj_buf import TrajectoryBuffer, TrajectoryHarvest
@@ -65,6 +72,16 @@ class FastCollector(object):
                  preprocess_fn: Optional[Callable[..., Batch]] = None,
                  exploration_noise: bool = False, traj_buffer: Optional[TrajectoryBuffer] = None) -> None:
         super().__init__()
+        # the observation-normalizing wrapper: self.env is the env it wraps, self.norm the wrapper
+        self.norm = env if isinstance(env, VectorEnvNormObs) else None
+        if self.norm is not None:
+            if traj_buffer is not None:
+                raise NotImplementedError("traj_buffer with a VectorEnvNormObs env would store a dataset of normalized "
+                                          "observations; harvest from the unwrapped env")
+            if getattr(policy, "_dp", None) is not None:
+                raise NotImplementedError("VectorEnvNormObs under data parallelism: each rank's statistics would "
+                                          "diverge")
+            env = self.norm.venv
         if not isinstance(env, (DeviceVectorEnv, HostVectorEnv)):
             if not is_vector_env(env):
                 raise TypeError("fsrl_b200.FastCollector steps a DeviceVectorEnv, a HostVectorEnv or an object with "
@@ -121,6 +138,13 @@ class FastCollector(object):
             self.buffer.reset(keep_statistics=keep_statistics)
 
     def reset_env(self, gym_reset_kwargs: Optional[Dict[str, Any]] = None) -> None:
+        if self.norm is not None:
+            # one update of all E rows
+            if self.host:
+                self._obs = self.norm.host_reset_all(**(gym_reset_kwargs or {}))
+            else:
+                self.norm.reset()
+            return
         if self.host:
             self._obs = self.env.reset_obs(None, **(gym_reset_kwargs or {}))
             return
@@ -171,7 +195,12 @@ class FastCollector(object):
             act = torch.as_tensor(act, dtype=torch.float32, device=env.device).contiguous()
             if tuple(act.shape) != want:
                 raise ValueError(f"the policy returned actions of shape {tuple(act.shape)}; the collect needs {want}")
-            _lib.check(_lib.lib.fsrl_rollout_steps_act(ctypes.byref(r), act.data_ptr(), stream))
+            if self.norm is not None:
+                desc = self.norm.descriptor()
+                _lib.check(_lib.lib.fsrl_rollout_norm_steps(ctypes.byref(r), ctypes.byref(desc), 1, act.data_ptr(),
+                                                            stream))
+            else:
+                _lib.check(_lib.lib.fsrl_rollout_steps_act(ctypes.byref(r), act.data_ptr(), stream))
 
     def collect(self, n_episode: int = 1, random: bool = False, render: bool = False,
                 no_grad: bool = True, gym_reset_kwargs: Optional[Dict[str, Any]] = None) -> Dict[str, Any]:
@@ -221,12 +250,15 @@ class FastCollector(object):
         st = types.SimpleNamespace(step_count=0, episode_count=0, total_cost=0.0, sum_ep_rew=0.0, sum_ep_len=0,
                                    term_count=0, trunc_count=0)
         stored = None                         # the previous step's transitions, stored by the next launch
+        norm = self.norm
+        fresh = None                          # wrapped: the envs restarted since the last launch, and their obs
         while True:
-            act = env.device_step(r, ready, obs[ready], stored)
+            act = env.device_step(r, ready, obs[ready], stored, norm, fresh)
+            fresh = None
             obs_next, rew, term, trunc, cost = env.step_envs(act, ready)
             if render:
                 env.render()
-            if self.buffer is not None:
+            if self.buffer is not None or norm is not None:
                 stored = (ready, obs_next, rew, cost, term, trunc)
             st.total_cost += float(np.sum(cost, dtype=np.float64))
             st.step_count += len(ready)
@@ -247,12 +279,14 @@ class FastCollector(object):
                 if surplus < len(ids):
                     restart = ids[surplus:]
                     obs[restart] = env.reset_obs(restart, **kw)
+                    if norm is not None:
+                        fresh = (restart, obs[restart])
                 if surplus:
                     ready = ready[~np.isin(ready, ids[:surplus])]
             if st.episode_count >= n_episode:
                 break
         if stored is not None:
-            env.device_step(r, ready[:0], obs[:0], stored)
+            env.device_step(r, ready[:0], obs[:0], stored, norm, fresh)
         return st
 
     def _device_steps(self, r, n_episode: int, no_grad: bool, random: bool):
@@ -265,7 +299,12 @@ class FastCollector(object):
                              f"{self.min_ring_capacity(n_episode)} slots per env; the buffer has {self.buffer.cap}")
         with torch.cuda.device(env.device):
             stream = torch.cuda.current_stream().cuda_stream
-            if self.fused or random:
+            if (self.fused or random) and self.norm is not None:
+                desc = self.norm.descriptor()
+
+                def steps(n):
+                    _lib.check(_lib.lib.fsrl_rollout_norm_steps(ctypes.byref(r), ctypes.byref(desc), n, None, stream))
+            elif self.fused or random:
                 def steps(n):
                     _lib.check(_lib.lib.fsrl_rollout_steps(ctypes.byref(r), n, stream))
             else:

@@ -202,3 +202,6 @@ class DeviceVectorEnv:
 
     def close(self):
         pass
+
+
+from .obs_norm import ObsRunningMeanStd, VectorEnvNormObs  # noqa: E402,F401  (obs_norm imports DeviceVectorEnv)

@@ -261,7 +261,7 @@ class HostVectorEnv:
             if self.device.type != "cuda":
                 raise RuntimeError(f"HostVectorEnv collects on CUDA devices only (device={self.device})")
             E, D, A, dev = self.env_num, self.D, self.A, self.device
-            nbytes = int(_lib.lib.fsrl_host_pack_bytes(D, E, E))
+            nbytes = int(_lib.lib.fsrl_host_pack_norm_bytes(D, E, E, E))   # room for a wrapped env's fresh rows
             pack_host = torch.empty(nbytes, dtype=torch.uint8).pin_memory()
             act_host = torch.empty((E, A), dtype=torch.float32).pin_memory()
             self._dev = dict(
@@ -282,10 +282,14 @@ class HostVectorEnv:
         for j in range(self.A):
             r.act_low[j], r.act_high[j] = float(low[j]), float(high[j])
 
-    def device_step(self, r: "_lib.Rollout", act_ids: np.ndarray, obs: np.ndarray, store=None) -> np.ndarray:
+    def device_step(self, r: "_lib.Rollout", act_ids: np.ndarray, obs: np.ndarray, store=None, norm=None,
+                    fresh=None) -> np.ndarray:
         """One ``fsrl_host_collect_step``: store ``store`` = (ids, obs_next, rew, cost, terminated, truncated) of
         the previous call into r's ring, then act on obs [n, D] of the envs act_ids.  Returns the env-range
-        actions [n, A].  One H2D copy, one launch, one D2H copy and one stream synchronisation."""
+        actions [n, A].  One H2D copy, one launch, one D2H copy and one stream synchronisation.  ``norm``: the
+        VectorEnvNormObs wrapping this env; the statistics then take the stored obs_next rows, then ``fresh`` =
+        (ids, reset obs) of the envs restarted since the previous call, and the actor and the ring see normalized
+        rows (the act rows come from the wrapper's ``obs_norm``)."""
         s = self._device_state()
         D, A = self.D, self.A
         n_a = len(act_ids)
@@ -299,6 +303,13 @@ class HostVectorEnv:
         if n_s:
             parts += [(store[1], np.float32), (store[2], np.float32), (store[3], np.float32),
                       (store[4], np.uint8), (store[5], np.uint8)]
+        n_f = 0
+        if norm is not None:
+            if fresh is not None and len(fresh[0]):
+                n_f = len(fresh[0])
+                parts += [(np.zeros(int(_lib.lib.fsrl_host_pack_norm_bytes(D, n_s, n_a, 0))
+                                    - int(_lib.lib.fsrl_host_pack_bytes(D, n_s, n_a)), np.uint8), np.uint8),
+                          (fresh[0], np.int32), (fresh[1], np.float32)]
         for arr, dt in parts:
             b = np.ascontiguousarray(arr, dtype=dt).reshape(-1).view(np.uint8)
             buf[o:o + b.size] = b
@@ -309,7 +320,13 @@ class HostVectorEnv:
                           act_host=s["act_host"].data_ptr())
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream(self.device)
-            _lib.check(_lib.lib.fsrl_host_collect_step(ctypes.byref(r), ctypes.byref(h), stream.cuda_stream))
+            if norm is not None:
+                desc = norm.descriptor()
+                hn = _lib.HostNorm(obs_rms=ctypes.addressof(desc), obs_norm=norm.obs_norm.data_ptr(), n_fresh=n_f)
+                _lib.check(_lib.lib.fsrl_host_collect_step_norm(ctypes.byref(r), ctypes.byref(h), ctypes.byref(hn),
+                                                                stream.cuda_stream))
+            else:
+                _lib.check(_lib.lib.fsrl_host_collect_step(ctypes.byref(r), ctypes.byref(h), stream.cuda_stream))
             stream.synchronize()
         self._parity ^= 1
         return s["act_np"][:n_a].copy()

@@ -199,6 +199,60 @@ typedef struct fsrl_host_step {
 } fsrl_host_step_t;
 size_t fsrl_host_pack_bytes(int D, int n_store, int n_act);
 int fsrl_host_collect_step(const fsrl_rollout_t* r, const fsrl_host_step_t* h, void* stream);
+/* fsrl_host_collect_step over an env wrapped by VectorEnvNormObs (observation normalization, csrc/obsnorm.cu).
+ * pack_host continues, from byte fsrl_host_pack_norm_bytes(D, n_store, n_act, 0), with
+ *   int32 fresh_ids[n_fresh] | f32 fresh_obs[n_fresh][D]
+ * (the reset observations of the envs restarted since the previous call), and before the launch the device
+ * (1) updates the statistics with the n_store obs_next rows and normalizes them in the pack and in obs_norm,
+ * (2) does the same with the fresh rows, (3) copies obs_norm[act_ids[k]] over the n_act observation rows of the
+ * pack.  The act and store phases then read normalized rows.  n_store may be positive without a ring (the store
+ * phase then stores nothing).  Everything else is fsrl_host_collect_step's. */
+typedef struct fsrl_host_norm {
+    const struct fsrl_obs_rms* obs_rms;
+    float* obs_norm;       /* device [E][D]: every env's current normalized observation */
+    int n_fresh, pad;
+} fsrl_host_norm_t;
+size_t fsrl_host_pack_norm_bytes(int D, int n_store, int n_act, int n_fresh);
+int fsrl_host_collect_step_norm(const fsrl_rollout_t* r, const fsrl_host_step_t* h, const fsrl_host_norm_t* n,
+                                void* stream);
+
+/* ---- observation normalization (tianshou's VectorEnvNormObs) on the device ---------------------------
+ * Running statistics mean[D], var[D] (float64) and count (int64) of every observation the wrapped envs
+ * returned.  An update with a batch of n >= 1 rows takes its mean and population variance per feature and
+ * merges them into the running values by the parallel (Chan) update; an empty batch changes nothing.  A
+ * value is normalized as clip((x - mean) / sqrt(var + eps), -clip_max, clip_max) in float64 (no clip when
+ * clip_max <= 0) and rounded to float32 once.
+ * The batch is split into fixed tiles of FSRL_OBS_RMS_TILE env ids; one launch forms each tile's
+ * (count, mean, M2) over its rows in ascending id order, a second merges the tiles in tile order
+ * (every CTA repeats the merge, CTA 0 publishes) and normalizes the rows.  No floating-point atomics: the
+ * result depends only on which env ids hold which rows, so repeated runs, the device-env path and the
+ * host-env path give the same bits.  `update` = 0 only normalizes.  `work` is per wrapper
+ * (fsrl_obs_rms_work_bytes(E, D) bytes): the statistics may be shared by several wrappers.
+ *   fsrl_obs_rms_rows        the rows of the envs ids[0..count) (HOST ids, each once; NULL: all E, count = E)
+ *                            in x[E][D]: if rows_in (device [count][D]) is given its row k is first copied
+ *                            to x[ids[k]]; update, normalize in x, and copy row ids[k] of x to out[k]
+ *                            (device [count][D], may be NULL)
+ *   fsrl_rollout_norm_steps  n_steps vector steps of a collect over a wrapped device env, r->obs_cur holding
+ *                            normalized observations: per step the fused step kernel (act == NULL) or the
+ *                            caller-action step kernel (act, device [E][A], n_steps = 1), then the update with
+ *                            the obs_next of every env that stepped, normalized in obs_cur and in the ring slot
+ *                            just written, then the resolve kernel, then the update with the observations of
+ *                            the envs it restarted, normalized in obs_cur.  6 launches per step, plus one.
+ * Both return FSRL_EINVAL before touching the device on a bad count, id, width or pointer. */
+#define FSRL_OBS_RMS_TILE 128
+typedef struct fsrl_obs_rms {
+    double* mean;          /* device [D] */
+    double* var;           /* device [D] */
+    long long* count;      /* device [1] */
+    void* work;            /* device, fsrl_obs_rms_work_bytes(E, D) bytes */
+    int D, update;
+    double clip_max, eps;
+} fsrl_obs_rms_t;
+size_t fsrl_obs_rms_work_bytes(int E, int D);
+int fsrl_obs_rms_rows(const fsrl_obs_rms_t* n, float* x, int E, const int32_t* ids, int count, const float* rows_in,
+                      float* out, void* stream);
+int fsrl_rollout_norm_steps(const fsrl_rollout_t* r, const fsrl_obs_rms_t* n, int n_steps, const float* act,
+                            void* stream);
 
 /* ---- offline datasets: finished episodes of the rollout ring -> trajectory arena ----------------
  * Replaces the per-transition Batch.cat / return sums of TrajectoryBuffer.store
