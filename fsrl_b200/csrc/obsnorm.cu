@@ -169,7 +169,8 @@ __global__ void __launch_bounds__(OBS_APPLY_TPB) obs_rms_apply_kernel(const ObsK
         const int e = e0 + r;
         float* xp = p.x + (size_t)e * D + d;
         double y = __ddiv_rn(__dsub_rn((double)*xp, s_mean[d]), s_sd[d]);
-        if (clip > 0.0) y = fmin(fmax(y, -clip), clip);
+        // comparisons rather than fmin/fmax, which return the non-NaN operand: a NaN stays NaN, as in np.clip
+        if (clip > 0.0) y = y < -clip ? -clip : (y > clip ? clip : y);
         const float f = (float)y;
         *xp = f;
         if (p.ring) {

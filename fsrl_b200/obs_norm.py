@@ -21,7 +21,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .envs import DeviceVectorEnv
 from .host_envs import HostVectorEnv, is_vector_env
 
 
@@ -87,6 +86,9 @@ class VectorEnvNormObs:
     """tianshou's ``VectorEnvNormObs(venv, update_obs_rms=True)`` over a device or host vector env."""
 
     def __init__(self, venv, update_obs_rms: bool = True):
+        # imported here: envs re-exports this module's classes, so a module-level import would make
+        # `import fsrl_b200.obs_norm` in a fresh interpreter fail on the cycle
+        from .envs import DeviceVectorEnv
         if isinstance(venv, VectorEnvNormObs):
             raise TypeError("VectorEnvNormObs wraps a DeviceVectorEnv or a HostVectorEnv, not another VectorEnvNormObs")
         if not isinstance(venv, (DeviceVectorEnv, HostVectorEnv)):

@@ -46,7 +46,7 @@ def _assert_stats(rms, orms):
         np.testing.assert_allclose(got, want, rtol=1e-9, atol=1e-12)
 
 
-def _wrapped(task, E, buffer_size, generic=False, update=True):
+def _wrapped(task, E, buffer_size, generic=False, update=True, hidden=(64, 64)):
     from fsrl_b200 import envs
     from fsrl_b200.data import FastCollector, VectorReplayBuffer
     from fsrl_b200.envs import VectorEnvNormObs
@@ -57,7 +57,7 @@ def _wrapped(task, E, buffer_size, generic=False, update=True):
         venv = envs.DeviceVectorEnv(task, E, seed=12)
         buf = VectorReplayBuffer(buffer_size, E)
     else:
-        policy, venv, buf, _ = build_ppo(task, n_env=E, buffer_size=buffer_size)
+        policy, venv, buf, _ = build_ppo(task, hidden=hidden, n_env=E, buffer_size=buffer_size)
     norm = VectorEnvNormObs(venv, update_obs_rms=update)
     col = FastCollector(policy, norm, buf, exploration_noise=True)
     onorm = OracleNormObs(_twin(venv), update=update)
@@ -69,21 +69,28 @@ def _wrapped(task, E, buffer_size, generic=False, update=True):
 
 def _assert_successors(b, cap, E):
     """obs[t + 1] == obs_next[t] bit for bit wherever env e continued (ring not wrapped)."""
-    for e in range(E):
-        L = int(b["len"][e])
-        for t in range(L - 1):
-            p = e * cap + t
-            if not (b["terminated"][p] or b["truncated"][p]):
-                assert np.array_equal(b["obs"][p + 1].view(np.int32), b["obs_next"][p].view(np.int32)), (e, t)
+    D = b["obs"].shape[1]
+    obs, nxt = (b[k].reshape(E, cap, D).view(np.int32) for k in ("obs", "obs_next"))
+    ended = (b["terminated"] | b["truncated"]).reshape(E, cap)
+    cont = (np.arange(cap - 1)[None, :] < b["len"].astype(np.int64)[:, None] - 1) & ~ended[:, :-1]
+    bad = np.argwhere(cont & (obs[:, 1:] != nxt[:, :-1]).any(axis=2))
+    assert len(bad) == 0, bad[:4].tolist()
 
 
 @pytest.mark.parametrize("task", TASKS)
 @pytest.mark.parametrize("E,n_episode", [(16, 16), (6, 14)])
 def test_random_collect_matches_oracle(task, E, n_episode):
+    _check_random_collect(task, E, n_episode)
+
+
+def _check_random_collect(task, E, n_episode, hidden=(64, 64), twin=None, T=1000):
+    """A random-mode collect of the wrapped device env against the twin wrapper (ring of T slots per env and
+    round); ``twin`` may replace the twin's inner env (a recording proxy).  Returns the twin wrapper."""
     from oracle import collector as ocol
-    T = 1000
     rounds = n_episode // E + 2
-    policy, venv, norm, buf, col, onorm = _wrapped(task, E, E * T * rounds)
+    policy, venv, norm, buf, col, onorm = _wrapped(task, E, E * T * rounds, hidden=hidden)
+    if twin is not None:
+        onorm.inner = twin(onorm.inner)
     _assert_stats(norm.get_obs_rms(), onorm.rms)
     stats = col.collect(n_episode=n_episode, random=True)
     obuf = ocol.OracleBuffer(E * T * rounds, E, venv.D, venv.A)
@@ -105,6 +112,7 @@ def test_random_collect_matches_oracle(task, E, n_episode):
     _assert_successors(b, buf.cap, E)
     if task == HOPPER:
         assert b["terminated"].any()
+    return onorm
 
 
 def _replay_inline(policy, norm_env, b, cap, E, onorm):
@@ -139,11 +147,11 @@ def test_train_collect_replays_through_twin(task, generic):
     _assert_successors(b, buf.cap, E)
 
 
-def _host_vs_device(task, E, n_episode, mode):
+def _host_vs_device(task, E, n_episode, mode, hidden=(64, 64)):
     from fsrl_b200.data import FastCollector, VectorReplayBuffer
     from fsrl_b200.envs import DeviceVectorEnv, VectorEnvNormObs
     from host_twin import host_twin
-    policy, _, _, _ = build_ppo(task, n_env=E)
+    policy, _, _, _ = build_ppo(task, hidden=hidden, n_env=E)
     getattr(policy, mode)()
     out = []
     for venv in (DeviceVectorEnv(task, E, seed=7), host_twin(task, E, 7)):
@@ -160,7 +168,12 @@ def _host_vs_device(task, E, n_episode, mode):
 @pytest.mark.parametrize("task", [HOPPER, BUTTON])
 @pytest.mark.parametrize("E,n_episode", [(8, 8), (5, 13)])
 def test_host_path_matches_device_path_bitwise(task, E, n_episode):
-    (bd, md, vd, cd, ad, sd, sd2, cap), (bh, mh, vh, ch, ah, sh, sh2, _) = _host_vs_device(task, E, n_episode, "train")
+    _check_host_vs_device(task, E, n_episode)
+
+
+def _check_host_vs_device(task, E, n_episode, hidden=(64, 64)):
+    (bd, md, vd, cd, ad, sd, sd2, cap), (bh, mh, vh, ch, ah, sh, sh2, _) = _host_vs_device(task, E, n_episode, "train",
+                                                                                          hidden)
     for k in bd:
         assert np.array_equal(bd[k], bh[k]), k
     assert md.tobytes() == mh.tobytes() and vd.tobytes() == vh.tobytes() and cd == ch

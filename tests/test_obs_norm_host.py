@@ -116,6 +116,20 @@ def test_wrapper_adopts_vector_protocol_objects_and_compat_exports_it():
     assert tianshou.env.VectorEnvNormObs is VectorEnvNormObs
 
 
+@pytest.mark.parametrize("first", ["fsrl_b200.obs_norm", "fsrl_b200.envs"])
+def test_obs_norm_imports_in_either_order(first):
+    """envs re-exports obs_norm's classes and obs_norm wraps envs' DeviceVectorEnv: a fresh interpreter can import
+    either module first."""
+    import os
+    import subprocess
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    code = (f"import {first}\nfrom fsrl_b200.obs_norm import ObsRunningMeanStd, VectorEnvNormObs\n"
+            "from fsrl_b200 import envs\nassert envs.VectorEnvNormObs is VectorEnvNormObs\n"
+            "assert envs.ObsRunningMeanStd is ObsRunningMeanStd\n")
+    subprocess.run([sys.executable, "-c", code], cwd=root, check=True)
+
+
 def test_agents_pass_the_wrapper_through():
     from fsrl_b200.agent.base_agent import _as_vector
     from fsrl_b200.envs import DeviceVectorEnv, VectorEnvNormObs
