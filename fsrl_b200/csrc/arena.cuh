@@ -61,7 +61,7 @@ struct AdamStep {
 };
 
 // the scalars of step t as torch computes them: python doubles, rounded to f32 at the op
-inline AdamStep adam_step_scalars(double lr, double beta1, double beta2, double eps, long long t) {
+__host__ __device__ inline AdamStep adam_step_scalars(double lr, double beta1, double beta2, double eps, long long t) {
     const double bc1 = 1.0 - pow(beta1, (double)t), bc2 = 1.0 - pow(beta2, (double)t);
     return AdamStep{(float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)sqrt(bc2), (float)eps,
                     (float)(-(lr / bc1))};

@@ -244,8 +244,8 @@ __global__ void alpha_step_kernel(const fsrl_offpolicy_t d, const float* __restr
     stat_out[FSRL_OFF_ST_ALPHA_LOSS] = -la * (mean_lp + d.target_entropy);
     float m = st[1], v = st[2];
     const float t = st[3] + 1.0f;
-    const float bc1 = 1.0f - powf(0.9f, t), bc2 = 1.0f - powf(0.999f, t);
-    const AdamStep ad = {0.1f, 0.999f, 0.001f, sqrtf(bc2), 1e-8f, -(d.alpha_lr / bc1)};   // f32 scalars, as before
+    // torch's bias corrections, in double: in f32, 1 - 0.999f^t loses ~1e-5 of its value to the rounding of 0.999f
+    const AdamStep ad = adam_step_scalars(d.alpha_lr, 0.9, 0.999, 1e-8, (long long)t);
     const float nla = adam_update(la, g, m, v, ad);
     st[0] = nla; st[1] = m; st[2] = v; st[3] = t;
     *d.alpha = expf(nla);

@@ -87,6 +87,55 @@ def cg_stop_tol(res, lo=2, hi=7):
     return k, (min(res[:k]) * res[k]) ** 0.5
 
 
+KEY_UPD = 0x55504454
+
+
+def upd_noise(seed, B, A, step, stream_id):
+    """eps [B, A] of the off-policy update's reparameterised samples at gradient step `step`
+    (csrc/offpolicy.cu sac_sample_kernel): stream 0 draws the target-side sample, stream 1 the actor's."""
+    from oracle.philox import normal_pair, philox4x32
+    out = np.zeros((B, A), np.float32)
+    b = np.arange(B, dtype=np.uint32)
+    for c in range((A + 3) // 4):
+        r = philox4x32(b, np.uint32(step & 0xFFFFFFFF), np.uint32((step >> 32) * 8 + c), np.uint32(stream_id), seed, KEY_UPD)
+        n = list(normal_pair(r[0], r[1])) + list(normal_pair(r[2], r[3]))
+        for j in range(4):
+            if 4 * c + j < A:
+                out[:, 4 * c + j] = n[j]
+    return torch.from_numpy(out)
+
+
+def synthetic_ring(D, A, n_env, cap, layout, seed=0, max_action=1.0, p_term=0.02, p_trunc=0.01):
+    """A VectorReplayBuffer filled directly, without collecting.  layout: "wrapped" (every ring full,
+    ptr mid-ring), "partial" (every ring partly filled) or "mixed" (alternate envs).  Besides the
+    random flags, env e gets a termination (even e) or a truncation (odd e) 1 + e % 8 steps before
+    its ptr, so n-step walks from near the newest slot meet both kinds of ends at every distance."""
+    from fsrl_b200.data import VectorReplayBuffer
+    g = np.random.default_rng(seed)
+    buf = VectorReplayBuffer(n_env * cap, n_env, device="cuda")
+    buf.allocate(D, A)
+    n = n_env * cap
+    f32 = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).cuda()
+    buf.obs.copy_(f32(g.standard_normal((n, D))))
+    buf.obs_next.copy_(f32(g.standard_normal((n, D))))
+    buf.act.copy_(f32(max_action * g.uniform(-1.0, 1.0, (n, A))))
+    buf.rew.copy_(f32(g.standard_normal(n)))
+    buf.cost.copy_(f32(g.random(n) < 0.3))
+    term, trunc = g.random(n) < p_term, g.random(n) < p_trunc
+    ptr, ln = np.zeros(n_env, np.int64), np.zeros(n_env, np.int64)
+    for e in range(n_env):
+        full = layout == "wrapped" or (layout == "mixed" and e % 2 == 0)
+        ptr[e] = g.integers(1, cap) if full else g.integers(max(cap // 3, 9), cap)
+        ln[e] = cap if full else ptr[e]
+        k = e * cap + (ptr[e] - 1 - e % 8) % cap
+        term[k], trunc[k] = e % 2 == 0, e % 2 == 1
+    buf.terminated.copy_(torch.from_numpy(term.astype(np.uint8)).cuda())
+    buf.truncated.copy_(torch.from_numpy(trunc.astype(np.uint8)).cuda())
+    buf.ptr.copy_(torch.from_numpy(ptr.astype(np.int32)).cuda())
+    buf.len.copy_(torch.from_numpy(ln.astype(np.int32)).cuda())
+    return buf
+
+
 def buffer_to_numpy(buf):
     g = lambda t: t.detach().cpu().numpy()
     return dict(obs=g(buf.obs), obs_next=g(buf.obs_next), act=g(buf.act), rew=g(buf.rew),

@@ -7,24 +7,9 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import buffer_to_numpy
+from helpers import buffer_to_numpy, synthetic_ring, upd_noise as _upd_noise
 
 pytestmark = pytest.mark.gpu
-KEY_UPD = 0x55504454
-
-
-def _upd_noise(seed, B, A, step, stream_id):
-    from oracle.philox import normal_pair, philox4x32
-    out = np.zeros((B, A), np.float32)
-    b = np.arange(B, dtype=np.uint32)
-    for c in range((A + 3) // 4):
-        r = philox4x32(b, np.uint32(step & 0xFFFFFFFF), np.uint32((step >> 32) * 8 + c), np.uint32(stream_id), seed, KEY_UPD)
-        n = list(normal_pair(r[0], r[1])) + list(normal_pair(r[2], r[3]))
-        for j in range(4):
-            if 4 * c + j < A:
-                out[:, 4 * c + j] = n[j]
-    return torch.from_numpy(out)
-
 
 def _build(algo, task="SafetyCarRun-v0", hidden=(64, 64), n_env=4, seed=10):
     from fsrl_b200 import envs
@@ -67,30 +52,49 @@ def _flat(mods):
 
 
 def test_nstep_prepare_matches_oracle():
+    """The n-step walk on a collected ring that never wrapped, and on synthetic rings: full rings wrapped with
+    ptr mid-ring, partly filled rings, and terminations and truncations 1 to 8 steps before ptr, up to
+    n_step = FSRL_MAX_NSTEP = 8.  n_step = 9 is refused."""
     import ctypes
     from fsrl_b200 import _lib
     from oracle import offpolicy as ooff
     policy, venv, buf, col = _build("ddpg", n_env=3)
     col.collect(n_episode=5)                    # several episodes per env, ring not wrapped
     policy._ensure_engine(256)
-    ob = _oracle_buffer(buf)
+    D, A = venv.D, venv.A
     rng = np.random.default_rng(0)
-    valid = ob.sample_all()
-    idx = rng.choice(valid, 256).astype(np.int32)
-    for n_step in (1, 2, 3, 5):
-        policy._n_step = n_step
-        d = policy._descriptor(buf)
-        it = torch.as_tensor(idx, device="cuda")
-        _lib.check(_lib.lib.fsrl_nstep_prepare(ctypes.byref(d), it.data_ptr(), 256, torch.cuda.current_stream().cuda_stream))
-        torch.cuda.synchronize()
-        tq = [rng.standard_normal(256).astype(np.float32) for _ in range(2)]
-        rets, terminal = ooff.nstep_targets(ob, idx, tq, 0.97 if False else policy._gamma, n_step)
-        w = policy._w
-        assert np.array_equal(w["term_idx"].cpu().numpy()[:256], terminal.astype(np.int32))      # integer-exact
-        vm = w["vmask"].cpu().numpy()[:256]; gp = w["gpow"].cpu().numpy()[:256]; part = w["partial"].cpu().numpy()
-        for i in range(2):
-            got = (tq[i] * vm).astype(np.float64) * gp + part[i * 256:(i + 1) * 256]
-            np.testing.assert_allclose(got.astype(np.float32), rets[:, i], rtol=1e-6, atol=1e-6)
+    s = torch.cuda.current_stream().cuda_stream
+    rings = [(buf, (1, 2, 3, 5))] + [(synthetic_ring(D, A, 8, 64, layout, seed=k), (1, 2, 5, 8))
+                                     for k, layout in enumerate(("wrapped", "partial", "mixed"))]
+    for ring, n_steps in rings:
+        ob = _oracle_buffer(ring)
+        valid = ob.sample_all()
+        # every transition within 9 steps of a ring's newest slot, where the walk wraps or stops, plus random ones
+        near = np.concatenate([e * ob.cap + (ob.ptr[e] - 1 - np.arange(9)) % ob.cap for e in range(ob.E) if ob.len[e] >= 9])
+        idx = np.concatenate([near, rng.choice(valid, 256 - len(near))]).astype(np.int32)
+        assert np.isin(idx, valid).all()
+        for n_step in n_steps:
+            policy._n_step = n_step
+            d = policy._descriptor(ring)
+            it = torch.as_tensor(idx, device="cuda")
+            _lib.check(_lib.lib.fsrl_nstep_prepare(ctypes.byref(d), it.data_ptr(), 256, s))
+            torch.cuda.synchronize()
+            tq = [rng.standard_normal(256).astype(np.float32) for _ in range(2)]
+            rets, terminal = ooff.nstep_targets(ob, idx, tq, policy._gamma, n_step)
+            w = policy._w
+            assert np.array_equal(w["term_idx"].cpu().numpy()[:256], terminal.astype(np.int32))      # integer-exact
+            vm = w["vmask"].cpu().numpy()[:256]; gp = w["gpow"].cpu().numpy()[:256]; part = w["partial"].cpu().numpy()
+            assert np.array_equal(vm, (~ob.terminated[terminal]).astype(np.float32))
+            for i in range(2):
+                got = (tq[i] * vm).astype(np.float64) * gp + part[i * 256:(i + 1) * 256]
+                np.testing.assert_allclose(got.astype(np.float32), rets[:, i], rtol=1e-6, atol=1e-6)
+        if ring is not buf:
+            # the synthetic rings put both kinds of ends inside the 8-step walks
+            assert ob.terminated[terminal].any() and (ob.truncated[terminal] & ~ob.terminated[terminal]).any()
+    policy._n_step = 9
+    d = policy._descriptor(buf)
+    with pytest.raises(ValueError, match="n_step 9 out of range"):
+        _lib.check(_lib.lib.fsrl_nstep_prepare(ctypes.byref(d), it.data_ptr(), 256, s))
 
 
 @pytest.mark.parametrize("auto_alpha", [True, False])
