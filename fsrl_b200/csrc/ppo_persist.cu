@@ -111,7 +111,12 @@ struct Args {
     unsigned dp_seq;         // data-parallel runs: launch sequence number (same on every rank), upper half of the packet tags
     int dp_direct;           // W2 gradient tiles exchanged in one hop (2 ranks) instead of the two-hop owner scheme
 };
-constexpr int DBG_N = 48;
+// clock stamps per CTA: 0 .. 47 phase boundaries (tools/persist_check.py names them), then per chunk of each GEMM phase
+// (g = 0: G1, 1: G2 / G3) DBG_CH + 3 NCH g + NCH e + j: e = 0 the producer's bar_empty wait returned, 1 its copies
+// were issued, 2 warpgroup 0's bar_full wait returned.  The per-chunk stamps exist only in a build with
+// -DFSRL_PPO_CHUNK_STAMPS: even untaken, their checks inside the chunk loops lengthen every step (~0.7 us on c2).
+constexpr int DBG_CH = 48;
+constexpr int DBG_N = DBG_CH + 2 * 3 * NCH;
 #define STAMP(i) do { if (P.dbg && t == P.dbg_step) P.dbg[(size_t)blockIdx.x * DBG_N + (i)] = clock64(); } while (0)
 
 struct AdamS { float w1, b2, w2, rbc2s, eps, neg_step; };
@@ -205,10 +210,13 @@ __device__ __forceinline__ float ld_cluster(uint32_t raddr) {
     asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(raddr) : "memory");
     return v;
 }
-// remote mbarrier arrival with cluster-scope release: the CTA's shared-memory stores before it (ordered by a CTA barrier)
-// are visible to a peer that acquires the phase (mbar_wait_cluster) -- once per step, so the fence it implies is cheap
-__device__ __forceinline__ void mbar_arrive_release_cluster(uint32_t raddr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
+// remote mbarrier arrivals with cluster-scope release on two peers: the CTA's shared-memory stores before them (ordered by
+// a CTA barrier) are visible to a peer that acquires the phase (mbar_wait_cluster).  One fence, then relaxed arrivals:
+// the same release pattern as two release arrivals, which would each carry a GPU-scope memory barrier.
+__device__ __forceinline__ void mbar_arrive_release_cluster2(uint32_t raddr0, uint32_t raddr1) {
+    asm volatile("fence.acq_rel.cluster;\n\t"
+                 "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];\n\t"
+                 "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%1];" ::"r"(raddr0), "r"(raddr1) : "memory");
 }
 __device__ __forceinline__ bool mbar_wait_cluster(uint64_t* bar, uint32_t parity, long long timeout_cycles) {
     const long long t0 = clock64();
@@ -266,7 +274,8 @@ __device__ __forceinline__ void acc_st(float* accs, int row, int col, const floa
 // flight.
 template <int N>
 __device__ __forceinline__ void gemm_phase(const unsigned char* ring, unsigned& qq, uint64_t* bar_full, uint32_t empty_r,
-                                           float (&dm)[N / 2], float (&dc)[N / 2], int* err, int code, int lane) {
+                                           float (&dm)[N / 2], float (&dc)[N / 2], int* err, int code, int lane,
+                                           const Args& P, int t, int g) {
 #pragma unroll
     for (int e = 0; e < N / 2; ++e) dm[e] = dc[e] = 0.f;
     const uint32_t ring_a = smem_u32(ring);
@@ -274,6 +283,9 @@ __device__ __forceinline__ void gemm_phase(const unsigned char* ring, unsigned& 
     for (int j = 0; j < NCH; ++j, ++qq) {
         const int s = qq % NSLOT;
         if (!mbar_wait(&bar_full[s], (qq / NSLOT) & 1, WAIT_CYCLES)) fail(err, code);
+#ifdef FSRL_PPO_CHUNK_STAMPS
+        if (P.dbg && t == P.dbg_step && threadIdx.x < 32) P.dbg[(size_t)blockIdx.x * DBG_N + DBG_CH + 3 * NCH * g + 2 * NCH + j] = clock64();
+#endif
         __syncwarp();
         wgmma_fence();
         // descriptors of the slot's k-step 0; k-step ks starts 2048 (A) / 2 b_lbo (B) bytes further (the address field
@@ -607,23 +619,29 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             for (int t = 0; t < P.n_mb; ++t) {
                 if (!flag_wait_ge<true>(fl_net + F_A * FLAG_LINE, 32u * (t + 1), WAIT_CYCLES)) fail(P.err, 10);
                 STAMP(12);
-                fence_proxy_async();
+                fence_proxy_async_global();
                 // the producer loops stay rolled: one thread runs them, and the kernel's instruction footprint is tight
 #pragma unroll 1
                 for (int j = 0; j < NCH; ++j, ++qq) {             // G1: K = k in chunks of KC
                     const int s = qq % NSLOT;
                     if (!mbar_wait(&bar_empty[s], ((qq / NSLOT) & 1) ^ 1, WAIT_CYCLES)) fail(P.err, 11);
+#ifdef FSRL_PPO_CHUNK_STAMPS
+                    STAMP(DBG_CH + j);
+#endif
                     unsigned char* dst = ring + (size_t)s * SLOT_BYTES;
                     mbar_expect_tx(&bar_full[s], 3 * A_CHUNK);
                     const size_t ao = (size_t)a * 16384 + (size_t)j * 64 * KC, bo = (size_t)b * 8192 + (size_t)j * 32 * KC;
                     // A = H1A block a: the same for the 8 CTAs of the row block (cluster)
                     copy_operand(dst, wsn + (size_t)I_H1A_HI * IMG + ao, A_CHUNK, &bar_full[s], 8, b, 0xff);
                     copy_operand(dst + 2 * A_CHUNK, wsn + (size_t)I_W2A_HI * IMG + bo, A_CHUNK / 2, &bar_full[s], 1, 0, 0);
+#ifdef FSRL_PPO_CHUNK_STAMPS
+                    STAMP(DBG_CH + NCH + j);
+#endif
                 }
                 STAMP(13);
                 if (!flag_wait_ge<true>(fl_net + F_C * FLAG_LINE, 32u * (t + 1), WAIT_CYCLES)) fail(P.err, 12);
                 STAMP(14);
-                fence_proxy_async();
+                fence_proxy_async_global();
                 const int ia = is_g2 ? I_W2B_HI : I_DZT_HI, ib = is_g2 ? I_DZA_HI : I_H1T_HI;
                 const int blk_a = is_g2 ? ka : q4, blk_b = is_g2 ? q4 : ka;
                 // the k block ka (G2: A = W2B, G3: B = H1T) is shared by the 4 CTAs with the same b >> 2, the block q4
@@ -633,11 +651,17 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 for (int j = 0; j < NCH; ++j, ++qq) {             // G2: K = o ; G3: K = r ; chunks of KC
                     const int s = qq % NSLOT;
                     if (!mbar_wait(&bar_empty[s], ((qq / NSLOT) & 1) ^ 1, WAIT_CYCLES)) fail(P.err, 13);
+#ifdef FSRL_PPO_CHUNK_STAMPS
+                    STAMP(DBG_CH + 3 * NCH + j);
+#endif
                     unsigned char* dst = ring + (size_t)s * SLOT_BYTES;
                     mbar_expect_tx(&bar_full[s], 4 * A_CHUNK);
                     const size_t ao = (size_t)blk_a * 16384 + (size_t)j * 64 * KC, bo = (size_t)blk_b * 16384 + (size_t)j * 64 * KC;
                     copy_operand(dst, wsn + (size_t)ia * IMG + ao, A_CHUNK, &bar_full[s], is_g2 ? 4 : 2, is_g2 ? b & 3 : b >> 2, is_g2 ? m4 : m2);
                     copy_operand(dst + 2 * A_CHUNK, wsn + (size_t)ib * IMG + bo, A_CHUNK, &bar_full[s], is_g2 ? 2 : 4, is_g2 ? b >> 2 : b & 3, is_g2 ? m2 : m4);
+#ifdef FSRL_PPO_CHUNK_STAMPS
+                    STAMP(DBG_CH + 4 * NCH + j);
+#endif
                 }
             }
         }
@@ -818,7 +842,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             // ---- G1 (wgmma), then its epilogue: h2 = relu(acc + b2), head partial over this tile's 32 columns ----
             {
                 float dm[16], dc[16];
-                if (wq == 0) gemm_phase<32>(ring, qq, bar_full, empty_r, dm, dc, P.err, 30, lane);
+                if (wq == 0) gemm_phase<32>(ring, qq, bar_full, empty_r, dm, dc, P.err, 30, lane, P, t, 0);
                 else qq += NCH;
                 stage_acc<32>(accs, dm, dc, wq, sp, lane);
             }
@@ -1053,7 +1077,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             }
             {
                 float dm[32], dc[32];
-                if (wq == 0) gemm_phase<64>(ring, qq, bar_full, empty_r, dm, dc, P.err, 32, lane);
+                if (wq == 0) gemm_phase<64>(ring, qq, bar_full, empty_r, dm, dc, P.err, 32, lane, P, t, 1);
                 else qq += NCH;
                 stage_acc<64>(accs, dm, dc, wq, sp, lane);
             }
@@ -1086,10 +1110,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 if (et == 0) STAMP(23);
                 epi_bar();
                 // the reducers of column blocks 2 ka and 2 ka + 1 (cluster ranks = column blocks) may read them now
-                if (et == 0) {
-                    mbar_arrive_release_cluster(mapa_u32(smem_u32(&bar_w1), 2 * ka));
-                    mbar_arrive_release_cluster(mapa_u32(smem_u32(&bar_w1), 2 * ka + 1));
-                }
+                if (et == 0) mbar_arrive_release_cluster2(mapa_u32(smem_u32(&bar_w1), 2 * ka), mapa_u32(smem_u32(&bar_w1), 2 * ka + 1));
             } else {
                 float g[C2];
                 acc_ld<C2>(accs, trow, cb2, g);

@@ -73,9 +73,10 @@ __device__ __forceinline__ void bulk_g2s_multicast(void* smem_dst, const void* g
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
         ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask) : "memory");
 }
-// orders this thread's earlier generic-proxy operations (the acquire of a flag) before its later
-// async-proxy operations (bulk copies reading what another SM wrote with ordinary stores)
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
+// orders this thread's earlier generic-proxy operations on global memory (the acquire of a flag) before its later
+// async-proxy operations (bulk copies reading what another SM wrote with ordinary stores).  Restricted to global
+// memory: the unqualified fence.proxy.async also carries a GPU-scope memory barrier (MEMBAR.ALL.GPU in the SASS).
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 // orders this thread's earlier generic stores to shared memory before later async-proxy writes to the same bytes
 // (scratch in the operand ring that the next phase's bulk copies overwrite)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }

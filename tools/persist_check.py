@@ -5,7 +5,9 @@
    fp64 evaluation of the same minibatch, and compare parameters / Adam moments after the step with the
    three-launch chain (csrc/ppo.cu) and with the fp32 oracle;
 2. a 75-step epoch (64 envs x 300 steps): per-step statistics and final parameters, persistent vs chain;
-3. timing of both paths on the c2-shaped batch when --time is given.
+3. timing of both paths on the c2-shaped batch when --time is given.  The per-chunk table of the GEMM phases needs a
+   library built with the chunk stamps:
+       touch fsrl_b200/csrc/ppo_persist.cu && make -C fsrl_b200/csrc EXTRA_NVCCFLAGS=-DFSRL_PPO_CHUNK_STAMPS
 
 Usage: python tools/persist_check.py [--time]"""
 import copy
@@ -24,6 +26,9 @@ from helpers import build_ppo, oracle_nets  # noqa: E402
 from test_ppo_scale_gpu import _adam, _collect, _sub_batch  # noqa: E402
 
 IMG = 65536
+N_CTA = 96              # 32 CTAs per network, 3 networks
+DBG_N = 96              # clock stamps per CTA: pp::DBG_N in csrc/ppo_persist.cu
+DBG_CH, NCH = 48, 8     # first per-chunk stamp (pp::DBG_CH), chunks per GEMM phase (pp::NCH)
 NAMES = ["H1A_HI", "H1A_LO", "H1T_HI", "H1T_LO", "DZA_HI", "DZA_LO", "DZT_HI", "DZT_LO", "W2A_HI", "W2A_LO", "W2B_HI", "W2B_LO"]
 
 
@@ -51,6 +56,37 @@ def run(policy, batch, bs, persist, seed=3):
     policy.learn(batch, batch_size=bs, repeat=1)
     torch.cuda.synchronize()
     return {k: np.asarray(v).copy() for k, v in policy.last_stats.items()}
+
+
+def chunk_report(dbg, red):
+    """Per chunk of each GEMM phase (stamps DBG_CH ..): when the producer's bar_empty wait returned, when it had issued
+    the chunk's copies and when warpgroup 0's bar_full wait returned (the chunk landed), in cycles since the phase's
+    flag passed (stamp 12 / 14); issue -> land latency, the period between landings and, by Little's law, the bytes in
+    flight (latency / period chunks of the phase's chunk size)."""
+    rel = dbg - dbg[:, :1]
+    for g, (name, flag, chunk_kb) in enumerate((("G1", 12, 24), ("G2 / G3", 14, 32))):
+        base = DBG_CH + 3 * NCH * g
+        for grp, sel in (("G2 reducer CTAs", [i for i in range(N_CTA) if red(i)]),
+                         ("other G2 CTAs", [i for i in range(N_CTA) if i % 32 < 16 and not red(i)]),
+                         ("G3 CTAs", [i for i in range(N_CTA) if i % 32 >= 16])):
+            sel = [i for i in sel if dbg[i, base:base + 3 * NCH].all() and dbg[i, flag] != 0]
+            if not sel:
+                print("  (no per-chunk stamps: build with EXTRA_NVCCFLAGS=-DFSRL_PPO_CHUNK_STAMPS for the %s table)" % name)
+                return
+            t0 = rel[sel, flag][:, None]
+            emp, iss, land = (rel[sel, base + e * NCH: base + (e + 1) * NCH] - t0 for e in range(3))
+            lat = land - iss
+            per = np.diff(land, axis=1)
+            print("  --- %s chunks, %s (%d CTAs): cycles since the flag passed (means) ---" % (name, grp, len(sel)))
+            print("     chunk   empty ok   issued   landed   issue->land   period")
+            for j in range(NCH):
+                print("    %5d %10.0f %8.0f %8.0f %13.0f %8s" % (j, emp[:, j].mean(), iss[:, j].mean(), land[:, j].mean(),
+                                                                 lat[:, j].mean(), "%.0f" % per[:, j - 1].mean() if j else "-"))
+            l_m, p_m = lat.mean(), per.mean()
+            print("    %s: latency %.0f cycles (chunk min %.0f / max %.0f), period %.0f cycles, window flag -> last land %.0f "
+                  "cycles, in flight latency / period = %.2f chunks = %.0f KB -> %.1f B/clk" % (
+                      name, l_m, lat.mean(axis=0).min(), lat.mean(axis=0).max(), p_m, land[:, -1].mean(), l_m / p_m,
+                      l_m / p_m * chunk_kb, chunk_kb * 1024 / p_m))
 
 
 def main():
@@ -85,7 +121,7 @@ def main():
     # decode the images (they hold the operands of the LAST step = the only step)
     ws = policy._persist_ws.detach().cpu().numpy()
     from fsrl_b200 import _lib as _fl
-    lib_net_ws = int(_fl.lib.fsrl_ppo_persist_ws_floats(2, 8, 256)) - int(_fl.lib.fsrl_ppo_persist_ws_floats(1, 8, 256)) - 2 * 32 - 2 * 32 * 48   # minus one network's flag lines (A, C) and stamp rows
+    lib_net_ws = int(_fl.lib.fsrl_ppo_persist_ws_floats(2, 8, 256)) - int(_fl.lib.fsrl_ppo_persist_ws_floats(1, 8, 256)) - 2 * 32 - 2 * 32 * DBG_N   # minus one network's flag lines (A, C) and stamp rows
     x = sub.obs.cpu().double().numpy()
     perm = None
     for net in range(3):
@@ -138,11 +174,11 @@ def main():
             print("  c2 epoch (2400 steps) %s: %.1f ms -> %.2f us / step" % ("persistent" if persist else "chain", dt * 1e3, dt * 1e6 / 2400))
         # per-phase clock stamps of one step in the middle of the epoch (FSRL_PPO_PERSIST_DBG=<step>)
         os.environ["FSRL_PPO_PERSIST_DBG"] = "1000"
-        policy2._persist_ws[-2 * 96 * 48:].zero_()          # stamps a CTA does not take stay 0 and are left out below
+        policy2._persist_ws[-2 * N_CTA * DBG_N:].zero_()          # stamps a CTA does not take stay 0 and are left out below
         run(policy2, batch2, 256, True, seed=5)
         del os.environ["FSRL_PPO_PERSIST_DBG"]
         ws = policy2._persist_ws.detach().cpu().numpy()
-        dbg = ws[-2 * 96 * 48:].view(np.int64).reshape(96, 48)
+        dbg = ws[-2 * N_CTA * DBG_N:].view(np.int64).reshape(N_CTA, DBG_N)
         names = {1: "S done (h1 tile + W2 images)", 2: "G1 accumulators ready", 3: "head partial written", 4: "hop B passed",
                  5: "dz2 + partials written", 6: "G2/G3 accumulators ready", 7: "G2/G3 epilogue done",
                  8: "[reducer] dW1 partials arrived", 9: "sumsq (+ slice) out", 10: "flag D2 passed",
@@ -171,6 +207,7 @@ def main():
             b0 = [i for i in sel if i % 8 == 0]
             print("         (b == 0 CTAs)        B passed %6.0f | loss %6.0f | images %6.0f | sums %6.0f | C arrive %6.0f" % tuple(
                 rel[b0, i].mean() for i in (4, 26, 27, 28, 5)))
+        chunk_report(dbg, red)
         gt = dbg[:, 30]
         print("  step start skew across CTAs (globaltimer ns): %d" % (gt.max() - gt.min()))
         cyc = (dbg[:, 29] - dbg[:, 0]) / 64.0

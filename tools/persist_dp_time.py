@@ -10,7 +10,9 @@ import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 import bench  # noqa: E402
+from persist_check import DBG_N, N_CTA  # noqa: E402
 
 
 def main():
@@ -26,12 +28,12 @@ def main():
         bench.one_cycle(trainer)
     torch.cuda.synchronize()
     os.environ["FSRL_PPO_PERSIST_DBG"] = "1000"
-    agent.policy._persist_ws[-2 * 96 * 48:].zero_()      # stamps a CTA does not take stay 0 and are left out below
+    agent.policy._persist_ws[-2 * N_CTA * DBG_N:].zero_()      # stamps a CTA does not take stay 0 and are left out below
     bench.one_cycle(trainer)
     torch.cuda.synchronize()
     del os.environ["FSRL_PPO_PERSIST_DBG"]
     ws = agent.policy._persist_ws.detach().cpu().numpy()
-    dbg = ws[-2 * 96 * 48:].view(np.int64).reshape(96, 48)
+    dbg = ws[-2 * N_CTA * DBG_N:].view(np.int64).reshape(N_CTA, DBG_N)
     rel = dbg - dbg[:, :1]
     names = {1: "S done", 2: "G1 accumulators ready", 4: "hop B passed", 5: "dz2 + partials written", 6: "G2/G3 accumulators ready",
              7: "G2/G3 epilogue done", 8: "[reducer] dW1 partials arrived",
