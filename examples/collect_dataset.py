@@ -11,7 +11,13 @@ collects with ``FastCollector(..., traj_buffer=...)`` over N device envs.  Test 
 through ``BasicCollector`` and also feed the buffer.  The dataset is written as
 ``<logdir>/<name>/dataset.npz`` (see TrajectoryBuffer.save).
 
+``--user_env True`` collects the dataset of a user-written gymnasium-style env instead of a registered task
+(``HazardReach`` of ``examples/train_host_env.py``): ``DummyVectorEnv`` over its constructors for N > 1 and
+``BasicCollector`` over one instance otherwise, both stepping it on the host while the actor, the ring and the
+trajectory copies stay on the GPU.
+
   python examples/collect_dataset.py --task SafetyCarCircle-v0 --epoch 20 --training_num 64
+  python examples/collect_dataset.py --user_env True --epoch 20 --training_num 16
 """
 import ast
 import os
@@ -29,7 +35,7 @@ import bullet_safety_gym  # noqa: E402,F401  (task registration side effect in t
 import gymnasium as gym  # noqa: E402
 import torch  # noqa: E402
 from tianshou.data import ReplayBuffer, VectorReplayBuffer  # noqa: E402
-from tianshou.env import ShmemVectorEnv, SubprocVectorEnv  # noqa: E402,F401
+from tianshou.env import DummyVectorEnv, ShmemVectorEnv, SubprocVectorEnv  # noqa: E402,F401
 from tianshou.utils.net.common import Net  # noqa: E402
 from tianshou.utils.net.continuous import ActorProb, Critic  # noqa: E402
 from torch.distributions import Independent, Normal  # noqa: E402
@@ -40,11 +46,13 @@ from fsrl.trainer import OnpolicyTrainer  # noqa: E402
 from fsrl.utils import DummyLogger  # noqa: E402
 from fsrl.utils.exp_util import seed_all  # noqa: E402
 from fsrl.utils.net.common import ActorCritic  # noqa: E402
+from train_host_env import HazardReach  # noqa: E402
 
 
 @dataclass
 class TrainCfg:
     task: str = "SafetyCarCircle-v0"
+    user_env: bool = False            # HazardReach, a user env stepped on the host, instead of `task`
     cost_start: float = 5
     cost_end: float = 100
     epoch_start: int = 100
@@ -105,7 +113,13 @@ def main(argv=None):
     args = TrainCfg(**cfg)
     seed_all(args.seed)
 
-    env = gym.make(args.task)
+    if args.user_env:
+        def make_env(i=0):
+            return HazardReach(seed=args.seed + i)
+    else:
+        def make_env(i=0):
+            return gym.make(args.task)
+    env = make_env()
     state_shape, action_shape = env.observation_space.shape, env.action_space.shape
     max_action = env.action_space.high[0]
     net = Net(state_shape, hidden_sizes=args.hidden_sizes, device=args.device)
@@ -134,10 +148,11 @@ def main(argv=None):
     if args.training_num == 1:
         train_collector = BasicCollector(policy, env, ReplayBuffer(args.buffer_size), traj_buffer=traj_buffer)
     else:
-        train_envs = eval(args.worker)([lambda: gym.make(args.task) for _ in range(args.training_num)])
+        worker = DummyVectorEnv if args.user_env else eval(args.worker)
+        train_envs = worker([lambda i=i: make_env(i) for i in range(args.training_num)])
         train_collector = FastCollector(policy, train_envs, VectorReplayBuffer(args.buffer_size, len(train_envs)),
                                         exploration_noise=True, traj_buffer=traj_buffer)
-    test_collector = BasicCollector(policy, gym.make(args.task), traj_buffer=traj_buffer)
+    test_collector = BasicCollector(policy, make_env(1000), traj_buffer=traj_buffer)
     trainer = OnpolicyTrainer(
         policy=policy, train_collector=train_collector, test_collector=test_collector, max_epoch=args.epoch,
         batch_size=args.batch_size, cost_limit=args.cost_end, step_per_epoch=args.step_per_epoch,

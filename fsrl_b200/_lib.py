@@ -222,6 +222,8 @@ SIGNATURES = {
     "fsrl_traj_begin": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_vp]),
     "fsrl_traj_scan": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajScan), c_int, c_vp]),
     "fsrl_traj_copy": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajArena), c_vp, c_int, c_vp]),
+    "fsrl_traj_copy_host": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(TrajArena), c_int, c_int, c_vp, c_int,
+                                    c_vp]),
     "fsrl_traj_gather": (c_int, [ctypes.POINTER(TrajArena), ctypes.POINTER(TrajArena), c_vp, c_int, c_vp]),
     "fsrl_mlp_forward": (c_int, [ctypes.POINTER(Mlp3), c_vp, c_vp, ctypes.c_longlong, c_vp, c_vp]),
     "fsrl_engine_slot_floats": (c_size, [c_int, c_int]),

@@ -4,7 +4,9 @@
 // (/root/reference/fsrl/data/traj_buf.py:60-95, fed one step at a time by basic_collector.py:238-248).
 //   scan   one thread per env walks the ring slots written since the last scan and emits one
 //          row per finished episode (return / cost summed in fp64 in time order, as ep_rew)
-//   copy   one CTA per kept episode: ring -> arena slot, actions remapped like the env saw them
+//   copy   one CTA per kept episode: ring -> arena slot, actions remapped like the env saw them; the
+//          ring of host-stepped envs takes the same kernel with its widths from the caller (no scan:
+//          the host collect loop knows every finished episode)
 //   gather one CTA per kept trajectory: arena slots -> contiguous tensors (get_all / save)
 // copy and gather are bandwidth-bound: 16-byte streaming loads and stores wherever source and
 // destination share their alignment.
@@ -126,9 +128,13 @@ __global__ void __launch_bounds__(TRAJ_TPB) traj_gather_kernel(const fsrl_traj_a
 
 using namespace fsrl;
 
-static int check_ring(const fsrl_rollout_t* r) {
+// host: the descriptor of a host-stepped env (kind -1), whose widths the caller gives
+static int check_ring(const fsrl_rollout_t* r, bool host = false) {
     FSRL_REQUIRE(r != nullptr, "trajectory harvest: null rollout descriptor");
-    FSRL_REQUIRE(env_kind_known(r->kind), "trajectory harvest: unknown env kind %d", r->kind);
+    if (host)
+        FSRL_REQUIRE(r->kind == -1, "trajectory copy: a host ring has env kind -1, got %d", r->kind);
+    else
+        FSRL_REQUIRE(env_kind_known(r->kind), "trajectory harvest: unknown env kind %d", r->kind);
     FSRL_REQUIRE(r->E > 0 && r->cap > 0, "trajectory harvest: E and cap must be positive");
     FSRL_REQUIRE(r->b_obs && r->b_obs_next && r->b_act && r->b_rew && r->b_cost && r->b_term && r->b_trunc &&
                  r->b_ptr, "trajectory harvest: the rollout has no transition ring");
@@ -167,13 +173,10 @@ extern "C" int fsrl_traj_scan(const fsrl_rollout_t* r, const fsrl_traj_scan_t* h
     return FSRL_OK;
 }
 
-extern "C" int fsrl_traj_copy(const fsrl_rollout_t* r, const fsrl_traj_arena_t* a, const int* jobs, int n_jobs,
-                              void* stream) {
-    int rc = check_ring(r);
-    if (rc || (rc = check_arena(a))) return rc;
-    const EnvDims d = env_dims(r->kind);
-    FSRL_REQUIRE(a->D == d.D && a->A == d.A, "trajectory copy: arena dims (%d, %d) != env dims (%d, %d)",
-                 a->D, a->A, d.D, d.A);
+static int launch_copy(const fsrl_rollout_t* r, const fsrl_traj_arena_t* a, int D, int A, const int* jobs,
+                       int n_jobs, void* stream) {
+    FSRL_REQUIRE(a->D == D && a->A == A, "trajectory copy: arena dims (%d, %d) != env dims (%d, %d)",
+                 a->D, a->A, D, A);
     FSRL_REQUIRE(n_jobs >= 0 && (n_jobs == 0 || jobs), "trajectory copy: bad job list");
     FSRL_REQUIRE((reinterpret_cast<uintptr_t>(jobs) & 15u) == 0, "trajectory copy: jobs must be 16-byte aligned");
     if (n_jobs == 0) return FSRL_OK;
@@ -181,6 +184,22 @@ extern "C" int fsrl_traj_copy(const fsrl_rollout_t* r, const fsrl_traj_arena_t* 
         *r, *a, reinterpret_cast<const int4*>(jobs));
     FSRL_LAUNCH_CHECK();
     return FSRL_OK;
+}
+
+extern "C" int fsrl_traj_copy(const fsrl_rollout_t* r, const fsrl_traj_arena_t* a, const int* jobs, int n_jobs,
+                              void* stream) {
+    int rc = check_ring(r);
+    if (rc || (rc = check_arena(a))) return rc;
+    const EnvDims d = env_dims(r->kind);
+    return launch_copy(r, a, d.D, d.A, jobs, n_jobs, stream);
+}
+
+extern "C" int fsrl_traj_copy_host(const fsrl_rollout_t* r, const fsrl_traj_arena_t* a, int D, int A,
+                                   const int* jobs, int n_jobs, void* stream) {
+    int rc = check_ring(r, true);
+    if (rc || (rc = check_arena(a))) return rc;
+    FSRL_REQUIRE(D >= 1 && A >= 1 && A <= ENV_MAX_A, "trajectory copy: bad host ring dims D=%d A=%d", D, A);
+    return launch_copy(r, a, D, A, jobs, n_jobs, stream);
 }
 
 extern "C" int fsrl_traj_gather(const fsrl_traj_arena_t* a, const fsrl_traj_arena_t* out, const long long* jobs,

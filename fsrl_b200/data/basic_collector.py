@@ -3,15 +3,19 @@
 optionally feeding a :class:`TrajectoryBuffer`.
 
 The reference steps a gym env on the host and hands every transition to
-``TrajectoryBuffer.store``.  Here the one env is a device env stepped by the fused rollout kernel
-(a one-env :class:`FastCollector`), and finished episodes reach the trajectory buffer through the
-device harvest; a single env makes the two orders the same (completion order).
+``TrajectoryBuffer.store``.  Here every collect goes through a one-env :class:`FastCollector`: a device env
+is stepped by the fused rollout kernel and finished episodes reach the trajectory buffer through the device
+harvest; any other gymnasium-style env (a real simulator, a user's own env) becomes a one-env
+:class:`HostVectorEnv`, stepped on the host while the device acts, stores and copies its finished episodes
+out of the ring.  A single env makes the two orders the same (completion order).
 """
 from __future__ import annotations
 
 from typing import Any, Dict, Optional
 
 from ..envs import DeviceEnv, DeviceVectorEnv
+from ..host_envs import HostVectorEnv, is_vector_env
+from ..obs_norm import VectorEnvNormObs
 from .buffer import DeviceVectorReplayBuffer
 from .fast_collector import FastCollector
 from .traj_buf import TrajectoryBuffer
@@ -21,8 +25,10 @@ class BasicCollector:
     """Collect whole episodes from one env.
 
     :param policy: a policy of :mod:`fsrl_b200.policy`.
-    :param env: what ``gym.make(task)`` returns (a :class:`DeviceEnv`, stepped with env seed 0) or a
-        :class:`DeviceVectorEnv` holding one env.
+    :param env: what ``gym.make(task)`` returns (a :class:`DeviceEnv`, stepped with env seed 0), a
+        :class:`DeviceVectorEnv` holding one env, any single gymnasium-style env (``reset`` / ``step``, ``Box``
+        spaces, 4- or 5-tuple ``step``, ``cost`` in ``info``), or a :class:`HostVectorEnv` or other vector env
+        holding one env.
     :param buffer: a replay buffer with one sub-buffer (``ReplayBuffer(size)``) that receives every
         transition; with None and a ``traj_buffer`` a private ring of the least size is used.
     :param bool exploration_noise: add the policy's exploration noise to its actions.
@@ -31,10 +37,20 @@ class BasicCollector:
 
     def __init__(self, policy, env, buffer: Optional[DeviceVectorReplayBuffer] = None,
                  exploration_noise: Optional[bool] = False, traj_buffer: Optional[TrajectoryBuffer] = None):
+        device = getattr(policy, "device", "cuda")
         if isinstance(env, DeviceEnv):
-            env = DeviceVectorEnv(env.task, 1, device=getattr(policy, "device", "cuda"), seed=0)
-        if not isinstance(env, DeviceVectorEnv) or len(env) != 1:
-            raise TypeError("BasicCollector steps one device env: pass gym.make(task) or a one-env DeviceVectorEnv")
+            env = DeviceVectorEnv(env.task, 1, device=device, seed=0)
+        elif isinstance(env, (DeviceVectorEnv, HostVectorEnv, VectorEnvNormObs)):
+            pass
+        elif is_vector_env(env):
+            if len(env) == 1:
+                env = HostVectorEnv.from_vector_env(env, device=device)
+        elif callable(getattr(env, "step", None)) and callable(getattr(env, "reset", None)):
+            env = HostVectorEnv._from_envs([env], device=device)
+        if not isinstance(env, (DeviceVectorEnv, HostVectorEnv)) or len(env) != 1:
+            raise TypeError("BasicCollector steps one env: pass gym.make(task), a gymnasium-style env, or a "
+                            f"DeviceVectorEnv / HostVectorEnv holding one env (got {type(env).__name__}"
+                            f"{f' of {len(env)} envs' if hasattr(env, '__len__') else ''})")
         self.env = env
         self.policy = policy
         self.exploration_noise = exploration_noise

@@ -20,7 +20,10 @@ A :class:`HostVectorEnv` (or any other object with tianshou's vector-env protoco
 envs' own ``step`` / ``reset``, and per vector step one launch (csrc/rollout_host.cu) stores the previous
 step's transitions into the same ring and computes this step's actions with the fused path's actor,
 sampling and noise stream.  Finished envs are reset, surplus ones retired without a reset, as on the
-device path; the statistics are summed on the host in float64, in step order.
+device path; the statistics are summed on the host in float64, in step order.  A ``traj_buffer`` is fed there
+without a ring scan: the loop offers each finished episode with the float64 return and cost the env reported, and
+copies the kept ones from the ring (``fsrl_traj_copy_host``) right after the launch that stores their last transition,
+so an episode must fit the ring (``cap >= max_episode_steps``, or ``cap >=`` its length when the horizon is unknown).
 
 An env wrapped by :class:`~fsrl_b200.obs_norm.VectorEnvNormObs` collects normalized observations: per vector step
 the statistics take the ``obs_next`` of every env that stepped, then the reset observations of the envs that
@@ -91,11 +94,9 @@ class FastCollector(object):
             raise NotImplementedError("preprocess_fn would need a host round trip per step")
         # host path: the host steps the envs, one launch per vector step acts and stores
         self.host = isinstance(env, HostVectorEnv)
-        if self.host and traj_buffer is not None:
-            raise NotImplementedError("traj_buffer harvests the ring of device envs only; host envs collect into "
-                                      "a VectorReplayBuffer")
         if self.host and not _fused_policy(policy):
-            raise NotImplementedError("host envs need a policy whose actor the rollout kernel runs (a built-in "
+            what = "host envs collecting into a traj_buffer" if traj_buffer is not None else "host envs"
+            raise NotImplementedError(f"{what} need a policy whose actor the rollout kernel runs (a built-in "
                                       "actor the parameter arena holds); this policy would take the generic path")
         self.env = env
         self.env_num = len(env)
@@ -103,8 +104,13 @@ class FastCollector(object):
         self._store = buffer is not None
         self.traj_buffer = traj_buffer
         if traj_buffer is not None:
-            self._harvest = TrajectoryHarvest(self.env_num, env.device)
+            if not self.host:       # host envs: the collect loop itself knows every finished episode, no scan
+                self._harvest = TrajectoryHarvest(self.env_num, env.device)
             if buffer is None:      # the harvest reads finished episodes from a ring: a private one of the least size
+                if self.host and env.max_episode_steps is None:
+                    raise ValueError("traj_buffer over host envs without a horizon (spec.max_episode_steps is None) "
+                                     "needs a buffer: a private ring cannot be sized; pass a VectorReplayBuffer "
+                                     "whose sub-buffers hold the longest episode")
                 buffer = DeviceVectorReplayBuffer(self.env_num * self.min_ring_capacity(), self.env_num)
         self._assign_buffer(buffer)
         self.policy = policy
@@ -153,8 +159,11 @@ class FastCollector(object):
     def min_ring_capacity(self, n_episode: Optional[int] = None) -> int:
         """Ring slots per env a ``traj_buffer`` harvest needs: an episode must still be in the ring when the scan
         after its last step runs.  That is once after the collect when every ready env runs one episode
-        (``n_episode <= env_num``), else after every chunk of ``min(T, 64)`` steps."""
+        (``n_episode <= env_num``), else after every chunk of ``min(T, 64)`` steps.  Host envs copy an episode
+        right after the launch that stores its last transition: ``T`` slots (None when the horizon is unknown)."""
         T = self.env.max_episode_steps
+        if self.host:
+            return T
         if n_episode is not None and n_episode <= self.env_num:
             return T
         return T + self._chunk()
@@ -240,7 +249,12 @@ class FastCollector(object):
         }
 
     def _host_steps(self, r, n_episode: int, render: bool, gym_reset_kwargs) -> types.SimpleNamespace:
-        """The reference's collect loop (:252-368) over host envs; the device acts and stores once per step."""
+        """The reference's collect loop (:252-368) over host envs; the device acts and stores once per step.
+
+        With a ``traj_buffer`` the loop also keeps every env's episode: its first ring slot (``b_ptr`` read once,
+        then advanced here by one per stored transition) and its float64 cost.  An env that finishes is offered
+        to the buffer in ascending env id within the step, the device path's (finish step, env) order, and the
+        kept episodes are copied out of the ring right after the next launch, which stores their last transition."""
         env = self.env
         E = self.env_num
         kw = gym_reset_kwargs or {}
@@ -252,10 +266,35 @@ class FastCollector(object):
         stored = None                         # the previous step's transitions, stored by the next launch
         norm = self.norm
         fresh = None                          # wrapped: the envs restarted since the last launch, and their obs
+        traj = self.traj_buffer
+        if traj is not None:
+            T, cap = env.max_episode_steps, self.buffer.cap
+            if T is not None and cap < T:
+                raise ValueError(f"a traj_buffer harvest of host envs needs a ring of at least {T} slots per env "
+                                 f"(max_episode_steps); the buffer has {cap}")
+            head = self.buffer.ptr[:E].cpu().numpy().astype(np.int64)   # the ring slot each env's next store takes
+            ep_start, ep_cost = head.copy(), np.zeros(E, np.float64)
+            jobs = []                         # kept episodes whose last transition the next launch stores
+            with torch.cuda.device(env.device):
+                stream = torch.cuda.current_stream().cuda_stream
         while True:
             act = env.device_step(r, ready, obs[ready], stored, norm, fresh)
             fresh = None
+            if traj is not None and jobs:
+                traj._copy_host(r, jobs, T or 0, env.D, env.A, env.device, stream)
+                jobs = []
             obs_next, rew, term, trunc, cost = env.step_envs(act, ready)
+            if traj is not None:
+                over = ready[ep_len[ready] >= cap]
+                if len(over):
+                    e = int(over[0])
+                    raise ValueError(f"env {e}'s episode reached {ep_len[e] + 1} steps, longer than the ring's "
+                                     f"{cap} slots per env: storing it would overwrite its first transition before "
+                                     "the traj_buffer copies it; pass a buffer whose sub-buffers hold the longest "
+                                     "episode")
+                ep_start[ready] = np.where(ep_len[ready] == 0, head[ready], ep_start[ready])
+                head[ready] = (head[ready] + 1) % cap
+                ep_cost[ready] += cost
             if render:
                 env.render()
             if self.buffer is not None or norm is not None:
@@ -273,6 +312,10 @@ class FastCollector(object):
                 st.sum_ep_len += int(np.sum(ep_len[ids]))
                 st.term_count += int(term.sum())
                 st.trunc_count += int(trunc.sum())
+                if traj is not None:
+                    jobs = traj._offer_episodes((int(e), int(ep_start[e]), int(ep_len[e]), float(ep_rew[e]),
+                                                 float(ep_cost[e])) for e in ids)
+                    ep_cost[ids] = 0.0
                 ep_rew[ids], ep_len[ids] = 0.0, 0
                 # the surplus rule (:357-363): the lowest finished ids retire, without a reset; the rest restart
                 surplus = min(max(len(ready) - (n_episode - st.episode_count), 0), len(ids))
@@ -287,6 +330,8 @@ class FastCollector(object):
                 break
         if stored is not None:
             env.device_step(r, ready[:0], obs[:0], stored, norm, fresh)
+            if traj is not None and jobs:
+                traj._copy_host(r, jobs, T or 0, env.D, env.A, env.device, stream)
         return st
 
     def _device_steps(self, r, n_episode: int, no_grad: bool, random: bool):

@@ -274,19 +274,37 @@ class TrajectoryBuffer:
     def _commit(self, r, rows: np.ndarray, stride: int, D: int, A: int, device, stream: int) -> None:
         """Offer harvested episodes in order; copy the ones still kept at the end straight from the ring."""
         from .. import _lib
-        pending = {}
-        for row in rows:
-            slot = self._index.offer(float(row["ret"]), float(row["cost"]), int(row["len"]))
-            if slot is not None:
-                pending[slot] = (int(row["env"]), int(row["start"]), int(row["len"]), slot)
-        live = set(self._index.slots)
-        jobs = [j for s, j in pending.items() if s in live]
+        jobs = self._offer_episodes((int(row["env"]), int(row["start"]), int(row["len"]), float(row["ret"]),
+                                     float(row["cost"])) for row in rows)
         if not jobs:
             return
         self._arena.reserve(self._index.n_slots, stride, D, A, device)
         jt = torch.tensor(jobs, dtype=torch.int32).to(device)
         a = self._arena.descriptor()
         _lib.check(_lib.lib.fsrl_traj_copy(ctypes.byref(r), ctypes.byref(a), jt.data_ptr(), len(jobs), stream))
+
+    def _offer_episodes(self, episodes) -> List[tuple]:
+        """Offer finished episodes (env, ring start, length, return, cost) in order; the copy jobs
+        (env, start, length, arena slot) of the ones still kept after the last offer."""
+        pending = {}
+        for env, start, length, ret, cost in episodes:
+            slot = self._index.offer(ret, cost, length)
+            if slot is not None:
+                pending[slot] = (env, start, length, slot)
+        live = set(self._index.slots)
+        return [j for s, j in pending.items() if s in live]
+
+    def _copy_host(self, r, jobs: List[tuple], stride: int, D: int, A: int, device, stream: int) -> None:
+        """Copy kept episodes from the ring of host-stepped envs (``fsrl_traj_copy_host``); the arena stride grows to
+        ``stride`` or the longest of them."""
+        from .. import _lib
+        if not jobs:
+            return
+        self._arena.reserve(self._index.n_slots, max([stride] + [j[2] for j in jobs]), D, A, device)
+        jt = torch.tensor(jobs, dtype=torch.int32).to(device)
+        a = self._arena.descriptor()
+        _lib.check(_lib.lib.fsrl_traj_copy_host(ctypes.byref(r), ctypes.byref(a), D, A, jt.data_ptr(), len(jobs),
+                                                stream))
 
     # ---- read-out ----------------------------------------------------------------------------------------------
     def _gather(self, jobs: np.ndarray, n: int, src: "_Arena") -> Dict[str, torch.Tensor]:

@@ -269,6 +269,12 @@ int fsrl_rollout_norm_steps(const fsrl_rollout_t* r, const fsrl_obs_rms_t* n, in
  *                    wrote exactly cap slots.  n_ready = 0 otherwise.
  *   fsrl_traj_copy   jobs[n][4] = (env, start slot, length, arena slot): copy episodes into the
  *                    arena; act is stored remapped, as the env received it (map_action)
+ *   fsrl_traj_copy_host  fsrl_traj_copy from the ring of host-stepped envs (r->kind = -1, whose widths the
+ *                    descriptor does not carry): D >= 1 and 1 <= A <= 8 are the ring's widths and must equal
+ *                    the arena's.  The host knows every finished episode (the collector's own loop), so
+ *                    there is no scan on this path; the caller copies an episode after the launch that
+ *                    stores its last transition and before its first slot is written again.  map_action
+ *                    takes r's action bounds (HostVectorEnv.fill).
  *   fsrl_traj_gather jobs[n][3] = (arena slot, length, first output row): pack into `out`, whose
  *                    arrays are contiguous rows (out->stride and out->n_slots are ignored) */
 typedef struct fsrl_traj_row {
@@ -297,6 +303,8 @@ int fsrl_traj_begin(const fsrl_rollout_t* r, const fsrl_traj_scan_t* h, void* st
 int fsrl_traj_scan(const fsrl_rollout_t* r, const fsrl_traj_scan_t* h, int n_ready, void* stream);
 int fsrl_traj_copy(const fsrl_rollout_t* r, const fsrl_traj_arena_t* a, const int* jobs, int n_jobs,
                    void* stream);
+int fsrl_traj_copy_host(const fsrl_rollout_t* r, const fsrl_traj_arena_t* a, int D, int A, const int* jobs,
+                        int n_jobs, void* stream);
 int fsrl_traj_gather(const fsrl_traj_arena_t* a, const fsrl_traj_arena_t* out, const long long* jobs,
                      int n_jobs, void* stream);
 
