@@ -8,7 +8,8 @@
 //
 // Work decomposition of one network (H = 256, minibatch = 256 rows = 4 row blocks of 64):
 //   CTA c = 8 a + b           a = row block (4), b = 32-wide column block (8)
-//   S   h1 tile   [64 r x 32 k]   FFMA (K = D)            -> images H1A (MN = r, K = k), H1T (MN = k, K = r)
+//   S   h1 tile   [64 r x 32 k]   FFMA (K = D) over observation rows staged one step ahead
+//                                                         -> images H1A (MN = r, K = k), H1T (MN = k, K = r)
 //   G1  h2 tile   [64 r x 32 o] = h1[r, :] W2t[:, o]      A = H1A block a, B = W2A block b      (wgmma)
 //       head partial over the tile's 32 columns -> 8 partials per row block -> loss gradient dOut
 //       dz2 tile = (dOut W3^T) * relu'(h2)                -> images DZA (MN = r, K = o), DZT (MN = o, K = r)
@@ -43,6 +44,7 @@
 #include "arena.cuh"
 #include "ppo_loss.cuh"
 #include "wgmma.cuh"
+#include <cuda_pipeline.h>
 #include <cstdlib>
 #include <cmath>
 #include <vector>
@@ -72,6 +74,10 @@ constexpr int DB2P_OFF = N_IMG * IMG;                           // [4 a][H]
 constexpr int DW3P_OFF = DB2P_OFF + 4 * H_;                     // [4 a][H][OUTP]
 constexpr int DB3P_OFF = DW3P_OFF + 4 * H_ * OUTP;              // [4 a][16]
 constexpr int MAXD = 40;
+// byte offset in the operand ring of the h1 tiles' observation rows, staged one step ahead (stage_rows)
+constexpr int XS_OFF = 2 * SLOT_BYTES;
+static_assert(XS_OFF >= 2 * 32 * 65 * 2 * 4 && XS_OFF >= 2 * (MAXD + 1) * 64 * 4 &&
+              XS_OFF + 128 * (MAXD + 1) * 4 <= NSLOT * SLOT_BYTES, "staged rows overlap the ring's scratch or dW1 partials");
 constexpr int NSMAX = (MAXD + 1) * 32 + 32 + 32 * OUTP + 16;    // floats of the largest small-parameter slice (SliceMap)
 constexpr int SLICE_OFF = DB3P_OFF + 4 * 16;                    // [8 b][NSMAX]: final gradient slices, written by the reducers
 constexpr int NET_WS = SLICE_OFF + 8 * NSMAX;
@@ -395,6 +401,24 @@ __device__ __forceinline__ void store_transposed(float* scr, const float (&hi)[N
     epi_bar();                                                 // scratch may be reused
 }
 
+// Observation rows of a G2 CTA's two h1 tiles (row blocks a and a + 2 of the minibatch whose first row is row0: 128 rows
+// of D floats) into xs, row i at i * (D | 1): the S phase reads one row per lane, and the odd stride puts the 32 rows
+// of a warp into 32 banks.  4-byte asynchronous copies (LDGSTS) hold no registers; the caller waits for them
+// (__pipeline_wait_prior) before the barrier that precedes their readers.
+//
+// Liveness of the landing area, ring bytes [XS_OFF, XS_OFF + 128 (D | 1) 4) (slot 2 on): the copies for step t + 1 are
+// issued after this CTA's G2 of step t has consumed every chunk (all bytes bound for this ring have landed), and peers
+// copy into the ring again only after flag A of step t + 1, which counts this CTA's arrival after its S phase has read
+// the rows.  Below XS_OFF the ring holds the dW1 / db1 partials until D2 ([wq][D + 1][64 k], at most 21 KB) and the
+// S-phase transposed staging (two [64 x 32] hi / lo tiles, 33 KB).
+__device__ __forceinline__ void stage_rows(float* xs, const float* obs, long long row0, int a, int D, int et) {
+    const int i = et >> 1;                                   // row i of the 128: two threads per row, alternate d
+    const float* src = obs + (row0 + 64 * a + i + (i & 64)) * D;
+    float* dst = xs + i * (D | 1);
+    for (int d = et & 1; d < D; d += 2) __pipeline_memcpy_async(dst + d, src + d, 4);
+    __pipeline_commit();
+}
+
 // sum over the 16 lanes of a half-warp (lanes l and l ^ 16 hold different data)
 __device__ __forceinline__ float half_sum(float v) {
 #pragma unroll
@@ -700,7 +724,9 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             return d;
         };
 
-        // ---- initial state: small slices from the arena, the W2 tile (p, m, v) into registers ----
+        // ---- initial state: small slices from the arena, the W2 tile (p, m, v) into registers; step 0's h1 rows ----
+        float* xs = reinterpret_cast<float*>(ring + XS_OFF);
+        if (is_g2) stage_rows(xs, u.obs, 0, a, D, et);
         for (int i = et; i < sm.n; i += NEPI) {
             long long src = -1;
             if (i < sm.b2) { const int d = i / 32, kk = i % 32; src = (d < D) ? o_w1 + (long long)d * H + 32 * b + kk : o_b1 + 32 * b + kk; }
@@ -723,6 +749,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
 #pragma unroll
             for (int j = 0; j < C2; ++j) w2p[j] = w2m[j] = w2v[j] = 0.f;
         }
+        __pipeline_wait_prior(0);
         epi_bar();
 
         for (int t = 0; t < P.n_mb; ++t) {
@@ -772,17 +799,17 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             }
             // ---- S(b): h1 tiles [64 rows][32 columns of block b].  The CTAs that own a W2 tile are busy with its Adam
             // step and images, so the other half of the grid (CTAs 0-15: a in {0, 1}) computes the tiles of row
-            // blocks a and a + 2 -- same column block, hence the same W1 slice.
+            // blocks a and a + 2 -- same column block, hence the same W1 slice.  Their observation rows are already in
+            // shared memory (stage_rows, issued while the previous step waited for D2).
             if (is_g2) {
                 const int r = et & 63, kc = C1 * (et >> 6);  // row, first of C1 columns
-                // both row blocks' observation rows are in flight before anything is stored
-                const float* x0 = u.obs + (row0 + 64 * a + r) * D;
-                const float* x1 = u.obs + (row0 + 64 * (a + 2) + r) * D;
+                const float* x0 = xs + r * (D | 1);
+                const float* x1 = xs + (64 + r) * (D | 1);
                 float acc2[2][C1];
 #pragma unroll
                 for (int j = 0; j < C1; ++j) acc2[0][j] = acc2[1][j] = sp_p[sm.w1 + D * 32 + kc + j];      // b1
                 for (int d = 0; d < D; ++d) {
-                    const float xv0 = __ldg(x0 + d), xv1 = __ldg(x1 + d);
+                    const float xv0 = x0[d], xv1 = x1[d];
                     const float* w = sp_p + sm.w1 + d * 32 + kc;
 #pragma unroll
                     for (int j = 0; j < C1; ++j) { acc2[0][j] = fmaf(xv0, w[j], acc2[0][j]); acc2[1][j] = fmaf(xv1, w[j], acc2[1][j]); }
@@ -1007,7 +1034,8 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
             // this lane's h1 entries (image H1A, complete since flag A) and this thread's share of the 64 x D
             // observation block of row block q4.  Neither stays in registers across the GEMM, whose accumulators need
             // them: the mask is kept as C2 bits, the block is staged in the hop-B landing zone, idle until the next step
-            // (row r at r * D + (r >> 5): the two half-warps read different banks).
+            // (row r at r * dp4 + 4 (r >> 5), dp4 = D rounded up to a multiple of 4: 16-byte aligned rows for the dW1
+            // loop's vector reads, and the two half-warps read different banks).
             unsigned mbits = 0;
             if (is_g2) {
                 const int k = 64 * ka + trow;
@@ -1026,7 +1054,7 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
 #pragma unroll
                 for (int q = 0; q < (64 * MAXD + NEPI - 1) / NEPI; ++q) {
                     const int e = et + q * NEPI;
-                    if (q < nx && e < 64 * D) { const int r = e / D; land[e + (r >> 5)] = xr[q]; }
+                    if (q < nx && e < 64 * D) { const int r = e / D; land[r * ((D + 3) & ~3) + 4 * (r >> 5) + (e - r * D)] = xr[q]; }
                 }
             }
             // reducers: warpgroup 1 would only wait for warpgroup 0's GEMM -- it sums the b2 / W3 / b3 / log sigma
@@ -1093,14 +1121,29 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 for (int jq = 0; jq < C2; ++jq) v[jq] = ((mbits >> jq) & 1u) ? v[jq] : 0.f;
                 epi_bar();
                 if (et == 0) STAMP(22);
-                const float* xh = land + (size_t)cb2 * D + half;
+                // 4 of the D independent sums at a time, so that their FMA chains interleave: each d keeps its own
+                // accumulator, fed in jq order from 0, and one 16-byte read gives the 4 d of row cb2 + jq.  The last
+                // batch may run past D into the row's padding; those sums are not stored.
+                const int dp4 = (D + 3) & ~3;
+                const float* xh = land + (size_t)cb2 * dp4 + 4 * half;
                 float* dst = reinterpret_cast<float*>(ring) + (size_t)wq * (D + 1) * 64 + trow;
-                for (int d = 0; d < D; ++d) {
-                    float sacc = 0.f;
+                for (int d0 = 0; d0 < D; d0 += 4) {
+                    float sacc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-                    for (int jq = 0; jq < C2; ++jq) sacc = fmaf(xh[jq * D + d], v[jq], sacc);
-                    sacc += __shfl_xor_sync(0xffffffffu, sacc, 16);
-                    if (half == 0) dst[d * 64] = sacc;
+                    for (int jq = 0; jq < C2; ++jq) {
+                        const float4 x = *reinterpret_cast<const float4*>(xh + jq * dp4 + d0);
+                        sacc[0] = fmaf(x.x, v[jq], sacc[0]);
+                        sacc[1] = fmaf(x.y, v[jq], sacc[1]);
+                        sacc[2] = fmaf(x.z, v[jq], sacc[2]);
+                        sacc[3] = fmaf(x.w, v[jq], sacc[3]);
+                    }
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) sacc[i] += __shfl_xor_sync(0xffffffffu, sacc[i], 16);
+                    if (half == 0) {
+#pragma unroll
+                        for (int i = 0; i < 4; ++i)
+                            if (d0 + i < D) dst[(d0 + i) * 64] = sacc[i];
+                    }
                 }
                 float sb1 = 0.f;
 #pragma unroll
@@ -1193,6 +1236,8 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                     flag_add_release(fl_d2);
                 }
             }
+            // the next step's h1 rows travel while the CTA waits for D2 and steps its parameters
+            if (is_g2 && t + 1 < P.n_mb) stage_rows(xs, u.obs, row0 + MB, a, D, et);
             if (et == 0) {
                 if (!flag_wait_ge(fl_d2, 24u * (unsigned)u.n_nets * (t + 1), WAIT_CYCLES)) fail(P.err, 34);
                 STAMP(10);
@@ -1226,8 +1271,11 @@ __global__ void __launch_bounds__(TPB, 1) ppo_persist_kernel(const Args P) {
                 acc_ld<C2>(accs, trow, cb2, g);            // data-parallel runs: the ranks' mean (dp_tile_*)
 #pragma unroll
                 for (int j = 0; j < C2; ++j) w2p[j] = adam_one(w2p[j], g[j] * gscale, w2m[j], w2v[j], ad);
+            } else {
+                __pipeline_wait_prior(0);                 // the next step's h1 rows (stage_rows) landed
+                if (et == 0) STAMP(18);
             }
-            epi_bar();     // slices final before the next h1 tile / head reads them; s_adam may be rewritten
+            epi_bar();     // slices and h1 rows final before the next h1 tile / head reads them; s_adam may be rewritten
             if (et == 0) STAMP(11);
         }
 

@@ -184,7 +184,7 @@ def main():
                  8: "[reducer] dW1 partials arrived", 9: "sumsq (+ slice) out", 10: "flag D2 passed",
                  11: "Adam done (step end)", 12: "[producer] flag A passed", 13: "[producer] G1 copies issued",
                  14: "[producer] flag C passed", 15: "[reducer wg1] flag C passed", 16: "[reducer wg1] b2/W3/b3 reduced",
-                 17: "[reducer] W1/b1 reduced (DSMEM)", 22: "G2: mask applied", 23: "G2: dW1 partial in smem",
+                 17: "[reducer] W1/b1 reduced (DSMEM)", 18: "[G2] next step's h1 rows landed", 22: "G2: mask applied", 23: "G2: dW1 partial in smem",
                  24: "norm known (+ slice read)", 25: "small slices stepped", 26: "head gathered, loss gradient",
                  27: "dz2 images stored", 28: "partial sums exchanged"}
         rel = dbg - dbg[:, :1]
