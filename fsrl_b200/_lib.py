@@ -212,6 +212,7 @@ SIGNATURES = {
     "fsrl_rollout_steps_act": (c_int, [ctypes.POINTER(Rollout), c_f32p, c_vp]),
     "fsrl_env_step": (c_int, [ctypes.POINTER(Rollout), c_f32p, c_vp, c_int, c_f32p, c_f32p, c_f32p, c_u8p, c_u8p, c_vp]),
     "fsrl_env_reset_ids": (c_int, [ctypes.POINTER(Rollout), c_vp, c_int, c_f32p, c_vp]),
+    "fsrl_env_render": (c_int, [ctypes.POINTER(Rollout), c_vp, c_int, c_int, c_int, c_f32p, c_u8p, c_vp]),
     "fsrl_host_pack_bytes": (c_size, [c_int, c_int, c_int]),
     "fsrl_host_collect_step": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(HostStep), c_vp]),
     "fsrl_host_pack_norm_bytes": (c_size, [c_int, c_int, c_int, c_int]),

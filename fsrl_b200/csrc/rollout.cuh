@@ -596,3 +596,38 @@ ROLLOUT_BP_KINDS(ROLLOUT_LAUNCHERS, extern)
 ROLLOUT_VEL_KINDS(ROLLOUT_LAUNCHERS, extern)
 
 }  // namespace fsrl
+
+// a C-ABI entry point reaches kind `kind` as the compile-time constant K in CALL (used after `using namespace fsrl`)
+#define DISPATCH_KIND(kind, CALL)                                                    \
+    switch (kind) {                                                                  \
+        case ENV_CAR_CIRCLE: { constexpr int K = ENV_CAR_CIRCLE; CALL; } break;      \
+        case ENV_CAR_RUN: { constexpr int K = ENV_CAR_RUN; CALL; } break;            \
+        case ENV_BALL_CIRCLE: { constexpr int K = ENV_BALL_CIRCLE; CALL; } break;    \
+        case ENV_BALL_RUN: { constexpr int K = ENV_BALL_RUN; CALL; } break;          \
+        case ENV_ANT_CIRCLE: { constexpr int K = ENV_ANT_CIRCLE; CALL; } break;      \
+        case ENV_POINT_GOAL: { constexpr int K = ENV_POINT_GOAL; CALL; } break;      \
+        case ENV_ANT_RUN: { constexpr int K = ENV_ANT_RUN; CALL; } break;            \
+        case ENV_DRONE_CIRCLE: { constexpr int K = ENV_DRONE_CIRCLE; CALL; } break;  \
+        case ENV_DRONE_RUN: { constexpr int K = ENV_DRONE_RUN; CALL; } break;        \
+        case ENV_POINT_CIRCLE1: { constexpr int K = ENV_POINT_CIRCLE1; CALL; } break;\
+        case ENV_POINT_CIRCLE2: { constexpr int K = ENV_POINT_CIRCLE2; CALL; } break;\
+        case ENV_CAR_CIRCLE1: { constexpr int K = ENV_CAR_CIRCLE1; CALL; } break;    \
+        case ENV_CAR_CIRCLE2: { constexpr int K = ENV_CAR_CIRCLE2; CALL; } break;    \
+        case ENV_POINT_GOAL2: { constexpr int K = ENV_POINT_GOAL2; CALL; } break;    \
+        case ENV_CAR_GOAL1: { constexpr int K = ENV_CAR_GOAL1; CALL; } break;        \
+        case ENV_CAR_GOAL2: { constexpr int K = ENV_CAR_GOAL2; CALL; } break;        \
+        case ENV_POINT_BUTTON1: { constexpr int K = ENV_POINT_BUTTON1; CALL; } break;\
+        case ENV_POINT_BUTTON2: { constexpr int K = ENV_POINT_BUTTON2; CALL; } break;\
+        case ENV_CAR_BUTTON1: { constexpr int K = ENV_CAR_BUTTON1; CALL; } break;    \
+        case ENV_CAR_BUTTON2: { constexpr int K = ENV_CAR_BUTTON2; CALL; } break;    \
+        case ENV_POINT_PUSH1: { constexpr int K = ENV_POINT_PUSH1; CALL; } break;    \
+        case ENV_POINT_PUSH2: { constexpr int K = ENV_POINT_PUSH2; CALL; } break;    \
+        case ENV_CAR_PUSH1: { constexpr int K = ENV_CAR_PUSH1; CALL; } break;        \
+        case ENV_CAR_PUSH2: { constexpr int K = ENV_CAR_PUSH2; CALL; } break;        \
+        case ENV_HALF_CHEETAH_VEL: { constexpr int K = ENV_HALF_CHEETAH_VEL; CALL; } break; \
+        case ENV_HOPPER_VEL: { constexpr int K = ENV_HOPPER_VEL; CALL; } break;      \
+        case ENV_SWIMMER_VEL: { constexpr int K = ENV_SWIMMER_VEL; CALL; } break;    \
+        case ENV_WALKER2D_VEL: { constexpr int K = ENV_WALKER2D_VEL; CALL; } break;  \
+        case ENV_ANT_VEL: { constexpr int K = ENV_ANT_VEL; CALL; } break;            \
+        default: set_error("unknown env kind %d", kind); return FSRL_EINVAL;         \
+    }

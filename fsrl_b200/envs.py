@@ -40,6 +40,9 @@ KINDS = {
     "SafetyAntVelocityGymnasium-v1": 37,
 }
 
+RENDER_MODES = (None, "rgb_array")
+RENDER_MIN, RENDER_MAX = 16, 1024     # frame height and width (fsrl_env_render)
+
 
 def env_dims(kind: int):
     D, A, S, T = (ctypes.c_int() for _ in range(4))
@@ -73,7 +76,14 @@ def make(task: str, **_) -> DeviceEnv:
 class DeviceVectorEnv:
     """E independent envs of one task, resident on one GPU."""
 
-    def __init__(self, task: str, env_num: int, device="cuda", seed: int = 0):
+    def __init__(self, task: str, env_num: int, device="cuda", seed: int = 0, render_mode: Optional[str] = None,
+                 render_size=(256, 256)):
+        if render_mode not in RENDER_MODES:
+            raise ValueError(f"render_mode must be one of {RENDER_MODES}, got {render_mode!r}")
+        height, width = (int(v) for v in render_size)
+        if not (RENDER_MIN <= height <= RENDER_MAX and RENDER_MIN <= width <= RENDER_MAX):
+            raise ValueError(f"render_size (height, width) = {(height, width)} outside [{RENDER_MIN}, {RENDER_MAX}]")
+        self.render_mode, self.render_size = render_mode, (height, width)
         proto = DeviceEnv(task)
         self.task, self.kind = task, proto.kind
         self.env_num = int(env_num)
@@ -98,6 +108,8 @@ class DeviceVectorEnv:
         self.stats = torch.zeros(ctypes.sizeof(_lib.CollectStats), dtype=torch.uint8, device=dev)
         self._stats_host = torch.zeros(ctypes.sizeof(_lib.CollectStats), dtype=torch.uint8).pin_memory() \
             if torch.cuda.is_available() else torch.zeros(ctypes.sizeof(_lib.CollectStats), dtype=torch.uint8)
+        # rgb_array only: each env's cost of its last step() (0 after a reset), drawn by render()
+        self.last_cost = torch.zeros(E, dtype=torch.float32, device=dev) if render_mode == "rgb_array" else None
 
     def __len__(self):
         return self.env_num
@@ -156,9 +168,13 @@ class DeviceVectorEnv:
             stream = self._stream()
             if ids is None:
                 _lib.check(_lib.lib.fsrl_env_reset_all(ctypes.byref(r), stream))
+                if self.last_cost is not None:
+                    self.last_cost.zero_()
                 return self.obs_cur, [{} for _ in range(self.env_num)]
             obs = torch.empty((len(ids), self.D), dtype=torch.float32, device=self.device)
             _lib.check(_lib.lib.fsrl_env_reset_ids(ctypes.byref(r), ids.ctypes.data, len(ids), obs.data_ptr(), stream))
+            if self.last_cost is not None:
+                self.last_cost[torch.from_numpy(ids.astype(np.int64)).to(self.device)] = 0.0
         return obs, [{} for _ in range(len(ids))]
 
     def read_stats(self) -> "_lib.CollectStats":
@@ -195,10 +211,28 @@ class DeviceVectorEnv:
                                               n, obs_next.data_ptr(), rew.data_ptr(), cost.data_ptr(),
                                               term.data_ptr(), trunc.data_ptr(), stream))
         env_id = np.arange(n) if ids is None else ids.astype(np.int64)
+        if self.last_cost is not None:
+            self.last_cost.index_copy_(0, torch.from_numpy(env_id).to(dev), cost)
         return obs_next, rew, term, trunc, Batch(cost=cost, env_id=env_id)
 
-    def render(self, **kwargs):
-        return None
+    def render(self, id=None, **kwargs):
+        """With ``render_mode="rgb_array"``: one RGB frame per env (all, or the ones ``id`` lists; an env may be listed
+        twice), a contiguous ``uint8`` CUDA tensor of shape ``(n, height, width, 3)``, drawn from the envs' state by
+        csrc/render.cu (views, primitives and palette: DESIGN §7).  Robots whose last step cost are drawn in the cost
+        colour.  Reads the env state only.  With ``render_mode=None``: ``None``."""
+        if self.render_mode is None:
+            return None
+        ids = self._ids(id)
+        n = self.env_num if ids is None else len(ids)
+        height, width = self.render_size
+        stream = self._stream()
+        with torch.cuda.device(self.device):
+            out = torch.empty((n, height, width, 3), dtype=torch.uint8, device=self.device)
+            r = _lib.Rollout()
+            self.fill(r)
+            _lib.check(_lib.lib.fsrl_env_render(ctypes.byref(r), None if ids is None else ids.ctypes.data, n, height,
+                                                width, self.last_cost.data_ptr(), out.data_ptr(), stream))
+        return out
 
     def close(self):
         pass

@@ -167,6 +167,19 @@ int fsrl_env_step(const fsrl_rollout_t* r, const float* act, const int32_t* ids,
                   float* rew, float* cost, uint8_t* term, uint8_t* trunc, void* stream);
 int fsrl_env_reset_ids(const fsrl_rollout_t* r, const int32_t* ids, int n, float* obs, void* stream);
 
+/* ---- frames of the device envs (DeviceVectorEnv.render with render_mode="rgb_array") ------------
+ * out[n][height][width][3] (u8 RGB, device) receives one top-down or side-view frame per row of ids
+ * (HOST int32 env ids in [0, E), duplicates allowed; NULL = every env in order, then n must be E).
+ * Row 0 is the top of the frame; pixel (i, j) samples the world point (x0 + (j + 0.5) sx,
+ * y1 - (i + 0.5) sy) of the task's view window and takes the colour of the last primitive of the
+ * env's scene that covers it (a fixed drawing order, one fixed palette, no antialiasing; DESIGN §7).
+ * last_cost (device, E floats, may be NULL): the robot of env e is drawn in the cost colour when
+ * last_cost[e] > 0.  Reads only env_state, env_t, ep_idx and seed_env of r, writes only out.
+ * Returns FSRL_EINVAL before touching the device on an unknown kind, n < 1, an id outside [0, E),
+ * height or width outside [16, 1024], or a null r, out or state pointer. */
+int fsrl_env_render(const fsrl_rollout_t* r, const int32_t* ids, int n, int height, int width,
+                    const float* last_cost, uint8_t* out, void* stream);
+
 /* ---- host-stepped envs: one vector step of FastCollector.collect around a host env.step ----------
  * The host steps its own envs (gymnasium / tianshou objects); the device keeps the actor, the noise
  * stream and the ring.  One call per vector step enqueues, on `stream`: one H2D copy of the packed
