@@ -186,6 +186,12 @@ class HostNorm(ctypes.Structure):
     _fields_ = [("obs_rms", c_vp), ("obs_norm", c_vp), ("n_fresh", c_int), ("pad", c_int)]
 
 
+class EnvPlugin(ctypes.Structure):
+    _fields_ = [("abi_version", c_int), ("D", c_int), ("A", c_int), ("S", c_int), ("T", c_int), ("pad", c_int),
+                ("reset_all", c_vp), ("steps", c_vp), ("act_step", c_vp), ("env_step", c_vp), ("reset_ids", c_vp),
+                ("norm_steps", c_vp)]
+
+
 ALGO_SAC, ALGO_DDPG = 0, 1
 OFF_STATS = 8
 CVPO_STATS = 16
@@ -213,6 +219,7 @@ SIGNATURES = {
     "fsrl_env_step": (c_int, [ctypes.POINTER(Rollout), c_f32p, c_vp, c_int, c_f32p, c_f32p, c_f32p, c_u8p, c_u8p, c_vp]),
     "fsrl_env_reset_ids": (c_int, [ctypes.POINTER(Rollout), c_vp, c_int, c_f32p, c_vp]),
     "fsrl_env_render": (c_int, [ctypes.POINTER(Rollout), c_vp, c_int, c_int, c_int, c_f32p, c_u8p, c_vp]),
+    "fsrl_env_register": (c_int, [ctypes.POINTER(EnvPlugin), ctypes.POINTER(c_int)]),
     "fsrl_host_pack_bytes": (c_size, [c_int, c_int, c_int]),
     "fsrl_host_collect_step": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(HostStep), c_vp]),
     "fsrl_host_pack_norm_bytes": (c_size, [c_int, c_int, c_int, c_int]),
@@ -294,7 +301,8 @@ def _check_abi_sizes():
     lib.fsrl_abi_sizeof.restype = c_size
     lib.fsrl_abi_sizeof.argtypes = [c_int]
     for which, cls in enumerate((Mlp3, CollectStats, Rollout, PpoUpdate, NetRef, NetList, Engine, EngInput,
-                                 OffPolicy, Cpo, Cvpo, TrajRow, TrajScan, TrajArena, HostStep, ObsRms, HostNorm)):
+                                 OffPolicy, Cpo, Cvpo, TrajRow, TrajScan, TrajArena, HostStep, ObsRms, HostNorm,
+                                 EnvPlugin)):
         want = lib.fsrl_abi_sizeof(which)
         if want != ctypes.sizeof(cls):
             raise ImportError(f"ABI mismatch: {cls.__name__} is {ctypes.sizeof(cls)} bytes in python, "

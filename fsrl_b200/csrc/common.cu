@@ -43,7 +43,7 @@ int launch_w2_mirror(const W2Mirror& mr, int n_nets, int H, cudaStream_t s) {
 }  // namespace fsrl
 
 extern "C" const char* fsrl_last_error(void) { return fsrl::g_err; }
-extern "C" int fsrl_abi_version(void) { return 2; }
+extern "C" int fsrl_abi_version(void) { return FSRL_ABI_VERSION; }
 namespace fsrl { unsigned long long g_launches = 0; }
 extern "C" unsigned long long fsrl_launch_count(void) { return fsrl::g_launches; }
 extern "C" int fsrl_sm_count(void) { return fsrl::sm_count(); }
@@ -68,6 +68,7 @@ extern "C" size_t fsrl_abi_sizeof(int which) {
         case 14: return sizeof(fsrl_host_step_t);
         case 15: return sizeof(fsrl_obs_rms_t);
         case 16: return sizeof(fsrl_host_norm_t);
+        case 17: return sizeof(fsrl_env_plugin_t);
         default: return 0;
     }
 }

@@ -1,0 +1,56 @@
+// A user-defined device env as a plugin of libfsrl_b200.so (fsrl_b200.envs.build_device_env, `make plugin`).
+// Compiled once per env with `-include <header>`; the header includes "envs.cuh" and defines, at global scope,
+// `UserEnv`: a struct with the contract of envs.cuh's built-in envs (static constexpr int D, A, S, T and the
+// __device__ functions reset / observe / step), or an alias of one of them.  UserEnv becomes Env<ENV_USER>, and
+// the six launchers of ROLLOUT_LAUNCHERS are instantiated for it from the same templates as a built-in kind:
+// with the library's flags, a plugin of a built-in struct compiles to the same kernels as the library's.
+// fsrl_env_plugin() returns the table fsrl_env_register takes; the kind id is assigned there.
+#include "rollout.cuh"
+
+namespace fsrl {
+
+// the template argument of this plugin's instantiations, outside the built-in kinds (the plugin's symbols are
+// hidden, so plugins loaded side by side never share an instantiation)
+constexpr int ENV_USER = FSRL_ENV_PLUGIN_FIRST;
+
+// the limits every learner imposes (fsrl_env_register checks them again); build_device_env reports the text
+static_assert(::UserEnv::D >= 1, "env plugin limit: D >= 1");
+static_assert(::UserEnv::A >= 1 && ::UserEnv::A <= ENV_MAX_A, "env plugin limit: 1 <= A <= ENV_MAX_A (8)");
+static_assert(::UserEnv::D + ::UserEnv::A <= FSRL_ENG_DX_LD, "env plugin limit: D + A <= FSRL_ENG_DX_LD (80)");
+static_assert(::UserEnv::S >= 1 && ::UserEnv::S <= ENV_MAX_S, "env plugin limit: 1 <= S <= ENV_MAX_S (32)");
+static_assert(::UserEnv::T >= 1, "env plugin limit: T >= 1");
+
+template <>
+struct Env<ENV_USER> : ::UserEnv {};
+
+ROLLOUT_LAUNCHERS(, ENV_USER)
+
+static int reset_all(const fsrl_rollout_t* r, void* s) {
+    return launch_env_reset_all<ENV_USER>(*r, static_cast<cudaStream_t>(s));
+}
+static int steps(const fsrl_rollout_t* r, int n_steps, int one_launch, void* s) {
+    return launch_steps_h<ENV_USER>(*r, n_steps, one_launch != 0, static_cast<cudaStream_t>(s));
+}
+static int act_step(const fsrl_rollout_t* r, const float* act, void* s) {
+    return launch_act_step<ENV_USER>(*r, act, static_cast<cudaStream_t>(s));
+}
+static int env_step(const fsrl_rollout_t* r, const float* act, const int32_t* ids, int n, float* obs_next, float* rew,
+                    float* cost, uint8_t* term, uint8_t* trunc, void* s) {
+    return launch_env_step<ENV_USER>(*r, act, ids, n, obs_next, rew, cost, term, trunc, static_cast<cudaStream_t>(s));
+}
+static int reset_ids(const fsrl_rollout_t* r, const int32_t* ids, int n, float* obs, void* s) {
+    return launch_env_reset_ids<ENV_USER>(*r, ids, n, obs, static_cast<cudaStream_t>(s));
+}
+static int norm_steps(const fsrl_rollout_t* r, const fsrl_obs_rms_t* n, int n_steps, const float* act, void* s) {
+    return launch_norm_steps<ENV_USER>(*r, *n, n_steps, act, static_cast<cudaStream_t>(s));
+}
+
+}  // namespace fsrl
+
+extern "C" __attribute__((visibility("default"))) const fsrl_env_plugin_t* fsrl_env_plugin(void) {
+    using E_ = fsrl::Env<fsrl::ENV_USER>;
+    static const fsrl_env_plugin_t table = {FSRL_ABI_VERSION, E_::D, E_::A, E_::S, E_::T, 0,
+                                            fsrl::reset_all, fsrl::steps, fsrl::act_step,
+                                            fsrl::env_step, fsrl::reset_ids, fsrl::norm_steps};
+    return &table;
+}

@@ -144,6 +144,9 @@ __host__ __device__ inline EnvDims env_dims(int kind) {
 
 __host__ __device__ inline bool env_kind_known(int kind) { return env_dims(kind).D != 0; }
 
+// host: the widths of a built-in kind or of a registered plugin kind (rollout.cu); false for an unknown kind
+bool env_kind_dims(int kind, EnvDims& d);
+
 // ---------------------------------------------------------------------------------------------
 // Car (unicycle with first-order actuator lag).  state: x, y, c, s, v, w [, x0 (run)]
 // ---------------------------------------------------------------------------------------------

@@ -363,6 +363,8 @@ using namespace fsrl;
 extern "C" int fsrl_env_render(const fsrl_rollout_t* r, const int32_t* ids, int n, int height, int width,
                                const float* last_cost, uint8_t* out, void* stream) {
     FSRL_REQUIRE(r != nullptr, "fsrl_env_render: null descriptor");
+    FSRL_REQUIRE(!env_plugin(r->kind), "fsrl_env_render: env kind %d is a user-defined env, which has no renderer",
+                 r->kind);
     FSRL_REQUIRE(env_kind_known(r->kind), "fsrl_env_render: unknown env kind %d", r->kind);
     FSRL_REQUIRE(r->E > 0, "fsrl_env_render: E must be positive");
     FSRL_REQUIRE(n >= 1, "fsrl_env_render: n = %d must be at least 1", n);

@@ -13,7 +13,30 @@
 // everywhere, for A/B runs and the tests).
 #include "rollout.cuh"
 
+#include <atomic>
+#include <mutex>
+
 namespace fsrl {
+
+// Registered plugin kinds: slot k holds kind FSRL_ENV_PLUGIN_FIRST + k.  Slots are filled in order under the
+// mutex and never change afterwards; the count is published after its slot is written, so lookups take no lock.
+static fsrl_env_plugin_t g_plugins[FSRL_ENV_PLUGIN_END - FSRL_ENV_PLUGIN_FIRST];
+static std::atomic<int> g_n_plugins{0};
+static std::mutex g_register_mu;
+
+const fsrl_env_plugin_t* env_plugin(int kind) {
+    const int k = kind - FSRL_ENV_PLUGIN_FIRST;
+    return (k >= 0 && k < g_n_plugins.load(std::memory_order_acquire)) ? &g_plugins[k] : nullptr;
+}
+
+bool env_kind_dims(int kind, EnvDims& d) {
+    if (const fsrl_env_plugin_t* p = env_plugin(kind)) {
+        d = {p->D, p->A, p->S, p->T};
+        return true;
+    }
+    d = env_dims(kind);
+    return d.D != 0;
+}
 
 // begin a collect: ready envs = first min(E, n_episode) (:235-236), zero the per-collect stats
 __global__ void collect_begin_kernel(const fsrl_rollout_t a, int n_episode) {
@@ -32,10 +55,19 @@ __global__ void collect_begin_kernel(const fsrl_rollout_t a, int n_episode) {
 
 using namespace fsrl;
 
+// rc = kind's launcher: PCALL through the table p of a registered plugin kind, else CALL on the built-in kind K
+#define DISPATCH_ENV(kind, PCALL, CALL)                          \
+    if (const fsrl_env_plugin_t* p = env_plugin(kind)) {         \
+        rc = PCALL;                                              \
+    } else {                                                     \
+        DISPATCH_KIND(kind, rc = CALL);                          \
+    }
+
 // the env half of the descriptor (what every entry point touches)
 static int check_env_state(const fsrl_rollout_t* a) {
     FSRL_REQUIRE(a != nullptr, "rollout: null descriptor");
-    FSRL_REQUIRE(env_kind_known(a->kind), "rollout: unknown env kind %d", a->kind);
+    EnvDims d;
+    FSRL_REQUIRE(env_kind_dims(a->kind, d), "rollout: unknown env kind %d", a->kind);
     FSRL_REQUIRE(a->E > 0, "rollout: E must be positive");
     FSRL_REQUIRE(a->env_state && a->obs_cur && a->env_t && a->ep_idx && a->act_ctr && a->active &&
                  a->ep_rew && a->ep_len && a->done_now && a->stats, "rollout: null state pointer");
@@ -45,7 +77,8 @@ static int check_env_state(const fsrl_rollout_t* a) {
 static int check_rollout(const fsrl_rollout_t* a) {
     int rc = check_env_state(a);
     if (rc) return rc;
-    const EnvDims d = env_dims(a->kind);
+    EnvDims d;
+    env_kind_dims(a->kind, d);
     FSRL_REQUIRE(a->actor.in == d.D || a->mode == FSRL_MODE_RANDOM, "rollout: actor input dim %d != obs dim %d", a->actor.in, d.D);
     return FSRL_OK;
 }
@@ -61,8 +94,8 @@ static int check_ids(const char* fn, const fsrl_rollout_t* a, const int32_t* ids
 }
 
 extern "C" int fsrl_env_dims(int kind, int* D, int* A, int* S, int* T) {
-    FSRL_REQUIRE(env_kind_known(kind), "fsrl_env_dims: unknown env kind %d", kind);
-    const EnvDims d = env_dims(kind);
+    EnvDims d;
+    FSRL_REQUIRE(env_kind_dims(kind, d), "fsrl_env_dims: unknown env kind %d", kind);
     if (D) *D = d.D; if (A) *A = d.A; if (S) *S = d.S; if (T) *T = d.T;
     return FSRL_OK;
 }
@@ -71,7 +104,7 @@ extern "C" int fsrl_env_reset_all(const fsrl_rollout_t* a, void* stream) {
     int rc = check_rollout(a);
     if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_KIND(a->kind, rc = launch_env_reset_all<K>(*a, s));
+    DISPATCH_ENV(a->kind, p->reset_all(a, s), launch_env_reset_all<K>(*a, s));
     return rc;
 }
 
@@ -97,7 +130,7 @@ extern "C" int fsrl_rollout_steps(const fsrl_rollout_t* a, int n_steps, void* st
     // inline bookkeeping: no env's step depends on another env's, so all steps run in one launch
     const char* per_step = getenv("FSRL_ROLLOUT_PER_STEP");
     const bool one_launch = a->inline_done && !(per_step && atoi(per_step) != 0);
-    DISPATCH_KIND(a->kind, rc = launch_steps_h<K>(*a, n_steps, one_launch, s));
+    DISPATCH_ENV(a->kind, p->steps(a, n_steps, one_launch, s), launch_steps_h<K>(*a, n_steps, one_launch, s));
     return rc;
 }
 
@@ -106,7 +139,7 @@ extern "C" int fsrl_rollout_steps_act(const fsrl_rollout_t* a, const float* act,
     if (rc) return rc;
     FSRL_REQUIRE(act != nullptr, "fsrl_rollout_steps_act: null action array");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_KIND(a->kind, rc = launch_act_step<K>(*a, act, s));
+    DISPATCH_ENV(a->kind, p->act_step(a, act, s), launch_act_step<K>(*a, act, s));
     return rc;
 }
 
@@ -114,7 +147,9 @@ extern "C" int fsrl_rollout_norm_steps(const fsrl_rollout_t* a, const fsrl_obs_r
                                        void* stream) {
     int rc = act ? check_env_state(a) : check_rollout(a);
     if (rc) return rc;
-    rc = check_obs_rms("fsrl_rollout_norm_steps", n, a->E, env_dims(a->kind).D);
+    EnvDims d;
+    env_kind_dims(a->kind, d);
+    rc = check_obs_rms("fsrl_rollout_norm_steps", n, a->E, d.D);
     if (rc) return rc;
     FSRL_REQUIRE(n_steps >= 0, "fsrl_rollout_norm_steps: n_steps < 0");
     FSRL_REQUIRE(!act || n_steps == 1, "fsrl_rollout_norm_steps: caller actions cover one step (n_steps = %d)", n_steps);
@@ -125,7 +160,7 @@ extern "C" int fsrl_rollout_norm_steps(const fsrl_rollout_t* a, const fsrl_obs_r
     }
     if (n_steps == 0) return FSRL_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_KIND(a->kind, rc = launch_norm_steps<K>(*a, *n, n_steps, act, s));
+    DISPATCH_ENV(a->kind, p->norm_steps(a, n, n_steps, act, s), launch_norm_steps<K>(*a, *n, n_steps, act, s));
     return rc;
 }
 
@@ -137,7 +172,8 @@ extern "C" int fsrl_env_step(const fsrl_rollout_t* a, const float* act, const in
     if (rc) return rc;
     FSRL_REQUIRE(act && obs_next && rew && cost && term && trunc, "fsrl_env_step: null action or output array");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_KIND(a->kind, rc = launch_env_step<K>(*a, act, ids, n, obs_next, rew, cost, term, trunc, s));
+    DISPATCH_ENV(a->kind, p->env_step(a, act, ids, n, obs_next, rew, cost, term, trunc, s),
+                 launch_env_step<K>(*a, act, ids, n, obs_next, rew, cost, term, trunc, s));
     return rc;
 }
 
@@ -147,6 +183,27 @@ extern "C" int fsrl_env_reset_ids(const fsrl_rollout_t* a, const int32_t* ids, i
     rc = check_ids("fsrl_env_reset_ids", a, ids, n);
     if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_KIND(a->kind, rc = launch_env_reset_ids<K>(*a, ids, n, obs, s));
+    DISPATCH_ENV(a->kind, p->reset_ids(a, ids, n, obs, s), launch_env_reset_ids<K>(*a, ids, n, obs, s));
     return rc;
+}
+
+extern "C" int fsrl_env_register(const fsrl_env_plugin_t* p, int* kind) {
+    FSRL_REQUIRE(p != nullptr && kind != nullptr, "fsrl_env_register: null table or kind");
+    FSRL_REQUIRE(p->abi_version == fsrl_abi_version(),
+                 "fsrl_env_register: the plugin was built for ABI version %d, this library has version %d",
+                 p->abi_version, fsrl_abi_version());
+    FSRL_REQUIRE(p->D >= 1 && p->A >= 1 && p->A <= ENV_MAX_A && p->D + p->A <= FSRL_ENG_DX_LD && p->S >= 1 &&
+                 p->S <= ENV_MAX_S && p->T >= 1,
+                 "fsrl_env_register: D = %d, A = %d, S = %d, T = %d outside 1 <= A <= %d, D + A <= %d, "
+                 "1 <= S <= %d, T >= 1", p->D, p->A, p->S, p->T, ENV_MAX_A, FSRL_ENG_DX_LD, ENV_MAX_S);
+    FSRL_REQUIRE(p->reset_all && p->steps && p->act_step && p->env_step && p->reset_ids && p->norm_steps,
+                 "fsrl_env_register: null launcher in the table");
+    std::lock_guard<std::mutex> lock(g_register_mu);
+    const int n = g_n_plugins.load(std::memory_order_relaxed);
+    FSRL_REQUIRE(n < FSRL_ENV_PLUGIN_END - FSRL_ENV_PLUGIN_FIRST, "fsrl_env_register: all %d plugin kinds are taken",
+                 FSRL_ENV_PLUGIN_END - FSRL_ENV_PLUGIN_FIRST);
+    g_plugins[n] = *p;
+    g_n_plugins.store(n + 1, std::memory_order_release);
+    *kind = FSRL_ENV_PLUGIN_FIRST + n;
+    return FSRL_OK;
 }

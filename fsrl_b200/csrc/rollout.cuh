@@ -595,6 +595,9 @@ int launch_norm_steps(const fsrl_rollout_t& a, const fsrl_obs_rms_t& n, int n_st
 ROLLOUT_BP_KINDS(ROLLOUT_LAUNCHERS, extern)
 ROLLOUT_VEL_KINDS(ROLLOUT_LAUNCHERS, extern)
 
+// host: the launcher table of a registered plugin kind (fsrl_env_register, rollout.cu), NULL for any other kind
+const fsrl_env_plugin_t* env_plugin(int kind);
+
 }  // namespace fsrl
 
 // a C-ABI entry point reaches kind `kind` as the compile-time constant K in CALL (used after `using namespace fsrl`)

@@ -133,8 +133,10 @@ static int check_ring(const fsrl_rollout_t* r, bool host = false) {
     FSRL_REQUIRE(r != nullptr, "trajectory harvest: null rollout descriptor");
     if (host)
         FSRL_REQUIRE(r->kind == -1, "trajectory copy: a host ring has env kind -1, got %d", r->kind);
-    else
-        FSRL_REQUIRE(env_kind_known(r->kind), "trajectory harvest: unknown env kind %d", r->kind);
+    else {
+        EnvDims d;
+        FSRL_REQUIRE(env_kind_dims(r->kind, d), "trajectory harvest: unknown env kind %d", r->kind);
+    }
     FSRL_REQUIRE(r->E > 0 && r->cap > 0, "trajectory harvest: E and cap must be positive");
     FSRL_REQUIRE(r->b_obs && r->b_obs_next && r->b_act && r->b_rew && r->b_cost && r->b_term && r->b_trunc &&
                  r->b_ptr, "trajectory harvest: the rollout has no transition ring");
@@ -190,7 +192,8 @@ extern "C" int fsrl_traj_copy(const fsrl_rollout_t* r, const fsrl_traj_arena_t* 
                               void* stream) {
     int rc = check_ring(r);
     if (rc || (rc = check_arena(a))) return rc;
-    const EnvDims d = env_dims(r->kind);
+    EnvDims d;
+    env_kind_dims(r->kind, d);
     return launch_copy(r, a, d.D, d.A, jobs, n_jobs, stream);
 }
 

@@ -6,13 +6,20 @@ The dynamics are the analytic models of csrc/envs.cuh (bullet_safety_gym / safet
 are absent and irreproducible; SURVEY.md F5).  All state lives in HBM as SoA tensors; the
 fused rollout kernel (csrc/rollout.cu) steps every env without host involvement.  ``step`` /
 ``reset(id)`` give the gym protocol on the same state, for loops that bring their own actions.
-Envs the device cannot run (gymnasium simulators, a user's own env) go behind :class:`HostVectorEnv`
-(host_envs.py).
+A user's own env struct runs on the same path once built into a plugin (:func:`build_device_env`) and
+registered under a task name (:func:`register_device_env`; DESIGN §7).  Envs the device cannot run
+(gymnasium simulators) go behind :class:`HostVectorEnv` (host_envs.py).
 """
 from __future__ import annotations
 
 import ctypes
-from typing import Optional
+import hashlib
+import os
+import re
+import subprocess
+import sys
+import tempfile
+from typing import NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -40,8 +47,28 @@ KINDS = {
     "SafetyAntVelocityGymnasium-v1": 37,
 }
 
+PLUGIN_KIND_FIRST, PLUGIN_KIND_END = 64, 128   # FSRL_ENV_PLUGIN_FIRST / _END: the kinds of registered plugins
+
+
+class _Plugin(NamedTuple):
+    kind: int
+    path: str
+    so: ctypes.CDLL       # kept loaded: the library calls its launchers
+
+
+PLUGINS = {}   # task -> _Plugin, filled by register_device_env
+
 RENDER_MODES = (None, "rgb_array")
 RENDER_MIN, RENDER_MAX = 16, 1024     # frame height and width (fsrl_env_render)
+
+
+def task_kind(task: str) -> int:
+    """The env kind of a built-in or registered task."""
+    if task in KINDS:
+        return KINDS[task]
+    if task in PLUGINS:
+        return PLUGINS[task].kind
+    raise KeyError(f"unknown task {task!r}; available: {sorted(KINDS) + sorted(PLUGINS)}")
 
 
 def env_dims(kind: int):
@@ -55,10 +82,8 @@ class DeviceEnv:
     happens only inside a :class:`DeviceVectorEnv`)."""
 
     def __init__(self, task: str):
-        if task not in KINDS:
-            raise KeyError(f"unknown task {task!r}; available: {sorted(KINDS)}")
         self.task = task
-        self.kind = KINDS[task]
+        self.kind = task_kind(task)
         D, A, S, T = env_dims(self.kind)
         self.observation_space = Box(-np.inf, np.inf, (D,), np.float32)
         self.action_space = Box(-1.0, 1.0, (A,), np.float32)
@@ -85,6 +110,8 @@ class DeviceVectorEnv:
             raise ValueError(f"render_size (height, width) = {(height, width)} outside [{RENDER_MIN}, {RENDER_MAX}]")
         self.render_mode, self.render_size = render_mode, (height, width)
         proto = DeviceEnv(task)
+        if render_mode is not None and task in PLUGINS:
+            raise ValueError(f"{task!r} is a user-defined device env: it has no renderer, so render_mode must be None")
         self.task, self.kind = task, proto.kind
         self.env_num = int(env_num)
         self.device = torch.device(device)
@@ -238,4 +265,130 @@ class DeviceVectorEnv:
         pass
 
 
+# ---- user-defined device envs ------------------------------------------------------------------------------
+_CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
+_INCLUDE = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include")
+
+
+class EnvBuildError(RuntimeError):
+    """nvcc rejected a user env header; the message is the compiler's."""
+
+
+def default_plugin_dir() -> str:
+    """Where :func:`build_device_env` caches plugins by default: ``$FSRL_B200_CACHE/env_plugins``, else
+    ``~/.cache/fsrl_b200/env_plugins``."""
+    root = os.environ.get("FSRL_B200_CACHE") or os.path.join(os.path.expanduser("~"), ".cache", "fsrl_b200")
+    return os.path.join(root, "env_plugins")
+
+
+def _make(*args: str) -> subprocess.CompletedProcess:
+    return subprocess.run(["make", "-s", "-C", _CSRC, *args], stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
+                          text=True)
+
+
+def plugin_path(header: str, out: Optional[str] = None) -> str:
+    """The path :func:`build_device_env` gives the plugin of ``header``: ``<stem>-<key>.so`` in ``out``.  The key
+    hashes the header's bytes, the library's ABI version, the compiler and flags (csrc/flags.mk) and the library
+    sources the plugin is compiled from, so any change to one of them names a new artefact."""
+    flags = _make("print-flags")
+    if flags.returncode:
+        raise EnvBuildError(flags.stdout)
+    h = hashlib.sha256()
+    parts = [open(header, "rb").read(), str(_lib.lib.fsrl_abi_version()).encode(), flags.stdout.strip().encode()]
+    for name in sorted(os.listdir(_CSRC)):
+        if name.endswith(".cuh") or name == "env_plugin.cu":
+            parts += [name.encode(), open(os.path.join(_CSRC, name), "rb").read()]
+    parts.append(open(os.path.join(_INCLUDE, "fsrl_b200.h"), "rb").read())
+    for part in parts:
+        h.update(len(part).to_bytes(8, "little"))
+        h.update(part)
+    stem = os.path.splitext(os.path.basename(header))[0]
+    return os.path.join(os.path.abspath(out or default_plugin_dir()), f"{stem}-{h.hexdigest()[:20]}.so")
+
+
+def build_device_env(header: str, out: Optional[str] = None) -> str:
+    """Compile the env struct ``UserEnv`` that ``header`` defines into a plugin of the library (csrc/env_plugin.cu,
+    with the library's compiler and flags) and return the plugin's path, under ``out`` (default:
+    :func:`default_plugin_dir`).  A plugin already built from the same header, ABI, flags and sources is returned
+    as it is, without compiling.  Raises ``ValueError`` naming the limit when ``UserEnv`` breaks one of
+    1 <= A <= 8, D + A <= 80, 1 <= S <= 32, D >= 1, T >= 1, and :class:`EnvBuildError` with nvcc's message on any
+    other compile error."""
+    header = os.path.abspath(header)
+    if not os.path.isfile(header):
+        raise FileNotFoundError(header)
+    path = plugin_path(header, out)
+    if os.path.exists(path):
+        return path
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    fd, tmp = tempfile.mkstemp(suffix=".so", prefix=".build-", dir=os.path.dirname(path))
+    os.close(fd)
+    try:
+        res = _make("plugin", f"PLUGIN_HEADER={header}", f"PLUGIN_OUT={tmp}")
+        if res.returncode:
+            limits = re.findall(r"env plugin limit: ([^\"\n]+)", res.stdout)
+            if limits:
+                raise ValueError(f"{header}: UserEnv breaks the limit {limits[0]}")
+            raise EnvBuildError(f"building the env plugin of {header} failed:\n{res.stdout}")
+        os.replace(tmp + ".ptxas.log", path + ".ptxas.log")
+        os.replace(tmp, path)          # atomic: a concurrent build of the same key finds a complete file
+    finally:
+        for f in (tmp, tmp + ".ptxas.log", tmp + ".o"):
+            if os.path.exists(f):
+                os.remove(f)
+    return path
+
+
+def _load_plugin(plugin: str):
+    so = ctypes.CDLL(os.path.abspath(plugin))
+    so.fsrl_env_plugin.restype = ctypes.POINTER(_lib.EnvPlugin)
+    so.fsrl_env_plugin.argtypes = []
+    return so, so.fsrl_env_plugin()
+
+
+def plugin_dims(plugin: str):
+    """(D, A, S, T) of the env a plugin was built from (loads it; needs no GPU)."""
+    _, t = _load_plugin(plugin)
+    return t.contents.D, t.contents.A, t.contents.S, t.contents.T
+
+
+def register_device_env(task: str, plugin: str) -> int:
+    """Register the plugin ``plugin`` (a path from :func:`build_device_env`) under the task name ``task`` and return
+    its env kind.  Afterwards ``task`` works wherever a built-in device task does (``DeviceVectorEnv``, ``make``,
+    ``gym.make`` under ``compat.install()``, every collector, wrapper and agent), except rendering.  A built-in
+    task name is refused, and so is a name already registered from another plugin; registering the same plugin
+    under the same name again returns its kind."""
+    if task in KINDS:
+        raise ValueError(f"{task!r} is a built-in task; register the plugin under another name")
+    path = os.path.realpath(plugin)
+    if task in PLUGINS:
+        if PLUGINS[task].path == path:
+            return PLUGINS[task].kind
+        raise ValueError(f"{task!r} is already registered from {PLUGINS[task].path}")
+    so, table = _load_plugin(path)
+    kind = ctypes.c_int()
+    _lib.check(_lib.lib.fsrl_env_register(table, ctypes.byref(kind)))
+    PLUGINS[task] = _Plugin(kind.value, path, so)
+    return kind.value
+
+
+def _main(argv=None) -> int:
+    import argparse
+    ap = argparse.ArgumentParser(prog="python -m fsrl_b200.envs", description="user-defined device envs")
+    sub = ap.add_subparsers(dest="cmd", required=True)
+    b = sub.add_parser("build", help="compile a header defining UserEnv into an env plugin; prints its path")
+    b.add_argument("header")
+    b.add_argument("--out", default=None, help=f"plugin directory (default: {default_plugin_dir()})")
+    args = ap.parse_args(argv)
+    try:
+        print(build_device_env(args.header, args.out))
+    except (ValueError, EnvBuildError, FileNotFoundError) as e:
+        print(e, file=sys.stderr)
+        return 1
+    return 0
+
+
 from .obs_norm import ObsRunningMeanStd, VectorEnvNormObs  # noqa: E402,F401  (obs_norm imports DeviceVectorEnv)
+
+
+if __name__ == "__main__":
+    sys.exit(_main())

@@ -31,6 +31,7 @@ extern "C" {
 
 /* ---- plumbing ------------------------------------------------------------------- */
 const char* fsrl_last_error(void);
+#define FSRL_ABI_VERSION 2 /* what fsrl_abi_version() returns; compiled into env plugins */
 int fsrl_abi_version(void);
 size_t fsrl_abi_sizeof(int which); /* sizeof() of the descriptor structs, for binding self-checks */
 int fsrl_sm_count(void);
@@ -175,7 +176,7 @@ int fsrl_env_reset_ids(const fsrl_rollout_t* r, const int32_t* ids, int n, float
  * env's scene that covers it (a fixed drawing order, one fixed palette, no antialiasing; DESIGN §7).
  * last_cost (device, E floats, may be NULL): the robot of env e is drawn in the cost colour when
  * last_cost[e] > 0.  Reads only env_state, env_t, ep_idx and seed_env of r, writes only out.
- * Returns FSRL_EINVAL before touching the device on an unknown kind, n < 1, an id outside [0, E),
+ * Returns FSRL_EINVAL before touching the device on an unknown or a plugin kind (fsrl_env_register), n < 1, an id outside [0, E),
  * height or width outside [16, 1024], or a null r, out or state pointer. */
 int fsrl_env_render(const fsrl_rollout_t* r, const int32_t* ids, int n, int height, int width,
                     const float* last_cost, uint8_t* out, void* stream);
@@ -266,6 +267,31 @@ int fsrl_obs_rms_rows(const fsrl_obs_rms_t* n, float* x, int E, const int32_t* i
                       float* out, void* stream);
 int fsrl_rollout_norm_steps(const fsrl_rollout_t* r, const fsrl_obs_rms_t* n, int n_steps, const float* act,
                             void* stream);
+
+/* ---- user-defined device envs (plugins) --------------------------------------------------------------
+ * A plugin (csrc/env_plugin.cu compiled against a user's env struct, linked against this library) hands
+ * over the six launchers every env-dependent entry point reaches a kind through, instantiated for its
+ * struct by the same templates the built-in kinds use, and the struct's widths and horizon.
+ * fsrl_env_register copies the table and returns in *kind the next free id of
+ * [FSRL_ENV_PLUGIN_FIRST, FSRL_ENV_PLUGIN_END); from then on fsrl_env_dims, the rollout, gym-protocol,
+ * observation-normalizing and trajectory entry points accept that kind like a built-in one.
+ * fsrl_env_render refuses it.  Returns FSRL_EINVAL, registering nothing, when abi_version differs from
+ * fsrl_abi_version(), a width is outside the limits below, a launcher is NULL or the range is full.
+ * Limits: 1 <= D, 1 <= A <= 8, D + A <= FSRL_ENG_DX_LD, 1 <= S <= 32, T >= 1. */
+#define FSRL_ENV_PLUGIN_FIRST 64
+#define FSRL_ENV_PLUGIN_END 128
+typedef struct fsrl_env_plugin {
+    int abi_version;
+    int D, A, S, T, pad;
+    int (*reset_all)(const fsrl_rollout_t* r, void* stream);
+    int (*steps)(const fsrl_rollout_t* r, int n_steps, int one_launch, void* stream);
+    int (*act_step)(const fsrl_rollout_t* r, const float* act, void* stream);
+    int (*env_step)(const fsrl_rollout_t* r, const float* act, const int32_t* ids, int n, float* obs_next,
+                    float* rew, float* cost, uint8_t* term, uint8_t* trunc, void* stream);
+    int (*reset_ids)(const fsrl_rollout_t* r, const int32_t* ids, int n, float* obs, void* stream);
+    int (*norm_steps)(const fsrl_rollout_t* r, const fsrl_obs_rms_t* n, int n_steps, const float* act, void* stream);
+} fsrl_env_plugin_t;
+int fsrl_env_register(const fsrl_env_plugin_t* p, int* kind);
 
 /* ---- offline datasets: finished episodes of the rollout ring -> trajectory arena ----------------
  * Replaces the per-transition Batch.cat / return sums of TrajectoryBuffer.store
