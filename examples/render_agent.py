@@ -6,6 +6,11 @@ initialisation, step ``DeviceVectorEnv(task, --envs, render_mode="rgb_array")`` 
 
   python examples/render_agent.py --task SafetyPointButton2Gymnasium-v0 --envs 4 --out /tmp/button2
   python examples/render_agent.py --task SafetyCarCircle-v0 --path logs/.../checkpoint/model.pt --out /tmp/circle
+
+A user-defined device env renders when its struct defines ``draw`` (DESIGN §7): ``--header`` builds the plugin of the
+header, registers it as ``--task_name`` and watches the agent on it instead of ``--task``.
+
+  python examples/render_agent.py --header my_env.h --path logs/.../checkpoint/model.pt --out /tmp/mine
 """
 import argparse
 import math
@@ -86,6 +91,10 @@ def write(frames, out, fmt, fps):
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--task", default="SafetyCarCircle-v0", choices=sorted(envs.KINDS))
+    ap.add_argument("--header", default=None, help="a header defining UserEnv with draw: render its plugin, not --task")
+    ap.add_argument("--task_name", default=None, help="the task name of the --header plugin (default: <stem>-v0)")
+    ap.add_argument("--plugin_dir", default=None, help="where --header's plugin is built and cached "
+                                                       "(default: build_device_env's)")
     ap.add_argument("--algo", default="ppol", choices=sorted(ALGOS))
     ap.add_argument("--hidden_sizes", type=int, nargs="+", default=[128, 128])
     ap.add_argument("--path", default=None, help="checkpoint written by train_agent.py ({'model': state_dict, ...})")
@@ -98,10 +107,14 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=0)
     args = ap.parse_args(argv)
 
-    demo_env = envs.make(args.task)
+    task = args.task
+    if args.header is not None:
+        task = args.task_name or os.path.splitext(os.path.basename(args.header))[0] + "-v0"
+        envs.register_device_env(task, envs.build_device_env(args.header, out=args.plugin_dir))
+    demo_env = envs.make(task)
     agent = ALGOS[args.algo](env=demo_env, hidden_sizes=tuple(args.hidden_sizes), seed=args.seed)
     policy = agent.policy
-    venv = envs.DeviceVectorEnv(args.task, args.envs, seed=args.seed, render_mode="rgb_array",
+    venv = envs.DeviceVectorEnv(task, args.envs, seed=args.seed, render_mode="rgb_array",
                                 render_size=tuple(args.size))
     if args.path is not None:
         ckpt = torch.load(args.path, map_location="cuda")

@@ -192,6 +192,10 @@ class EnvPlugin(ctypes.Structure):
                 ("norm_steps", c_vp)]
 
 
+class EnvRenderer(ctypes.Structure):
+    _fields_ = [("abi_version", c_int), ("pad", c_int), ("render", c_vp)]
+
+
 ALGO_SAC, ALGO_DDPG = 0, 1
 OFF_STATS = 8
 CVPO_STATS = 16
@@ -220,6 +224,7 @@ SIGNATURES = {
     "fsrl_env_reset_ids": (c_int, [ctypes.POINTER(Rollout), c_vp, c_int, c_f32p, c_vp]),
     "fsrl_env_render": (c_int, [ctypes.POINTER(Rollout), c_vp, c_int, c_int, c_int, c_f32p, c_u8p, c_vp]),
     "fsrl_env_register": (c_int, [ctypes.POINTER(EnvPlugin), ctypes.POINTER(c_int)]),
+    "fsrl_env_register_renderer": (c_int, [c_int, ctypes.POINTER(EnvRenderer)]),
     "fsrl_host_pack_bytes": (c_size, [c_int, c_int, c_int]),
     "fsrl_host_collect_step": (c_int, [ctypes.POINTER(Rollout), ctypes.POINTER(HostStep), c_vp]),
     "fsrl_host_pack_norm_bytes": (c_size, [c_int, c_int, c_int, c_int]),
@@ -302,7 +307,7 @@ def _check_abi_sizes():
     lib.fsrl_abi_sizeof.argtypes = [c_int]
     for which, cls in enumerate((Mlp3, CollectStats, Rollout, PpoUpdate, NetRef, NetList, Engine, EngInput,
                                  OffPolicy, Cpo, Cvpo, TrajRow, TrajScan, TrajArena, HostStep, ObsRms, HostNorm,
-                                 EnvPlugin)):
+                                 EnvPlugin, EnvRenderer)):
         want = lib.fsrl_abi_sizeof(which)
         if want != ctypes.sizeof(cls):
             raise ImportError(f"ABI mismatch: {cls.__name__} is {ctypes.sizeof(cls)} bytes in python, "

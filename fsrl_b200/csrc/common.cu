@@ -69,6 +69,7 @@ extern "C" size_t fsrl_abi_sizeof(int which) {
         case 15: return sizeof(fsrl_obs_rms_t);
         case 16: return sizeof(fsrl_host_norm_t);
         case 17: return sizeof(fsrl_env_plugin_t);
+        case 18: return sizeof(fsrl_env_renderer_t);
         default: return 0;
     }
 }

@@ -5,7 +5,13 @@
 // the six launchers of ROLLOUT_LAUNCHERS are instantiated for it from the same templates as a built-in kind:
 // with the library's flags, a plugin of a built-in struct compiles to the same kernels as the library's.
 // fsrl_env_plugin() returns the table fsrl_env_register takes; the kind id is assigned there.
-#include "rollout.cuh"
+// A struct that also defines the optional `draw` of the drawing contract (render.cuh, DESIGN §7) gets the
+// rasterizer of fsrl_env_render instantiated for it, and fsrl_env_plugin_render() returns the table
+// fsrl_env_register_renderer takes; without draw nothing of the renderer is compiled and that getter returns NULL.
+#include "render.cuh"
+
+#include <type_traits>
+#include <utility>
 
 namespace fsrl {
 
@@ -22,6 +28,63 @@ static_assert(::UserEnv::T >= 1, "env plugin limit: T >= 1");
 
 template <>
 struct Env<ENV_USER> : ::UserEnv {};
+
+// The drawing contract: UserEnv may define
+//   __device__ static void draw(const float* st, uint32_t seed, uint32_t env, uint32_t ep, bool cost,
+//                               fsrl::render::Builder& b);
+// detected by name; a draw that cannot be called so is a compile error whose text build_device_env reports.
+template <typename E, typename = void>
+struct has_draw : std::false_type {};
+template <typename E>
+struct has_draw<E, std::void_t<decltype(&E::draw)>> : std::true_type {};
+template <typename E, typename = void>
+struct draw_callable : std::false_type {};
+template <typename E>
+struct draw_callable<E, std::void_t<decltype(E::draw(std::declval<const float*>(), uint32_t{}, uint32_t{}, uint32_t{},
+                                                     bool{}, std::declval<render::Builder&>()))>> : std::true_type {};
+constexpr bool USER_DRAWS = has_draw<::UserEnv>::value;
+static_assert(!USER_DRAWS || draw_callable<::UserEnv>::value,
+              "env plugin contract: UserEnv::draw must be a __device__ static function callable as "
+              "draw(const float* st, uint32_t seed, uint32_t env, uint32_t ep, bool cost, fsrl::render::Builder& b)");
+
+// UserEnv's scene: the window [-1, 1] x [-1, 1] unless draw sets one, then at most MAX_PRIM - 1 of draw's primitives
+// in order (Builder::put keeps the first MAX_PRIM), so decode's progress bar always fits.  Empty without draw, when
+// nothing instantiates it.
+template <typename E, bool = USER_DRAWS>
+struct UserScene {
+    __device__ static void draw(render::Builder&, float*, uint32_t, uint32_t, uint32_t, bool) {}
+};
+template <typename E>
+struct UserScene<E, true> {
+    __device__ static void draw(render::Builder& b, float* st, uint32_t seed, uint32_t env, uint32_t ep, bool cost) {
+        b.window(0.0f, 0.0f, 1.0f, 1.0f);
+        E::draw(st, seed, env, ep, cost, b);
+        if (b.sc.n > render::MAX_PRIM - 1) b.sc.n = render::MAX_PRIM - 1;
+    }
+};
+
+template <>
+__device__ void render::scene<ENV_USER>(render::Builder& b, float* st, uint32_t seed, uint32_t env, uint32_t ep,
+                                        bool cost) {
+    UserScene<::UserEnv>::draw(b, st, seed, env, ep, cost);
+}
+
+// the table fsrl_env_plugin_render returns: the render launcher with draw, NULL without
+template <typename E, bool = USER_DRAWS>
+struct UserRenderer {
+    static const fsrl_env_renderer_t* table() { return nullptr; }
+};
+template <typename E>
+struct UserRenderer<E, true> {
+    static int render(const fsrl_rollout_t* r, const int32_t* ids, int n, int height, int width, const float* last_cost,
+                      uint8_t* out, void* s) {
+        return render::launch<ENV_USER>(*r, ids, n, height, width, last_cost, out, static_cast<cudaStream_t>(s));
+    }
+    static const fsrl_env_renderer_t* table() {
+        static const fsrl_env_renderer_t t = {FSRL_ABI_VERSION, 0, render};
+        return &t;
+    }
+};
 
 ROLLOUT_LAUNCHERS(, ENV_USER)
 
@@ -53,4 +116,8 @@ extern "C" __attribute__((visibility("default"))) const fsrl_env_plugin_t* fsrl_
                                             fsrl::reset_all, fsrl::steps, fsrl::act_step,
                                             fsrl::env_step, fsrl::reset_ids, fsrl::norm_steps};
     return &table;
+}
+
+extern "C" __attribute__((visibility("default"))) const fsrl_env_renderer_t* fsrl_env_plugin_render(void) {
+    return fsrl::UserRenderer<::UserEnv>::table();
 }

@@ -23,10 +23,18 @@ namespace fsrl {
 static fsrl_env_plugin_t g_plugins[FSRL_ENV_PLUGIN_END - FSRL_ENV_PLUGIN_FIRST];
 static std::atomic<int> g_n_plugins{0};
 static std::mutex g_register_mu;
+// The render launcher of slot k, attached after the slot is published (fsrl_env_register_renderer): set once from
+// NULL, read with acquire, so lookups take no lock either.
+static fsrl_env_renderer_t g_renderer_tables[FSRL_ENV_PLUGIN_END - FSRL_ENV_PLUGIN_FIRST];
+static std::atomic<const fsrl_env_renderer_t*> g_renderers[FSRL_ENV_PLUGIN_END - FSRL_ENV_PLUGIN_FIRST];
 
 const fsrl_env_plugin_t* env_plugin(int kind) {
     const int k = kind - FSRL_ENV_PLUGIN_FIRST;
     return (k >= 0 && k < g_n_plugins.load(std::memory_order_acquire)) ? &g_plugins[k] : nullptr;
+}
+
+const fsrl_env_renderer_t* env_plugin_renderer(int kind) {
+    return env_plugin(kind) ? g_renderers[kind - FSRL_ENV_PLUGIN_FIRST].load(std::memory_order_acquire) : nullptr;
 }
 
 bool env_kind_dims(int kind, EnvDims& d) {
@@ -205,5 +213,21 @@ extern "C" int fsrl_env_register(const fsrl_env_plugin_t* p, int* kind) {
     g_plugins[n] = *p;
     g_n_plugins.store(n + 1, std::memory_order_release);
     *kind = FSRL_ENV_PLUGIN_FIRST + n;
+    return FSRL_OK;
+}
+
+extern "C" int fsrl_env_register_renderer(int kind, const fsrl_env_renderer_t* r) {
+    FSRL_REQUIRE(r != nullptr && r->render != nullptr, "fsrl_env_register_renderer: null table or launcher");
+    FSRL_REQUIRE(r->abi_version == fsrl_abi_version(),
+                 "fsrl_env_register_renderer: the plugin was built for ABI version %d, this library has version %d",
+                 r->abi_version, fsrl_abi_version());
+    FSRL_REQUIRE(env_plugin(kind) != nullptr, "fsrl_env_register_renderer: env kind %d is not a registered plugin kind",
+                 kind);
+    std::lock_guard<std::mutex> lock(g_register_mu);
+    const int k = kind - FSRL_ENV_PLUGIN_FIRST;
+    FSRL_REQUIRE(g_renderers[k].load(std::memory_order_relaxed) == nullptr,
+                 "fsrl_env_register_renderer: env kind %d already has a renderer", kind);
+    g_renderer_tables[k] = *r;
+    g_renderers[k].store(&g_renderer_tables[k], std::memory_order_release);
     return FSRL_OK;
 }

@@ -597,6 +597,8 @@ ROLLOUT_VEL_KINDS(ROLLOUT_LAUNCHERS, extern)
 
 // host: the launcher table of a registered plugin kind (fsrl_env_register, rollout.cu), NULL for any other kind
 const fsrl_env_plugin_t* env_plugin(int kind);
+// host: the render launcher registered for a plugin kind (fsrl_env_register_renderer), NULL when it has none
+const fsrl_env_renderer_t* env_plugin_renderer(int kind);
 
 }  // namespace fsrl
 

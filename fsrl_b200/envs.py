@@ -54,6 +54,7 @@ class _Plugin(NamedTuple):
     kind: int
     path: str
     so: ctypes.CDLL       # kept loaded: the library calls its launchers
+    renders: bool         # its struct defines draw: render_mode="rgb_array" draws it (DESIGN §7)
 
 
 PLUGINS = {}   # task -> _Plugin, filled by register_device_env
@@ -110,8 +111,9 @@ class DeviceVectorEnv:
             raise ValueError(f"render_size (height, width) = {(height, width)} outside [{RENDER_MIN}, {RENDER_MAX}]")
         self.render_mode, self.render_size = render_mode, (height, width)
         proto = DeviceEnv(task)
-        if render_mode is not None and task in PLUGINS:
-            raise ValueError(f"{task!r} is a user-defined device env: it has no renderer, so render_mode must be None")
+        if render_mode is not None and task in PLUGINS and not PLUGINS[task].renders:
+            raise ValueError(f"{task!r} is a user-defined device env whose struct has no draw: it has no renderer, "
+                             "so render_mode must be None")
         self.task, self.kind = task, proto.kind
         self.env_num = int(env_num)
         self.device = torch.device(device)
@@ -245,7 +247,7 @@ class DeviceVectorEnv:
     def render(self, id=None, **kwargs):
         """With ``render_mode="rgb_array"``: one RGB frame per env (all, or the ones ``id`` lists; an env may be listed
         twice), a contiguous ``uint8`` CUDA tensor of shape ``(n, height, width, 3)``, drawn from the envs' state by
-        csrc/render.cu (views, primitives and palette: DESIGN §7).  Robots whose last step cost are drawn in the cost
+        csrc/render.cuh (views, primitives and palette: DESIGN §7; a user-defined env's scene is its struct's draw).  Robots whose last step cost are drawn in the cost
         colour.  Reads the env state only.  With ``render_mode=None``: ``None``."""
         if self.render_mode is None:
             return None
@@ -311,8 +313,9 @@ def build_device_env(header: str, out: Optional[str] = None) -> str:
     with the library's compiler and flags) and return the plugin's path, under ``out`` (default:
     :func:`default_plugin_dir`).  A plugin already built from the same header, ABI, flags and sources is returned
     as it is, without compiling.  Raises ``ValueError`` naming the limit when ``UserEnv`` breaks one of
-    1 <= A <= 8, D + A <= 80, 1 <= S <= 32, D >= 1, T >= 1, and :class:`EnvBuildError` with nvcc's message on any
-    other compile error."""
+    1 <= A <= 8, D + A <= 80, 1 <= S <= 32, D >= 1, T >= 1, ``ValueError`` with the contract's text when ``UserEnv``
+    defines a ``draw`` that cannot be called with the drawing contract's arguments, and :class:`EnvBuildError` with
+    nvcc's message on any other compile error."""
     header = os.path.abspath(header)
     if not os.path.isfile(header):
         raise FileNotFoundError(header)
@@ -328,6 +331,9 @@ def build_device_env(header: str, out: Optional[str] = None) -> str:
             limits = re.findall(r"env plugin limit: ([^\"\n]+)", res.stdout)
             if limits:
                 raise ValueError(f"{header}: UserEnv breaks the limit {limits[0]}")
+            contract = re.findall(r"env plugin contract: ([^\"\n]+)", res.stdout)
+            if contract:
+                raise ValueError(f"{header}: env plugin contract: {contract[0]}")
             raise EnvBuildError(f"building the env plugin of {header} failed:\n{res.stdout}")
         os.replace(tmp + ".ptxas.log", path + ".ptxas.log")
         os.replace(tmp, path)          # atomic: a concurrent build of the same key finds a complete file
@@ -345,6 +351,19 @@ def _load_plugin(plugin: str):
     return so, so.fsrl_env_plugin()
 
 
+def _plugin_renderer(so: ctypes.CDLL):
+    """The render table of a loaded plugin (its ``fsrl_env_plugin_render()``), or None when its struct has no draw
+    or it was built before plugins could render (no such symbol)."""
+    try:
+        fn = so.fsrl_env_plugin_render
+    except AttributeError:
+        return None
+    fn.restype = ctypes.POINTER(_lib.EnvRenderer)
+    fn.argtypes = []
+    table = fn()
+    return table if table else None
+
+
 def plugin_dims(plugin: str):
     """(D, A, S, T) of the env a plugin was built from (loads it; needs no GPU)."""
     _, t = _load_plugin(plugin)
@@ -354,8 +373,8 @@ def plugin_dims(plugin: str):
 def register_device_env(task: str, plugin: str) -> int:
     """Register the plugin ``plugin`` (a path from :func:`build_device_env`) under the task name ``task`` and return
     its env kind.  Afterwards ``task`` works wherever a built-in device task does (``DeviceVectorEnv``, ``make``,
-    ``gym.make`` under ``compat.install()``, every collector, wrapper and agent), except rendering.  A built-in
-    task name is refused, and so is a name already registered from another plugin; registering the same plugin
+    ``gym.make`` under ``compat.install()``, every collector, wrapper and agent); ``render_mode="rgb_array"`` too when
+    the struct defines ``draw`` (DESIGN §7).  A built-in task name is refused, and so is a name already registered from another plugin; registering the same plugin
     under the same name again returns its kind."""
     if task in KINDS:
         raise ValueError(f"{task!r} is a built-in task; register the plugin under another name")
@@ -365,9 +384,12 @@ def register_device_env(task: str, plugin: str) -> int:
             return PLUGINS[task].kind
         raise ValueError(f"{task!r} is already registered from {PLUGINS[task].path}")
     so, table = _load_plugin(path)
+    renderer = _plugin_renderer(so)
     kind = ctypes.c_int()
     _lib.check(_lib.lib.fsrl_env_register(table, ctypes.byref(kind)))
-    PLUGINS[task] = _Plugin(kind.value, path, so)
+    if renderer is not None:
+        _lib.check(_lib.lib.fsrl_env_register_renderer(kind.value, renderer))
+    PLUGINS[task] = _Plugin(kind.value, path, so, renderer is not None)
     return kind.value
 
 

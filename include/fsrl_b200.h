@@ -176,8 +176,11 @@ int fsrl_env_reset_ids(const fsrl_rollout_t* r, const int32_t* ids, int n, float
  * env's scene that covers it (a fixed drawing order, one fixed palette, no antialiasing; DESIGN §7).
  * last_cost (device, E floats, may be NULL): the robot of env e is drawn in the cost colour when
  * last_cost[e] > 0.  Reads only env_state, env_t, ep_idx and seed_env of r, writes only out.
- * Returns FSRL_EINVAL before touching the device on an unknown or a plugin kind (fsrl_env_register), n < 1, an id outside [0, E),
- * height or width outside [16, 1024], or a null r, out or state pointer. */
+ * A plugin kind (fsrl_env_register) is drawn by the launcher its plugin registered with
+ * fsrl_env_register_renderer: the same rasterizer around the scene its struct's draw describes.
+ * Returns FSRL_EINVAL before touching the device on an unknown kind, n < 1, an id outside [0, E),
+ * height or width outside [16, 1024], a null r, out or state pointer, or, after all of these, a
+ * plugin kind without a renderer. */
 int fsrl_env_render(const fsrl_rollout_t* r, const int32_t* ids, int n, int height, int width,
                     const float* last_cost, uint8_t* out, void* stream);
 
@@ -274,8 +277,8 @@ int fsrl_rollout_norm_steps(const fsrl_rollout_t* r, const fsrl_obs_rms_t* n, in
  * struct by the same templates the built-in kinds use, and the struct's widths and horizon.
  * fsrl_env_register copies the table and returns in *kind the next free id of
  * [FSRL_ENV_PLUGIN_FIRST, FSRL_ENV_PLUGIN_END); from then on fsrl_env_dims, the rollout, gym-protocol,
- * observation-normalizing and trajectory entry points accept that kind like a built-in one.
- * fsrl_env_render refuses it.  Returns FSRL_EINVAL, registering nothing, when abi_version differs from
+ * observation-normalizing and trajectory entry points accept that kind like a built-in one, and
+ * fsrl_env_render does once a renderer is registered for it (below).  Returns FSRL_EINVAL, registering nothing, when abi_version differs from
  * fsrl_abi_version(), a width is outside the limits below, a launcher is NULL or the range is full.
  * Limits: 1 <= D, 1 <= A <= 8, D + A <= FSRL_ENG_DX_LD, 1 <= S <= 32, T >= 1. */
 #define FSRL_ENV_PLUGIN_FIRST 64
@@ -292,6 +295,18 @@ typedef struct fsrl_env_plugin {
     int (*norm_steps)(const fsrl_rollout_t* r, const fsrl_obs_rms_t* n, int n_steps, const float* act, void* stream);
 } fsrl_env_plugin_t;
 int fsrl_env_register(const fsrl_env_plugin_t* p, int* kind);
+/* A plugin whose struct defines draw also hands over a render launcher (its fsrl_env_plugin_render()):
+ * fsrl_env_render's rasterizer instantiated for the struct, called by fsrl_env_render with the
+ * arguments it has checked.  fsrl_env_register_renderer attaches it to the registered plugin kind
+ * `kind`, once.  Returns FSRL_EINVAL, attaching nothing, on a null table or launcher, an abi_version
+ * other than fsrl_abi_version(), a kind that is not a registered plugin kind, or a kind that already
+ * has a renderer.  A plugin built without draw, or before this entry point existed, has no renderer. */
+typedef struct fsrl_env_renderer {
+    int abi_version, pad;
+    int (*render)(const fsrl_rollout_t* r, const int32_t* ids, int n, int height, int width, const float* last_cost,
+                  uint8_t* out, void* stream);
+} fsrl_env_renderer_t;
+int fsrl_env_register_renderer(int kind, const fsrl_env_renderer_t* r);
 
 /* ---- offline datasets: finished episodes of the rollout ring -> trajectory arena ----------------
  * Replaces the per-transition Batch.cat / return sums of TrajectoryBuffer.store

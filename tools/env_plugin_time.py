@@ -76,13 +76,13 @@ def compare_ptxas():
     return 0 if same else 1
 
 
-def compile_time(reps):
+def compile_time(reps, header):
     from fsrl_b200 import envs
     for _ in range(reps):
         with tempfile.TemporaryDirectory() as d:
             t0 = time.perf_counter()
-            envs.build_device_env(HEADER, out=d)
-            print(json.dumps({"what": "plugin compile", "header": "tests/envs/car_circle.h",
+            envs.build_device_env(header, out=d)
+            print(json.dumps({"what": "plugin compile", "header": os.path.relpath(header, ROOT),
                               "seconds": round(time.perf_counter() - t0, 2)}))
 
 
@@ -124,12 +124,13 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--compile-time", action="store_true")
+    ap.add_argument("--header", default=HEADER, help="the header --compile-time builds (default: the CarCircle one)")
     ap.add_argument("--ptxas", action="store_true")
     a = ap.parse_args()
     if a.ptxas:
         return compare_ptxas()
     if a.compile_time:
-        return compile_time(a.reps)
+        return compile_time(a.reps, os.path.abspath(a.header))
     return time_collects(a.reps, a.warmup)
 
 

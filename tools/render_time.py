@@ -2,8 +2,11 @@
 of the task (default SafetyPointButton2Gymnasium-v0, the largest scene).  Each shape is timed with CUDA events over
 --iters back-to-back render() calls after a warm-up, best of --reps; the output tensor's allocation is inside the window,
 as a caller of render() pays it.  Prints one JSON line with frames/s per shape, the card name and its power limit.
+``--header`` times a user-defined env instead: the plugin of a header whose struct defines draw (DESIGN §7), e.g.
+tests/envs_render/car_circle_drawn.h beside the built-in SafetyCarCircle-v0 it restates.
 
     python tools/render_time.py [--task SafetyPointButton2Gymnasium-v0] [--iters 20] [--reps 5]
+    python tools/render_time.py --header tests/envs_render/car_circle_drawn.h [--plugin_dir fsrl_b200/_obj/env_plugins]
 """
 from __future__ import annotations
 
@@ -20,6 +23,8 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--task", default="SafetyPointButton2Gymnasium-v0")
+    ap.add_argument("--header", default=None, help="time the plugin of this header (its struct draws) instead of --task")
+    ap.add_argument("--plugin_dir", default=None, help="where --header's plugin is built and cached")
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--reps", type=int, default=5)
     a = ap.parse_args()
@@ -27,10 +32,13 @@ def main():
     import torch
     from env_collect_time import _card
 
-    from fsrl_b200.envs import DeviceVectorEnv
+    from fsrl_b200.envs import DeviceVectorEnv, build_device_env, register_device_env
     assert torch.cuda.is_available(), "render_time needs a GPU"
+    if a.header is not None:
+        a.task = "Plugin-" + os.path.splitext(os.path.basename(a.header))[0]
+        register_device_env(a.task, build_device_env(a.header, out=a.plugin_dir))
     name, plimit = _card()
-    res = {"tool": "render_time", "task": a.task, "gpu": name, "power_limit_w": plimit, "iters": a.iters}
+    res = {"tool": "render_time", "task": a.task, "header": a.header, "gpu": name, "power_limit_w": plimit, "iters": a.iters}
     for E in (16, 256):
         for size in ((256, 256), (64, 64)):
             venv = DeviceVectorEnv(a.task, E, seed=1, render_mode="rgb_array", render_size=size)
