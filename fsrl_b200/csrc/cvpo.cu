@@ -83,6 +83,9 @@ __device__ __forceinline__ float cvpo_qmin(const fsrl_offpolicy_t& o, int i, int
 // every dual iteration and once more for the weights.  Per iteration the dual gradients are closed-form:
 //   d/d eta    = eps_kl + mean_b(lse_b - log K) - mean_b(sum_k p_kb c_kb) / eta,   lse_b = logsumexp_k(c_kb / eta)
 //   d/d lambda = qc_thres - mean_b(sum_k p_kb q_c,kb),                              p = softmax_k(c / eta)
+// Each row is shifted by its largest c before the division: with x_k = (c_k - cm_b) / eta the eta term's row is
+// log(sum_k e^x_k) - sum_k p_k x_k, the entropy of the weights (at most log K), and the weights carry no exponent
+// error of size |c| / eta.  Unshifted, both are differences of numbers of size |c| / eta.
 __global__ void __launch_bounds__(ESTEP_T) cvpo_estep_kernel(const fsrl_cvpo_t d, int B, float* __restrict__ stat) {
     __shared__ double red[ESTEP_T / 32];
     __shared__ float s_dual[2];
@@ -101,39 +104,42 @@ __global__ void __launch_bounds__(ESTEP_T) cvpo_estep_kernel(const fsrl_cvpo_t d
     const float logK = logf((float)K);
     for (int it = 0; it < d.estep_iters; ++it) {
         const float eta = s_dual[0], lam = s_dual[1];
-        double s_lse = 0.0, s_pc = 0.0, s_pq = 0.0;
+        // Adam's bias corrections, in every thread before the rows: pow is a call, and few values are live here.
+        // st[6] was last written by thread 0 before the barrier.
+        const float t = st[6] + 1.0f;
+        const double bc1 = 1.0 - pow(0.9, (double)t), bc2 = 1.0 - pow(0.999, (double)t);
+        const AdamStep ad = {0.1f, 0.999f, 0.001f, (float)sqrt(bc2), 1e-8f, (float)(-(d.estep_dual_lr / bc1))};
+        double s_lse = 0.0, s_ent = 0.0, s_pq = 0.0;
         for (int b = tid; b < B; b += ESTEP_T) {
-            float mx = -INFINITY;
+            float cm = -INFINITY;
             for (int k = 0; k < K; ++k) {
                 const int r = k * B + b;
                 float c = d.comb[r];
                 if (C > 1) c = __fsub_rn(c, __fmul_rn(lam, cvpo_qmin(o, 1, r)));
                 d.comb[r] = c;
-                mx = fmaxf(mx, c / eta);
+                cm = fmaxf(cm, c);
             }
-            float se = 0.f, pc = 0.f, pq = 0.f;
+            float se = 0.f, sx = 0.f, pq = 0.f;
             for (int k = 0; k < K; ++k) {
                 const int r = k * B + b;
-                const float c = d.comb[r];
-                const float e = expf(c / eta - mx);
-                se += e; pc += e * c;
+                const float x = (d.comb[r] - cm) / eta;
+                const float e = expf(x);
+                se += e; sx += e * x;
                 if (C > 1) pq += e * cvpo_qmin(o, 1, r);
             }
-            s_lse += (double)(mx + logf(se) - logK);
-            s_pc += (double)(pc / se);
+            const float lse = logf(se);
+            s_lse += (double)(cm / eta + lse - logK);
+            s_ent += (double)(lse - sx / se - logK);
             s_pq += (double)(pq / se);
         }
         s_lse = block_sum<ESTEP_T / 32>(s_lse, red);
-        s_pc = block_sum<ESTEP_T / 32>(s_pc, red);
+        s_ent = block_sum<ESTEP_T / 32>(s_ent, red);
         s_pq = block_sum<ESTEP_T / 32>(s_pq, red);
         if (tid == 0) {
-            const float m_lse = (float)(s_lse / B), m_pc = (float)(s_pc / B), m_pq = (float)(s_pq / B);
+            const float m_lse = (float)(s_lse / B), m_ent = (float)(s_ent / B), m_pq = (float)(s_pq / B);
             float loss = eta * d.estep_kl + eta * m_lse;
-            const float g[2] = {d.estep_kl + m_lse - m_pc / eta, d.qc_thres - m_pq};
+            const float g[2] = {d.estep_kl + m_ent, d.qc_thres - m_pq};
             if (C > 1) loss += lam * d.qc_thres;
-            const float t = st[6] + 1.0f;
-            const double bc1 = 1.0 - pow(0.9, (double)t), bc2 = 1.0 - pow(0.999, (double)t);
-            const AdamStep ad = {0.1f, 0.999f, 0.001f, (float)sqrt(bc2), 1e-8f, (float)(-(d.estep_dual_lr / bc1))};
             for (int i = 0; i < C; ++i) {
                 float m = st[2 + i], v = st[4 + i];
                 st[i] = adam_update(st[i], g[i], m, v, ad);
@@ -155,18 +161,18 @@ __global__ void __launch_bounds__(ESTEP_T) cvpo_estep_kernel(const fsrl_cvpo_t d
     __syncthreads();
     const float eta = s_dual[0], lam = s_dual[1];
     for (int b = tid; b < B; b += ESTEP_T) {                        // optimal_q -= ...; softmax over k (:360-363)
-        float mx = -INFINITY;
+        float cm = -INFINITY;
         for (int k = 0; k < K; ++k) {
             const int r = k * B + b;
             float c = d.comb[r];
             if (C > 1) c = __fsub_rn(c, __fmul_rn(lam, cvpo_qmin(o, 1, r)));
             d.comb[r] = c;
-            mx = fmaxf(mx, c / eta);
+            cm = fmaxf(cm, c);
         }
         float se = 0.f;
         for (int k = 0; k < K; ++k) {
             const int r = k * B + b;
-            const float e = expf(d.comb[r] / eta - mx);
+            const float e = expf((d.comb[r] - cm) / eta);
             d.weights[r] = e;
             se += e;
         }

@@ -14,7 +14,9 @@ DX_LD = _lib.lib.fsrl_engine_dx_ld()   # row stride of the 'dx' region, and the 
 
 
 class EngineCtx:
-    def __init__(self, arena: Arena, bmax: int, extra_slots: int = 0):
+    def __init__(self, arena: Arena, bmax: int, extra_slots: int = 0, grown_from: Optional["EngineCtx"] = None):
+        """grown_from: the context this one replaces when a caller needs more rows.  Its Adam moments carry over,
+        since the learners' step counters keep counting across the growth."""
         self.arena = arena
         self.bmax = int(bmax)
         dev = arena.device
@@ -25,8 +27,11 @@ class EngineCtx:
         self._n_base = len(arena.slots)
         self.scratch = torch.zeros(n * self.slot_floats, dtype=torch.float32, device=dev)
         self.w2n = torch.zeros(len(arena.slots) * H * H, dtype=torch.float32, device=dev)
-        self.adam_m = torch.zeros_like(arena.theta)
-        self.adam_v = torch.zeros_like(arena.theta)
+        if grown_from is not None:
+            self.adam_m, self.adam_v = grown_from.adam_m, grown_from.adam_v
+        else:
+            self.adam_m = torch.zeros_like(arena.theta)
+            self.adam_v = torch.zeros_like(arena.theta)
         self._index = {id(s): i for i, s in enumerate(arena.slots)}
         self.sync_mirror(arena.slots)
 

@@ -48,7 +48,7 @@ class OffPolicyEngine(BasePolicy):
 
     def _ensure_engine(self, bmax: int):
         if self._eng is None or self._eng.bmax < bmax:
-            self._eng = EngineCtx(self.arena, max(bmax, 256))
+            self._eng = EngineCtx(self.arena, max(bmax, 256), grown_from=self._eng)
             B, dev = self._eng.bmax, self.device
             A = int(self.actor.output_dim)
             self._A = A

@@ -23,7 +23,7 @@ class TrustRegionMixin:
     # ---- engine ----------------------------------------------------------------------------------------
     def _ensure_engine(self, n: int) -> EngineCtx:
         if self._eng is None or self._eng.bmax < n:
-            self._eng = EngineCtx(self.arena, n, extra_slots=1)
+            self._eng = EngineCtx(self.arena, n, extra_slots=1, grown_from=self._eng)
             P = self.arena.slots[0].size
             dev = self.device
             self._vec = {k: torch.zeros(P, dtype=torch.float32, device=dev)

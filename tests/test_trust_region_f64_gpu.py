@@ -762,21 +762,27 @@ def _focops_head64(sq, z, ls, R, adv_r, adv_c, inv_lam, nu, eta):
     return kl.detach(), kl_s.detach(), sums, scl, torch.cat([gz, gl], 1), torch.cat([mz, ml], 1)
 
 
-@pytest.mark.parametrize("A,high,bounded,H,tem_lambda,clip", [
-    (2, 1.0, True, 64, 0.1, True), (3, 2.0, True, 128, 0.95, True), (8, 1.0, False, 256, 0.1, True),
-    (2, 1.0, False, 64, 50.0, False)], ids=["A2-b1-clip", "A3-b2-clip", "A8-unbounded-clip", "A2-unbounded-noclip"])
-def test_focops_step(A, high, bounded, H, tem_lambda, clip):
+@pytest.mark.parametrize("A,high,bounded,H,tem_lambda,clip,grown", [
+    (2, 1.0, True, 64, 0.1, True, False), (3, 2.0, True, 128, 0.95, True, False),
+    (8, 1.0, False, 256, 0.1, True, False), (2, 1.0, False, 64, 50.0, False, False), (2, 1.0, True, 64, 0.1, True, True)],
+    ids=["A2-b1-clip", "A3-b2-clip", "A8-unbounded-clip", "A2-unbounded-noclip", "A2-b1-clip-grown"])
+def test_focops_step(A, high, bounded, H, tem_lambda, clip, grown):
     """the merged last chunk of Batch.split(4000, merge_last=True) over 10 000 rows: 6000 rows, above one wgrad split.
-    tem_lambda sets the weight of the advantage term, and with it whether max_grad_norm = 0.5 clips"""
+    tem_lambda sets the weight of the advantage term, and with it whether max_grad_norm = 0.5 clips.  grown: the
+    warm-up step runs on a 3000-row engine, which the checked step's 6000 rows grow; Adam continues its moments"""
     D, n_all, n = 7 + A, 10_000, 6000
     p = _policy("focops", D, A, high, H=H, bounded=bounded, tem_lambda=tem_lambda, nu=0.3, auto_nu=False,
                 max_grad_norm=0.5)
     batch, _ = _batch(p, n_all, seed=10 + A, saturate=bounded)
     perm = _perm(batch.n, n, 12)
-    dv = _Dev(p, batch, perm, n)
-    s, sq, R = dv.a, _Sq(p), _Rows(batch, perm, n)
     p._eta = 1e9
-    p.policy_loss(batch, perm, n)               # warm-up: Adam moments away from zero
+    n_warm = n // 2 if grown else n
+    p._ensure_engine(n_warm)
+    p.policy_loss(batch, perm[:n_warm], n_warm)  # warm-up: Adam moments away from zero
+    eng_warm = p._eng
+    dv = _Dev(p, batch, perm, n)
+    assert (dv.eng is not eng_warm) == grown
+    s, sq, R = dv.a, _Sq(p), _Rows(batch, perm, n)
     _move(p, 13, 0.05 if clip else 0.03)        # and theta well away from theta_old, so the per-row KLs spread
     dv.eng.sync_mirror([s])
     masks = dv.forward()
@@ -795,7 +801,7 @@ def test_focops_step(A, high, bounded, H, tem_lambda, clip):
     assert gap / 2 > MARGIN * F32_EPS * float(kl_s[order[j:j + 2]].max()), (gap, kl_s[order[j:j + 2]])
     p._eta = eta
     sl = slice(s.offset, s.offset + s.size)
-    m0, v0, t0 = _d(dv.eng.adam_m[sl]).clone(), _d(dv.eng.adam_v[sl]).clone(), p._actor_t
+    m0, v0, t0 = _d(eng_warm.adam_m[sl]).clone(), _d(eng_warm.adam_v[sl]).clone(), p._actor_t   # the warm-up's moments
     st = p.policy_loss(batch, perm, n)
     errs = {}
     # per-minibatch normalised advantages (unbiased std)
@@ -830,23 +836,31 @@ def test_focops_step(A, high, bounded, H, tem_lambda, clip):
                        _ulps(_d(dv.eng.adam_v[sl]), vv, v0 + gc * gc))
     bounds = {"adv0": STD_TOL, "adv1": STD_TOL, "loss": SUM_TOL, "kl": SUM_TOL, "stat": SUM_TOL, "dout": DOUT_TOL,
               "grad": GRAD_TOL, "norm": SUM_TOL, "adam": ULP_TOL}
-    _report(f"focops A={A} high={high} bounded={bounded} H={H} eta={eta:.3e} kept={j + 1}/{n} "
+    _report(f"focops A={A} high={high} bounded={bounded} H={H} grown={grown} eta={eta:.3e} kept={j + 1}/{n} "
             f"|g|={math.sqrt(nsq64):.3f}", errs, bounds)
 
 
 # ---- 9. critic step --------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("algo,l2", [("cpo", 1e-3), ("focops", 1e-3), ("trpo", 0.0)])
-def test_critic_step(algo, l2):
+@pytest.mark.parametrize("algo,l2,grown", [("cpo", 1e-3, False), ("focops", 1e-3, False), ("trpo", 0.0, False),
+                                           ("trpo", 0.0, True)],
+                         ids=["cpo-0.001", "focops-0.001", "trpo-0.0", "trpo-0.0-grown"])
+def test_critic_step(algo, l2, grown):
+    """grown: the warm-up step runs on a 2000-row engine and the checked step on a 5000-row one, as learn() grows
+    the engine for a collect larger than all before it; Adam continues the warm-up's moments"""
     D, A, n_all, n = 12, 2, 6000, 5000
     p = _policy(algo, D, A, H=128)
     assert p._l2_reg == l2
     batch, _ = _batch(p, n_all, seed=14)
     perm = _perm(batch.n, n, 15)
+    n_warm = 2000 if grown else n
+    p._ensure_engine(n_warm)
+    p.critics_loss(batch, perm[:n_warm], n_warm)         # warm-up: Adam moments away from zero
+    eng = p._eng
+    th0, m0, v0 = _d(p.arena.theta).clone(), _d(eng.adam_m).clone(), _d(eng.adam_v).clone()
     p._ensure_engine(n)
-    p.critics_loss(batch, perm, n)                       # warm-up: Adam moments away from zero
+    assert (p._eng is not eng) == grown
     eng = p._eng
     crit = p.arena.slots[1:3]
-    th0, m0, v0 = _d(p.arena.theta).clone(), _d(eng.adam_m).clone(), _d(eng.adam_v).clone()
     t0 = p._critic_t
     st = p.critics_loss(batch, perm, n)
     torch.cuda.synchronize()
@@ -874,4 +888,4 @@ def test_critic_step(algo, l2):
         errs[f"adam{i}"] = max(_ulps(th1[sl], ref, ref.abs() + g["lr"]), _ulps(m1[sl], m, m0[sl].abs() + gd.abs()),
                                _ulps(v1[sl], v, v0[sl] + gd * gd))
     bounds = {k: {"gra": GRAD_TOL, "vf": SUM_TOL, "ada": ULP_TOL}[k[:3] if k[:2] != "vf" else "vf"] for k in errs}
-    _report(f"critic {algo} l2={l2} n={n}", errs, bounds)
+    _report(f"critic {algo} l2={l2} n={n} grown={grown}", errs, bounds)
