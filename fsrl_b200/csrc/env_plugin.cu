@@ -2,11 +2,11 @@
 // Compiled once per env with `-include <header>`; the header includes "envs.cuh" and defines, at global scope,
 // `UserEnv`: a struct with the contract of envs.cuh's built-in envs (static constexpr int D, A, S, T and the
 // __device__ functions reset / observe / step), or an alias of one of them.  UserEnv becomes Env<ENV_USER>, and
-// the six launchers of ROLLOUT_LAUNCHERS are instantiated for it from the same templates as a built-in kind:
-// with the library's flags, a plugin of a built-in struct compiles to the same kernels as the library's.
-// fsrl_env_plugin() returns the table fsrl_env_register takes; the kind id is assigned there.
+// fsrl_env_plugin() returns env_table<ENV_USER>(), the launcher table a built-in kind has, built from the same
+// templates: with the library's flags, a plugin of a built-in struct compiles to the same kernels as the library's.
+// fsrl_env_register takes the table; the kind id is assigned there.
 // A struct that also defines the optional `draw` of the drawing contract (render.cuh, DESIGN §7) gets the
-// rasterizer of fsrl_env_render instantiated for it, and fsrl_env_plugin_render() returns the table
+// rasterizer of fsrl_env_render instantiated for it, and fsrl_env_plugin_render() returns its render_table, which
 // fsrl_env_register_renderer takes; without draw nothing of the renderer is compiled and that getter returns NULL.
 #include "render.cuh"
 
@@ -76,45 +76,16 @@ struct UserRenderer {
 };
 template <typename E>
 struct UserRenderer<E, true> {
-    static int render(const fsrl_rollout_t* r, const int32_t* ids, int n, int height, int width, const float* last_cost,
-                      uint8_t* out, void* s) {
-        return render::launch<ENV_USER>(*r, ids, n, height, width, last_cost, out, static_cast<cudaStream_t>(s));
-    }
     static const fsrl_env_renderer_t* table() {
-        static const fsrl_env_renderer_t t = {FSRL_ABI_VERSION, 0, render};
+        static constexpr fsrl_env_renderer_t t = render_table<ENV_USER>();
         return &t;
     }
 };
 
-ROLLOUT_LAUNCHERS(, ENV_USER)
-
-static int reset_all(const fsrl_rollout_t* r, void* s) {
-    return launch_env_reset_all<ENV_USER>(*r, static_cast<cudaStream_t>(s));
-}
-static int steps(const fsrl_rollout_t* r, int n_steps, int one_launch, void* s) {
-    return launch_steps_h<ENV_USER>(*r, n_steps, one_launch != 0, static_cast<cudaStream_t>(s));
-}
-static int act_step(const fsrl_rollout_t* r, const float* act, void* s) {
-    return launch_act_step<ENV_USER>(*r, act, static_cast<cudaStream_t>(s));
-}
-static int env_step(const fsrl_rollout_t* r, const float* act, const int32_t* ids, int n, float* obs_next, float* rew,
-                    float* cost, uint8_t* term, uint8_t* trunc, void* s) {
-    return launch_env_step<ENV_USER>(*r, act, ids, n, obs_next, rew, cost, term, trunc, static_cast<cudaStream_t>(s));
-}
-static int reset_ids(const fsrl_rollout_t* r, const int32_t* ids, int n, float* obs, void* s) {
-    return launch_env_reset_ids<ENV_USER>(*r, ids, n, obs, static_cast<cudaStream_t>(s));
-}
-static int norm_steps(const fsrl_rollout_t* r, const fsrl_obs_rms_t* n, int n_steps, const float* act, void* s) {
-    return launch_norm_steps<ENV_USER>(*r, *n, n_steps, act, static_cast<cudaStream_t>(s));
-}
-
 }  // namespace fsrl
 
 extern "C" __attribute__((visibility("default"))) const fsrl_env_plugin_t* fsrl_env_plugin(void) {
-    using E_ = fsrl::Env<fsrl::ENV_USER>;
-    static const fsrl_env_plugin_t table = {FSRL_ABI_VERSION, E_::D, E_::A, E_::S, E_::T, 0,
-                                            fsrl::reset_all, fsrl::steps, fsrl::act_step,
-                                            fsrl::env_step, fsrl::reset_ids, fsrl::norm_steps};
+    static constexpr fsrl_env_plugin_t table = fsrl::env_table<fsrl::ENV_USER>();
     return &table;
 }
 

@@ -28,6 +28,19 @@ enum EnvKind { ENV_CAR_CIRCLE = 0, ENV_CAR_RUN = 1, ENV_BALL_CIRCLE = 2, ENV_BAL
                ENV_HALF_CHEETAH_VEL = 33, ENV_HOPPER_VEL = 34, ENV_SWIMMER_VEL = 35, ENV_WALKER2D_VEL = 36,
                ENV_ANT_VEL = 37 };
 
+// The built-in kinds, X(K) for each, in the three groups whose launchers compile in translation units of their own:
+// rollout.cu, rollout_bp.cu (Button, Push) and rollout_vel.cu (velocity).  One file for all of them would make the
+// library's build well over a third slower (DESIGN §5).
+#define ENV_KINDS_CORE(X)                                                                                              \
+    X(ENV_CAR_CIRCLE) X(ENV_CAR_RUN) X(ENV_BALL_CIRCLE) X(ENV_BALL_RUN) X(ENV_ANT_CIRCLE) X(ENV_POINT_GOAL)           \
+    X(ENV_ANT_RUN) X(ENV_DRONE_CIRCLE) X(ENV_DRONE_RUN) X(ENV_POINT_CIRCLE1) X(ENV_POINT_CIRCLE2) X(ENV_CAR_CIRCLE1) \
+    X(ENV_CAR_CIRCLE2) X(ENV_POINT_GOAL2) X(ENV_CAR_GOAL1) X(ENV_CAR_GOAL2)
+#define ENV_KINDS_BP(X)                                                                                                \
+    X(ENV_POINT_BUTTON1) X(ENV_POINT_BUTTON2) X(ENV_CAR_BUTTON1) X(ENV_CAR_BUTTON2) X(ENV_POINT_PUSH1)                \
+    X(ENV_POINT_PUSH2) X(ENV_CAR_PUSH1) X(ENV_CAR_PUSH2)
+#define ENV_KINDS_VEL(X) X(ENV_HALF_CHEETAH_VEL) X(ENV_HOPPER_VEL) X(ENV_SWIMMER_VEL) X(ENV_WALKER2D_VEL) X(ENV_ANT_VEL)
+#define ENV_KINDS(X) ENV_KINDS_CORE(X) ENV_KINDS_BP(X) ENV_KINDS_VEL(X)
+
 constexpr int ENV_MAX_A = 8;
 constexpr int ENV_MAX_S = 32;
 
@@ -115,36 +128,8 @@ constexpr float BOX_START = 1.0f;                   // the box starts in [-BOX_S
 
 struct EnvDims { int D, A, S, T; };
 
-__host__ __device__ inline EnvDims env_dims(int kind) {
-    switch (kind) {
-        case ENV_CAR_CIRCLE: return {8, 2, 6, 300};
-        case ENV_CAR_RUN: return {7, 2, 7, 200};
-        case ENV_BALL_CIRCLE: return {8, 2, 4, 200};
-        case ENV_BALL_RUN: return {7, 2, 5, 100};
-        case ENV_ANT_CIRCLE: return {34, 8, 30, 500};
-        case ENV_POINT_GOAL: return {60, 2, 28, 1000};
-        case ENV_ANT_RUN: return {34, 8, 31, 300};
-        case ENV_DRONE_CIRCLE: return {18, 4, 17, 300};
-        case ENV_DRONE_RUN: return {19, 4, 18, 200};
-        case ENV_POINT_CIRCLE1: case ENV_POINT_CIRCLE2: case ENV_CAR_CIRCLE1: case ENV_CAR_CIRCLE2:
-            return {28, 2, 7, 500};
-        case ENV_POINT_GOAL2: case ENV_CAR_GOAL2: return {60, 2, 10, 1000};
-        case ENV_CAR_GOAL1: return {60, 2, 28, 1000};
-        case ENV_POINT_BUTTON1: case ENV_POINT_BUTTON2: case ENV_CAR_BUTTON1: case ENV_CAR_BUTTON2:
-            return {76, 2, 12, 1000};
-        case ENV_POINT_PUSH1: case ENV_CAR_PUSH1: return {76, 2, 18, 1000};
-        case ENV_POINT_PUSH2: case ENV_CAR_PUSH2: return {76, 2, 28, 1000};
-        case ENV_HALF_CHEETAH_VEL: case ENV_WALKER2D_VEL: return {17, 6, 17, 1000};
-        case ENV_HOPPER_VEL: return {11, 3, 11, 1000};
-        case ENV_SWIMMER_VEL: return {8, 2, 9, 1000};
-        case ENV_ANT_VEL: return {27, 8, 26, 1000};
-        default: return {0, 0, 0, 0};
-    }
-}
-
-__host__ __device__ inline bool env_kind_known(int kind) { return env_dims(kind).D != 0; }
-
-// host: the widths of a built-in kind or of a registered plugin kind (rollout.cu); false for an unknown kind
+// host: the widths of a built-in kind or of a registered plugin kind, from its launcher table (rollout.cu); false for
+// an unknown kind
 bool env_kind_dims(int kind, EnvDims& d);
 
 // ---------------------------------------------------------------------------------------------

@@ -199,6 +199,22 @@ __device__ void scene(Builder& b, float* st, uint32_t seed, uint32_t env, uint32
 }
 
 }  // namespace render
+
+// the renderer of a known kind: a built-in kind's table, or the launcher registered for a plugin kind
+// (fsrl_env_register_renderer), NULL when it has none
+static const fsrl_env_renderer_t* env_renderer(int kind) {
+    switch (kind) {
+#define RENDER_TABLE_CASE(K)                                          \
+    case K: {                                                         \
+        static constexpr fsrl_env_renderer_t t = render_table<K>();   \
+        return &t;                                                    \
+    }
+        ENV_KINDS(RENDER_TABLE_CASE)
+#undef RENDER_TABLE_CASE
+        default: return env_plugin_renderer(kind);
+    }
+}
+
 }  // namespace fsrl
 
 using namespace fsrl;
@@ -206,28 +222,18 @@ using namespace fsrl;
 extern "C" int fsrl_env_render(const fsrl_rollout_t* r, const int32_t* ids, int n, int height, int width,
                                const float* last_cost, uint8_t* out, void* stream) {
     FSRL_REQUIRE(r != nullptr, "fsrl_env_render: null descriptor");
-    const bool plugin = env_plugin(r->kind) != nullptr;
-    FSRL_REQUIRE(plugin || env_kind_known(r->kind), "fsrl_env_render: unknown env kind %d", r->kind);
+    FSRL_REQUIRE(env_table(r->kind) != nullptr, "fsrl_env_render: unknown env kind %d", r->kind);
     FSRL_REQUIRE(r->E > 0, "fsrl_env_render: E must be positive");
     FSRL_REQUIRE(n >= 1, "fsrl_env_render: n = %d must be at least 1", n);
-    FSRL_REQUIRE(ids != nullptr || n == r->E, "fsrl_env_render: without ids, n must be E = %d (got %d)", r->E, n);
-    if (ids)
-        for (int i = 0; i < n; ++i)
-            FSRL_REQUIRE(ids[i] >= 0 && ids[i] < r->E, "fsrl_env_render: ids[%d] = %d outside [0, E = %d)", i, ids[i],
-                         r->E);
+    int rc = check_ids("fsrl_env_render", r, ids, n);
+    if (rc) return rc;
     FSRL_REQUIRE(height >= 16 && height <= 1024 && width >= 16 && width <= 1024,
                  "fsrl_env_render: frame size %d x %d outside [16, 1024]", height, width);
     FSRL_REQUIRE(out != nullptr, "fsrl_env_render: null output");
     FSRL_REQUIRE(r->env_state && r->env_t && r->ep_idx, "fsrl_env_render: null state pointer");
-    if (plugin) {   // a user-defined env draws through the launcher its plugin registered (fsrl_env_register_renderer)
-        const fsrl_env_renderer_t* pr = env_plugin_renderer(r->kind);
-        FSRL_REQUIRE(pr != nullptr,
-                     "fsrl_env_render: env kind %d is a user-defined env whose struct has no draw: it has no renderer",
-                     r->kind);
-        return pr->render(r, ids, n, height, width, last_cost, out, stream);
-    }
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    int rc = FSRL_OK;
-    DISPATCH_KIND(r->kind, rc = render::launch<K>(*r, ids, n, height, width, last_cost, out, s));
-    return rc;
+    const fsrl_env_renderer_t* t = env_renderer(r->kind);
+    FSRL_REQUIRE(t != nullptr,
+                 "fsrl_env_render: env kind %d is a user-defined env whose struct has no draw: it has no renderer",
+                 r->kind);
+    return t->render(r, ids, n, height, width, last_cost, out, stream);
 }

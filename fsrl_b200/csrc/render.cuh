@@ -184,6 +184,18 @@ int launch(const fsrl_rollout_t& r, const int32_t* ids, int n, int H, int W, con
 }
 
 }  // namespace render
+
+// The renderer table of kind K: render::launch<K> behind the C signature of fsrl_env_renderer_t.  fsrl_env_render
+// reaches a kind through such a table: render.cu defines the built-in kinds', env_plugin.cu a drawing plugin's.
+template <int K>
+constexpr fsrl_env_renderer_t render_table() {
+    return {FSRL_ABI_VERSION, 0,
+            [](const fsrl_rollout_t* r, const int32_t* ids, int n, int height, int width, const float* last_cost,
+               uint8_t* out, void* s) {
+                return render::launch<K>(*r, ids, n, height, width, last_cost, out, static_cast<cudaStream_t>(s));
+            }};
+}
+
 }  // namespace fsrl
 
 #endif  // FSRL_RENDER_CUH

@@ -28,7 +28,8 @@ static std::mutex g_register_mu;
 static fsrl_env_renderer_t g_renderer_tables[FSRL_ENV_PLUGIN_END - FSRL_ENV_PLUGIN_FIRST];
 static std::atomic<const fsrl_env_renderer_t*> g_renderers[FSRL_ENV_PLUGIN_END - FSRL_ENV_PLUGIN_FIRST];
 
-const fsrl_env_plugin_t* env_plugin(int kind) {
+// the table of a registered plugin kind, NULL for any other kind
+static const fsrl_env_plugin_t* env_plugin(int kind) {
     const int k = kind - FSRL_ENV_PLUGIN_FIRST;
     return (k >= 0 && k < g_n_plugins.load(std::memory_order_acquire)) ? &g_plugins[k] : nullptr;
 }
@@ -37,13 +38,28 @@ const fsrl_env_renderer_t* env_plugin_renderer(int kind) {
     return env_plugin(kind) ? g_renderers[kind - FSRL_ENV_PLUGIN_FIRST].load(std::memory_order_acquire) : nullptr;
 }
 
-bool env_kind_dims(int kind, EnvDims& d) {
-    if (const fsrl_env_plugin_t* p = env_plugin(kind)) {
-        d = {p->D, p->A, p->S, p->T};
-        return true;
+const fsrl_env_plugin_t* env_table(int kind) {
+    if (kind >= FSRL_ENV_PLUGIN_FIRST) return env_plugin(kind);
+    switch (kind) {
+        ENV_KINDS_CORE(ENV_TABLE_CASE)
+        default: break;
     }
-    d = env_dims(kind);
-    return d.D != 0;
+    if (const fsrl_env_plugin_t* t = env_table_bp(kind)) return t;
+    return env_table_vel(kind);
+}
+
+bool env_kind_dims(int kind, EnvDims& d) {
+    const fsrl_env_plugin_t* t = env_table(kind);
+    if (t) d = {t->D, t->A, t->S, t->T};
+    return t != nullptr;
+}
+
+int check_ids(const char* fn, const fsrl_rollout_t* a, const int32_t* ids, int n) {
+    FSRL_REQUIRE(ids != nullptr || n == a->E, "%s: without ids, n must be E = %d (got %d)", fn, a->E, n);
+    if (ids)
+        for (int i = 0; i < n; ++i)
+            FSRL_REQUIRE(ids[i] >= 0 && ids[i] < a->E, "%s: ids[%d] = %d outside [0, E = %d)", fn, i, ids[i], a->E);
+    return FSRL_OK;
 }
 
 // begin a collect: ready envs = first min(E, n_episode) (:235-236), zero the per-collect stats
@@ -62,14 +78,6 @@ __global__ void collect_begin_kernel(const fsrl_rollout_t a, int n_episode) {
 }  // namespace fsrl
 
 using namespace fsrl;
-
-// rc = kind's launcher: PCALL through the table p of a registered plugin kind, else CALL on the built-in kind K
-#define DISPATCH_ENV(kind, PCALL, CALL)                          \
-    if (const fsrl_env_plugin_t* p = env_plugin(kind)) {         \
-        rc = PCALL;                                              \
-    } else {                                                     \
-        DISPATCH_KIND(kind, rc = CALL);                          \
-    }
 
 // the env half of the descriptor (what every entry point touches)
 static int check_env_state(const fsrl_rollout_t* a) {
@@ -91,16 +99,6 @@ static int check_rollout(const fsrl_rollout_t* a) {
     return FSRL_OK;
 }
 
-// n rows, each an env id in [0, E) when ids (host) is given
-static int check_ids(const char* fn, const fsrl_rollout_t* a, const int32_t* ids, int n) {
-    FSRL_REQUIRE(n >= 1 && n <= a->E, "%s: n = %d outside [1, E = %d]", fn, n, a->E);
-    FSRL_REQUIRE(ids != nullptr || n == a->E, "%s: without ids, n must be E = %d (got %d)", fn, a->E, n);
-    if (ids)
-        for (int i = 0; i < n; ++i)
-            FSRL_REQUIRE(ids[i] >= 0 && ids[i] < a->E, "%s: ids[%d] = %d outside [0, E = %d)", fn, i, ids[i], a->E);
-    return FSRL_OK;
-}
-
 extern "C" int fsrl_env_dims(int kind, int* D, int* A, int* S, int* T) {
     EnvDims d;
     FSRL_REQUIRE(env_kind_dims(kind, d), "fsrl_env_dims: unknown env kind %d", kind);
@@ -111,9 +109,7 @@ extern "C" int fsrl_env_dims(int kind, int* D, int* A, int* S, int* T) {
 extern "C" int fsrl_env_reset_all(const fsrl_rollout_t* a, void* stream) {
     int rc = check_rollout(a);
     if (rc) return rc;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_ENV(a->kind, p->reset_all(a, s), launch_env_reset_all<K>(*a, s));
-    return rc;
+    return env_table(a->kind)->reset_all(a, stream);
 }
 
 extern "C" int fsrl_collect_begin(const fsrl_rollout_t* a, int n_episode, void* stream) {
@@ -134,21 +130,17 @@ extern "C" int fsrl_rollout_steps(const fsrl_rollout_t* a, int n_steps, void* st
                  "rollout: null actor weights");
     FSRL_REQUIRE(a->actor.out <= MLP_MAX_OUT, "rollout: actor out dim %d > %d", a->actor.out, MLP_MAX_OUT);
     if (n_steps == 0) return FSRL_OK;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     // inline bookkeeping: no env's step depends on another env's, so all steps run in one launch
     const char* per_step = getenv("FSRL_ROLLOUT_PER_STEP");
     const bool one_launch = a->inline_done && !(per_step && atoi(per_step) != 0);
-    DISPATCH_ENV(a->kind, p->steps(a, n_steps, one_launch, s), launch_steps_h<K>(*a, n_steps, one_launch, s));
-    return rc;
+    return env_table(a->kind)->steps(a, n_steps, one_launch, stream);
 }
 
 extern "C" int fsrl_rollout_steps_act(const fsrl_rollout_t* a, const float* act, void* stream) {
     int rc = check_env_state(a);
     if (rc) return rc;
     FSRL_REQUIRE(act != nullptr, "fsrl_rollout_steps_act: null action array");
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_ENV(a->kind, p->act_step(a, act, s), launch_act_step<K>(*a, act, s));
-    return rc;
+    return env_table(a->kind)->act_step(a, act, stream);
 }
 
 extern "C" int fsrl_rollout_norm_steps(const fsrl_rollout_t* a, const fsrl_obs_rms_t* n, int n_steps, const float* act,
@@ -167,32 +159,27 @@ extern "C" int fsrl_rollout_norm_steps(const fsrl_rollout_t* a, const fsrl_obs_r
         FSRL_REQUIRE(a->actor.out <= MLP_MAX_OUT, "rollout: actor out dim %d > %d", a->actor.out, MLP_MAX_OUT);
     }
     if (n_steps == 0) return FSRL_OK;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_ENV(a->kind, p->norm_steps(a, n, n_steps, act, s), launch_norm_steps<K>(*a, *n, n_steps, act, s));
-    return rc;
+    return env_table(a->kind)->norm_steps(a, n, n_steps, act, stream);
 }
 
 extern "C" int fsrl_env_step(const fsrl_rollout_t* a, const float* act, const int32_t* ids, int n, float* obs_next,
                              float* rew, float* cost, uint8_t* term, uint8_t* trunc, void* stream) {
     int rc = check_env_state(a);
     if (rc) return rc;
+    FSRL_REQUIRE(n >= 1 && n <= a->E, "fsrl_env_step: n = %d outside [1, E = %d]", n, a->E);   // one row per env at most
     rc = check_ids("fsrl_env_step", a, ids, n);
     if (rc) return rc;
     FSRL_REQUIRE(act && obs_next && rew && cost && term && trunc, "fsrl_env_step: null action or output array");
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_ENV(a->kind, p->env_step(a, act, ids, n, obs_next, rew, cost, term, trunc, s),
-                 launch_env_step<K>(*a, act, ids, n, obs_next, rew, cost, term, trunc, s));
-    return rc;
+    return env_table(a->kind)->env_step(a, act, ids, n, obs_next, rew, cost, term, trunc, stream);
 }
 
 extern "C" int fsrl_env_reset_ids(const fsrl_rollout_t* a, const int32_t* ids, int n, float* obs, void* stream) {
     int rc = check_env_state(a);
     if (rc) return rc;
+    FSRL_REQUIRE(n >= 1 && n <= a->E, "fsrl_env_reset_ids: n = %d outside [1, E = %d]", n, a->E);   // one row per env at most
     rc = check_ids("fsrl_env_reset_ids", a, ids, n);
     if (rc) return rc;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DISPATCH_ENV(a->kind, p->reset_ids(a, ids, n, obs, s), launch_env_reset_ids<K>(*a, ids, n, obs, s));
-    return rc;
+    return env_table(a->kind)->reset_ids(a, ids, n, obs, stream);
 }
 
 extern "C" int fsrl_env_register(const fsrl_env_plugin_t* p, int* kind) {

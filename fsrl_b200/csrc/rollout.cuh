@@ -1,6 +1,6 @@
 // The device side of rollout collection (see rollout.cu): the fused collect step, the caller-action step,
 // the resolve pass, resets and the gym-protocol step, templated over the env kind, and the host launchers
-// the C entry points of rollout.cu dispatch to.
+// of a kind with the table that carries them to the C entry points of rollout.cu.
 #pragma once
 #include "envs.cuh"
 #include "mlp.cuh"
@@ -428,44 +428,46 @@ __global__ void __launch_bounds__(128) env_step_ids_kernel(const fsrl_rollout_t 
     term_out[i] = term ? 1 : 0; trunc_out[i] = trunc ? 1 : 0;
 }
 
+// one launch of rollout_step_kernel<KIND, H> over the tiles of all E envs, n_steps steps each; the kernel's
+// dynamic shared memory limit is raised on its first launch
+template <int KIND, int H>
+int launch_step_tiles(const fsrl_rollout_t& a, int n_steps, cudaStream_t s) {
+    using TT = MlpTile<H>;
+    const size_t smem = TT::smem_bytes(Env<KIND>::D);
+    static bool attr_done = false;
+    if (!attr_done) {
+        FSRL_CUDA(cudaFuncSetAttribute(rollout_step_kernel<KIND, H>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)smem));
+        attr_done = true;
+    }
+    rollout_step_kernel<KIND, H><<<(a.E + TT::R - 1) / TT::R, MLP_TPB, smem, s>>>(a, n_steps);
+    FSRL_LAUNCH_CHECK();
+    return FSRL_OK;
+}
+
+// launch_step_tiles at the actor's hidden width
+template <int KIND>
+int launch_step_kernel(const fsrl_rollout_t& a, int n_steps, cudaStream_t s) {
+    switch (a.actor.H) {
+        case 64: return launch_step_tiles<KIND, 64>(a, n_steps, s);
+        case 128: return launch_step_tiles<KIND, 128>(a, n_steps, s);
+        case 256: return launch_step_tiles<KIND, 256>(a, n_steps, s);
+        case 512: return launch_step_tiles<KIND, 512>(a, n_steps, s);
+        default: set_error("rollout: hidden width %d unsupported (64/128/256/512)", a.actor.H); return FSRL_EINVAL;
+    }
+}
+
 // n_steps steps of the fused kernel, each followed by the resolve kernel; or, with `one_launch`, all of them
 // in one launch followed by one resolve (which turns finished_next into finished)
 template <int KIND>
 int launch_steps_h(const fsrl_rollout_t& a, int n_steps, bool one_launch, cudaStream_t s) {
-    const int H = a.actor.H;
-#define GO(HH)                                                                                   \
-    {                                                                                            \
-        using TT = MlpTile<HH>;                                                                  \
-        const size_t smem = TT::smem_bytes(Env<KIND>::D);                                        \
-        static bool attr_done = false;                                                           \
-        if (!attr_done) {                                                                        \
-            FSRL_CUDA(cudaFuncSetAttribute(rollout_step_kernel<KIND, HH>,                        \
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-            attr_done = true;                                                                    \
-        }                                                                                        \
-        const int grid = (a.E + TT::R - 1) / TT::R;                                              \
-        if (one_launch) {                                                                        \
-            rollout_step_kernel<KIND, HH><<<grid, MLP_TPB, smem, s>>>(a, n_steps);               \
-            FSRL_LAUNCH_CHECK();                                                                 \
-            rollout_resolve_kernel<KIND><<<1, 1024, 0, s>>>(a);                                  \
-            FSRL_LAUNCH_CHECK();                                                                 \
-        } else {                                                                                 \
-            for (int i = 0; i < n_steps; ++i) {                                                  \
-                rollout_step_kernel<KIND, HH><<<grid, MLP_TPB, smem, s>>>(a, 1);                 \
-                FSRL_LAUNCH_CHECK();                                                             \
-                rollout_resolve_kernel<KIND><<<1, 1024, 0, s>>>(a);                              \
-                FSRL_LAUNCH_CHECK();                                                             \
-            }                                                                                    \
-        }                                                                                        \
+    const int launches = one_launch ? 1 : n_steps, steps = one_launch ? n_steps : 1;
+    for (int i = 0; i < launches; ++i) {
+        const int rc = launch_step_kernel<KIND>(a, steps, s);
+        if (rc) return rc;
+        rollout_resolve_kernel<KIND><<<1, 1024, 0, s>>>(a);
+        FSRL_LAUNCH_CHECK();
     }
-    switch (H) {
-        case 64: GO(64) break;
-        case 128: GO(128) break;
-        case 256: GO(256) break;
-        case 512: GO(512) break;
-        default: set_error("rollout: hidden width %d unsupported (64/128/256/512)", H); return FSRL_EINVAL;
-    }
-#undef GO
     return FSRL_OK;
 }
 
@@ -537,102 +539,63 @@ int launch_norm_steps(const fsrl_rollout_t& a, const fsrl_obs_rms_t& n, int n_st
     if (rc) return rc;
     const ObsNormPass stepped{&n, a.obs_cur, a.E, OBS_SEL_STEPPED, 1, &a};
     const ObsNormPass restarted{&n, a.obs_cur, a.E, OBS_SEL_RESTARTED, 0, &a};
-#define GO(HH)                                                                                   \
-    {                                                                                            \
-        using TT = MlpTile<HH>;                                                                  \
-        const size_t smem = TT::smem_bytes(Env<KIND>::D);                                        \
-        static bool attr_done = false;                                                           \
-        if (!attr_done) {                                                                        \
-            FSRL_CUDA(cudaFuncSetAttribute(rollout_step_kernel<KIND, HH>,                        \
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-            attr_done = true;                                                                    \
-        }                                                                                        \
-        rollout_step_kernel<KIND, HH><<<(a.E + TT::R - 1) / TT::R, MLP_TPB, smem, s>>>(a, 1);    \
-        FSRL_LAUNCH_CHECK();                                                                     \
-    }
     for (int i = 0; i < n_steps; ++i) {
         if (act) {
             rollout_act_step_kernel<KIND><<<(a.E + 127) / 128, 128, 0, s>>>(a, act);
             FSRL_LAUNCH_CHECK();
-        } else {
-            switch (H) {
-                case 64: GO(64) break;
-                case 128: GO(128) break;
-                case 256: GO(256) break;
-                default: GO(512) break;
-            }
+        } else if ((rc = launch_step_kernel<KIND>(a, 1, s))) {
+            return rc;
         }
         if ((rc = launch_obs_norm(stepped, s))) return rc;
         rollout_resolve_kernel<KIND><<<1, 1024, 0, s>>>(a);
         FSRL_LAUNCH_CHECK();
         if ((rc = launch_obs_norm(restarted, s))) return rc;
     }
-#undef GO
     return FSRL_OK;
 }
 
-// Every entry point reaches a kind through these six launchers.  ROLLOUT_LAUNCHERS(extern, K) declares the
-// instantiations of kind K that another translation unit defines, ROLLOUT_LAUNCHERS(, K) defines them: the
-// Button and Push kinds are compiled in rollout_bp.cu and the velocity kinds in rollout_vel.cu, in parallel with the
-// rest of rollout.cu.
-#define ROLLOUT_LAUNCHERS(EXT, K)                                                                          \
-    EXT template int launch_env_reset_all<K>(const fsrl_rollout_t&, cudaStream_t);                         \
-    EXT template int launch_steps_h<K>(const fsrl_rollout_t&, int, bool, cudaStream_t);                    \
-    EXT template int launch_act_step<K>(const fsrl_rollout_t&, const float*, cudaStream_t);                \
-    EXT template int launch_env_step<K>(const fsrl_rollout_t&, const float*, const int32_t*, int, float*,  \
-                                        float*, float*, uint8_t*, uint8_t*, cudaStream_t);                  \
-    EXT template int launch_env_reset_ids<K>(const fsrl_rollout_t&, const int32_t*, int, float*, cudaStream_t);  \
-    EXT template int launch_norm_steps<K>(const fsrl_rollout_t&, const fsrl_obs_rms_t&, int, const float*, cudaStream_t);
+// The launcher table of kind K: Env<K>'s widths and horizon and its six launchers behind the C signatures of
+// fsrl_env_plugin_t.  Every env-dependent entry point reaches a kind through such a table (env_table(kind)): the
+// built-in kinds' tables are defined in the translation unit of their group (ENV_KINDS_*), a plugin's in
+// env_plugin.cu.
+template <int K>
+constexpr fsrl_env_plugin_t env_table() {
+    return {FSRL_ABI_VERSION, Env<K>::D, Env<K>::A, Env<K>::S, Env<K>::T, 0,
+            [](const fsrl_rollout_t* r, void* s) { return launch_env_reset_all<K>(*r, static_cast<cudaStream_t>(s)); },
+            [](const fsrl_rollout_t* r, int n_steps, int one_launch, void* s) {
+                return launch_steps_h<K>(*r, n_steps, one_launch != 0, static_cast<cudaStream_t>(s));
+            },
+            [](const fsrl_rollout_t* r, const float* act, void* s) {
+                return launch_act_step<K>(*r, act, static_cast<cudaStream_t>(s));
+            },
+            [](const fsrl_rollout_t* r, const float* act, const int32_t* ids, int n, float* obs_next, float* rew,
+               float* cost, uint8_t* term, uint8_t* trunc, void* s) {
+                return launch_env_step<K>(*r, act, ids, n, obs_next, rew, cost, term, trunc,
+                                          static_cast<cudaStream_t>(s));
+            },
+            [](const fsrl_rollout_t* r, const int32_t* ids, int n, float* obs, void* s) {
+                return launch_env_reset_ids<K>(*r, ids, n, obs, static_cast<cudaStream_t>(s));
+            },
+            [](const fsrl_rollout_t* r, const fsrl_obs_rms_t* n, int n_steps, const float* act, void* s) {
+                return launch_norm_steps<K>(*r, *n, n_steps, act, static_cast<cudaStream_t>(s));
+            }};
+}
 
-#define ROLLOUT_BP_KINDS(X, EXT)                                                           \
-    X(EXT, ENV_POINT_BUTTON1) X(EXT, ENV_POINT_BUTTON2) X(EXT, ENV_CAR_BUTTON1) X(EXT, ENV_CAR_BUTTON2) \
-    X(EXT, ENV_POINT_PUSH1) X(EXT, ENV_POINT_PUSH2) X(EXT, ENV_CAR_PUSH1) X(EXT, ENV_CAR_PUSH2)
+// `case K:` of a switch over kinds that returns kind K's table, a constant-initialized static
+#define ENV_TABLE_CASE(K)                                             \
+    case K: {                                                         \
+        static constexpr fsrl_env_plugin_t t = env_table<K>();        \
+        return &t;                                                    \
+    }
 
-#define ROLLOUT_VEL_KINDS(X, EXT)                                                                        \
-    X(EXT, ENV_HALF_CHEETAH_VEL) X(EXT, ENV_HOPPER_VEL) X(EXT, ENV_SWIMMER_VEL) X(EXT, ENV_WALKER2D_VEL) \
-    X(EXT, ENV_ANT_VEL)
-
-ROLLOUT_BP_KINDS(ROLLOUT_LAUNCHERS, extern)
-ROLLOUT_VEL_KINDS(ROLLOUT_LAUNCHERS, extern)
-
-// host: the launcher table of a registered plugin kind (fsrl_env_register, rollout.cu), NULL for any other kind
-const fsrl_env_plugin_t* env_plugin(int kind);
+// host: the table of a Button or Push kind (rollout_bp.cu), of a velocity kind (rollout_vel.cu); NULL for any other
+const fsrl_env_plugin_t* env_table_bp(int kind);
+const fsrl_env_plugin_t* env_table_vel(int kind);
+// host: the table of a built-in kind or of a registered plugin kind (rollout.cu); NULL for an unknown kind
+const fsrl_env_plugin_t* env_table(int kind);
 // host: the render launcher registered for a plugin kind (fsrl_env_register_renderer), NULL when it has none
 const fsrl_env_renderer_t* env_plugin_renderer(int kind);
+// host: the rows of a call over the envs ids[0..n) (host ids), or over all E envs in order when ids is NULL
+int check_ids(const char* fn, const fsrl_rollout_t* a, const int32_t* ids, int n);
 
 }  // namespace fsrl
-
-// a C-ABI entry point reaches kind `kind` as the compile-time constant K in CALL (used after `using namespace fsrl`)
-#define DISPATCH_KIND(kind, CALL)                                                    \
-    switch (kind) {                                                                  \
-        case ENV_CAR_CIRCLE: { constexpr int K = ENV_CAR_CIRCLE; CALL; } break;      \
-        case ENV_CAR_RUN: { constexpr int K = ENV_CAR_RUN; CALL; } break;            \
-        case ENV_BALL_CIRCLE: { constexpr int K = ENV_BALL_CIRCLE; CALL; } break;    \
-        case ENV_BALL_RUN: { constexpr int K = ENV_BALL_RUN; CALL; } break;          \
-        case ENV_ANT_CIRCLE: { constexpr int K = ENV_ANT_CIRCLE; CALL; } break;      \
-        case ENV_POINT_GOAL: { constexpr int K = ENV_POINT_GOAL; CALL; } break;      \
-        case ENV_ANT_RUN: { constexpr int K = ENV_ANT_RUN; CALL; } break;            \
-        case ENV_DRONE_CIRCLE: { constexpr int K = ENV_DRONE_CIRCLE; CALL; } break;  \
-        case ENV_DRONE_RUN: { constexpr int K = ENV_DRONE_RUN; CALL; } break;        \
-        case ENV_POINT_CIRCLE1: { constexpr int K = ENV_POINT_CIRCLE1; CALL; } break;\
-        case ENV_POINT_CIRCLE2: { constexpr int K = ENV_POINT_CIRCLE2; CALL; } break;\
-        case ENV_CAR_CIRCLE1: { constexpr int K = ENV_CAR_CIRCLE1; CALL; } break;    \
-        case ENV_CAR_CIRCLE2: { constexpr int K = ENV_CAR_CIRCLE2; CALL; } break;    \
-        case ENV_POINT_GOAL2: { constexpr int K = ENV_POINT_GOAL2; CALL; } break;    \
-        case ENV_CAR_GOAL1: { constexpr int K = ENV_CAR_GOAL1; CALL; } break;        \
-        case ENV_CAR_GOAL2: { constexpr int K = ENV_CAR_GOAL2; CALL; } break;        \
-        case ENV_POINT_BUTTON1: { constexpr int K = ENV_POINT_BUTTON1; CALL; } break;\
-        case ENV_POINT_BUTTON2: { constexpr int K = ENV_POINT_BUTTON2; CALL; } break;\
-        case ENV_CAR_BUTTON1: { constexpr int K = ENV_CAR_BUTTON1; CALL; } break;    \
-        case ENV_CAR_BUTTON2: { constexpr int K = ENV_CAR_BUTTON2; CALL; } break;    \
-        case ENV_POINT_PUSH1: { constexpr int K = ENV_POINT_PUSH1; CALL; } break;    \
-        case ENV_POINT_PUSH2: { constexpr int K = ENV_POINT_PUSH2; CALL; } break;    \
-        case ENV_CAR_PUSH1: { constexpr int K = ENV_CAR_PUSH1; CALL; } break;        \
-        case ENV_CAR_PUSH2: { constexpr int K = ENV_CAR_PUSH2; CALL; } break;        \
-        case ENV_HALF_CHEETAH_VEL: { constexpr int K = ENV_HALF_CHEETAH_VEL; CALL; } break; \
-        case ENV_HOPPER_VEL: { constexpr int K = ENV_HOPPER_VEL; CALL; } break;      \
-        case ENV_SWIMMER_VEL: { constexpr int K = ENV_SWIMMER_VEL; CALL; } break;    \
-        case ENV_WALKER2D_VEL: { constexpr int K = ENV_WALKER2D_VEL; CALL; } break;  \
-        case ENV_ANT_VEL: { constexpr int K = ENV_ANT_VEL; CALL; } break;            \
-        default: set_error("unknown env kind %d", kind); return FSRL_EINVAL;         \
-    }

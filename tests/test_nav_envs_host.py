@@ -1,6 +1,7 @@
 """The Safety-Gymnasium navigation tasks (Point / Car on Circle 1-2 and Goal 1-2) on the CPU: the registry
 and the C ABI agree with the env twin (oracle/envs_nav.py) on the dimensions, every config's default
 task resolves, and the twin's models behave as csrc/envs.cuh documents them."""
+import ctypes
 import dataclasses
 
 import numpy as np
@@ -41,11 +42,22 @@ def test_dims_agree_with_the_twin(task):
     assert (D <= 40) == (task in CIRCLES)        # Circle fits the persistent PPO launch's obs-width gate
 
 
-@pytest.mark.parametrize("kind", list(range(9, 16)) + [23, -1])
+@pytest.mark.parametrize("kind", list(range(-1, 64)) + [128])   # to FSRL_ENV_PLUGIN_FIRST, and FSRL_ENV_PLUGIN_END
 def test_unassigned_kinds_are_rejected(kind):
-    from fsrl_b200 import envs
+    """Every id below the plugin kinds: an assigned one reports its twin's widths and horizon, any other is an unknown
+    kind to the widths query, the rollout and the renderer."""
+    from fsrl_b200 import _lib, envs
+    from oracle.envs_velocity import DIMS as ALL_DIMS
+    if kind in ALL_DIMS:
+        assert envs.env_dims(kind) == ALL_DIMS[kind]
+        return
     with pytest.raises(Exception, match="unknown env kind"):
         envs.env_dims(kind)
+    r = _lib.Rollout(kind=kind, E=8)
+    assert _lib.lib.fsrl_env_reset_all(ctypes.byref(r), None) == _lib.FSRL_EINVAL
+    assert f"unknown env kind {kind}" in _lib.last_error()
+    assert _lib.lib.fsrl_env_render(ctypes.byref(r), None, 8, 64, 64, None, None, None) == _lib.FSRL_EINVAL
+    assert f"unknown env kind {kind}" in _lib.last_error()
 
 
 def test_every_config_default_task_resolves():
