@@ -330,9 +330,12 @@ __global__ void ppo_gather_kernel(const fsrl_ppo_update_t u, long long n) {
 // ------------------------------------------------------------------------------------------
 constexpr int WG_TPB = 256, WG_T = 64, WG_TKT = 32, WG_RC = 128, WG_NST = 2, WG_LD = WG_T + 8;   // LD = 8 mod 32: conflict-free fragments
 // shared memory of a weight-gradient role: WG_NST stages x (L chunk + G chunk), each [WG_RC][WG_LD]
-// (re-used as the cross-warp reduce buffer), then fin[80][WG_T] (layer-1 results) and 256 partials.
+// (re-used as the cross-warp reduce buffer), then fin[WG_FIN_ROWS][WG_T] (layer-1 results) and 256 partials.
+// The layer-1 role writes 16 rows per pass of 16 input columns (D observation columns and the bias column), so
+// fin is sized for the widest input check_update admits.
 // (64-row chunks x 3 stages, 132 KB, would let a forward CTA co-reside; the two have not been compared on H100)
-constexpr size_t WG_SMEM_FLOATS = 2 * WG_NST * (size_t)WG_RC * WG_LD + 80 * WG_T + 256;
+constexpr int WG_FIN_ROWS = 16 * ((FSRL_ENG_DX_LD + 1 + 15) / 16);
+constexpr size_t WG_SMEM_FLOATS = 2 * WG_NST * (size_t)WG_RC * WG_LD + (size_t)WG_FIN_ROWS * WG_T + 256;
 static_assert(2 * WG_NST * WG_RC * WG_LD >= 8 * 32 * (WG_T + 8), "reduce buffer must fit in the staging area");
 
 // One staged chunk of the weight-gradient contraction  C[m][n] += sum_r L[r][m] * G[r][n]
@@ -507,7 +510,7 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
                      }
                  });
         float* red = smem;                                  // staging is dead: cross-warp reduction buffer
-        float* bred = smem + 2 * WG_NST * WG_CHUNK + 80 * WG_T;      // [4][WG_T] bias partials
+        float* bred = smem + 2 * WG_NST * WG_CHUNK + WG_FIN_ROWS * WG_T;      // [4][WG_T] bias partials
         wg_store_partial<2, 8>(red, c);
         if (do_bias) bred[tid] = bpart;
         __syncthreads();
@@ -655,7 +658,7 @@ __device__ __forceinline__ void ppo_wgrad_role(const fsrl_ppo_update_t& u, int m
                      }
                  });
         float* red = smem;
-        float* cred = smem + 2 * WG_NST * WG_CHUNK + 80 * WG_T;      // [16][DOUT_LD] column-sum partials
+        float* cred = smem + 2 * WG_NST * WG_CHUNK + WG_FIN_ROWS * WG_T;      // [16][DOUT_LD] column-sum partials
         wg_store_partial<4, 2>(red, c);
         if (k0 == 0) cred[tid] = cpart;
         __syncthreads();
@@ -1015,6 +1018,7 @@ static int check_update(const fsrl_ppo_update_t* u) {
     FSRL_REQUIRE(u->H == 64 || u->H == 128 || u->H == 256 || u->H == 512, "ppo: hidden width %d unsupported", u->H);
     FSRL_REQUIRE(u->n_nets >= 1 && u->n_nets <= 3 && u->C == u->n_nets - 1, "ppo: n_nets/C inconsistent");
     FSRL_REQUIRE(u->A >= 1 && u->A <= 8, "ppo: action dim %d out of range", u->A);
+    FSRL_REQUIRE(u->D >= 1 && u->D <= FSRL_ENG_DX_LD, "ppo: observation width %d outside 1..%d", u->D, FSRL_ENG_DX_LD);
     FSRL_REQUIRE(u->theta && u->grad && u->adam_m && u->adam_v && u->w2n && u->scratch && u->norm_sq, "ppo: null buffer");
     if (u->world > 1 && u->p2p_on) {
         FSRL_REQUIRE(u->world <= FSRL_P2P_MAX_RANKS && u->p2p_rank >= 0 && u->p2p_rank < u->world && u->p2p_err && u->p2p_part,
