@@ -4,14 +4,18 @@ buffer, two FastCollectors and a trainer around a policy.  Host control code."""
 from __future__ import annotations
 
 import contextlib
+import warnings
 from abc import ABC, abstractmethod
 from typing import Optional, Tuple
+
+import torch
 
 from ..data import FastCollector, VectorReplayBuffer
 from ..envs import DeviceEnv, DeviceVectorEnv, HostVectorEnv
 from ..host_envs import is_vector_env
 from ..obs_norm import VectorEnvNormObs
 from ..trainer import OffpolicyTrainer, OnpolicyTrainer
+from ..utils.exp_util import seed_all
 from ..utils.logger import BaseLogger, DummyLogger
 
 
@@ -58,6 +62,29 @@ class BaseAgent(ABC):
     @property
     def state_dict(self):
         return self.policy.state_dict()
+
+    # shared by the presets' constructors
+    def _prologue(self, logger, cost_limit, seed: int, thread: int, device: str) -> str:
+        """Keep the logger and the cost limit, seed every RNG and set torch's host threads; returns the device
+        the networks are built on.  Runs before any network is built, as default initialisation draws from the
+        seeded generators."""
+        self.logger, self.cost_limit = logger, cost_limit
+        seed_all(seed)
+        torch.set_num_threads(thread)
+        if device == "cpu":
+            # the reference's default device; this engine has a GPU path only -- say so instead of remapping silently.
+            # stacklevel 3: the preset's caller, not the preset's constructor
+            warnings.warn("fsrl_b200 runs on CUDA devices only: device='cpu' is mapped to 'cuda'", RuntimeWarning,
+                          stacklevel=3)
+            device = "cuda"
+        return device
+
+    def _adopt_policy(self, policy, seed: int) -> None:
+        """Make ``policy`` the agent's: its networks move into the device arena and its action noise is keyed
+        by the seed."""
+        self.policy = policy
+        policy.arena
+        policy.set_action_seed(seed)
 
     # shared by both learn() flavours
     def _setup(self, train_envs, test_envs, buffer_size, reward_threshold, save_ckpt):

@@ -11,7 +11,6 @@ from torch.distributions import Independent, Normal
 from ..nets import ActorProb, Critic, Net
 from ..optim import FusedAdam
 from ..policy import CPO
-from ..utils.exp_util import seed_all
 from ..utils.logger import BaseLogger, DummyLogger
 from .base_agent import OnpolicyAgent
 from .ppo_lag_agent import init_actor_critic
@@ -30,14 +29,7 @@ class CPOAgent(OnpolicyAgent):
                  deterministic_eval: bool = True, action_scaling: bool = True,
                  action_bound_method: str = "clip", lr_scheduler=None) -> None:
         super().__init__()
-        self.logger, self.cost_limit = logger, cost_limit
-        seed_all(seed)
-        torch.set_num_threads(thread)
-        if device == "cpu":
-            # the reference's default device; this engine has a GPU path only -- say so instead of remapping silently
-            import warnings
-            warnings.warn("fsrl_b200 runs on CUDA devices only: device='cpu' is mapped to 'cuda'", RuntimeWarning, stacklevel=2)
-            device = "cuda"
+        device = self._prologue(logger, cost_limit, seed, thread, device)
         state_shape, action_shape = env.observation_space.shape, env.action_space.shape
         max_action = float(env.action_space.high[0])
         actor = ActorProb(Net(state_shape, hidden_sizes=hidden_sizes, device=device), action_shape,
@@ -45,17 +37,16 @@ class CPOAgent(OnpolicyAgent):
         critics = [Critic(Net(state_shape, hidden_sizes=hidden_sizes, device=device), device=device) for _ in range(2)]
         torch.nn.init.constant_(actor.sigma_param, -0.5)
         init_actor_critic(actor, critics, last_layer_scale)
-        self.policy = CPO(actor, critics, FusedAdam(lr=lr), lambda *l: Independent(Normal(*l), 1), logger=logger,
-                          target_kl=target_kl, backtrack_coeff=backtrack_coeff, damping_coeff=damping_coeff,
-                          max_backtracks=max_backtracks, optim_critic_iters=optim_critic_iters, l2_reg=l2_reg,
-                          gae_lambda=gae_lambda, advantage_normalization=advantage_normalization,
-                          cost_limit=cost_limit, gamma=gamma, max_batchsize=max_batchsize,
-                          reward_normalization=reward_normalization, deterministic_eval=deterministic_eval,
-                          action_scaling=action_scaling, action_bound_method=action_bound_method,
-                          observation_space=env.observation_space, action_space=env.action_space,
-                          lr_scheduler=lr_scheduler)
-        self.policy.arena
-        self.policy.set_action_seed(seed)
+        self._adopt_policy(CPO(
+            actor, critics, FusedAdam(lr=lr), lambda *l: Independent(Normal(*l), 1), logger=logger,
+            target_kl=target_kl, backtrack_coeff=backtrack_coeff, damping_coeff=damping_coeff,
+            max_backtracks=max_backtracks, optim_critic_iters=optim_critic_iters, l2_reg=l2_reg,
+            gae_lambda=gae_lambda, advantage_normalization=advantage_normalization,
+            cost_limit=cost_limit, gamma=gamma, max_batchsize=max_batchsize,
+            reward_normalization=reward_normalization, deterministic_eval=deterministic_eval,
+            action_scaling=action_scaling, action_bound_method=action_bound_method,
+            observation_space=env.observation_space, action_space=env.action_space,
+            lr_scheduler=lr_scheduler), seed)
 
     def learn(self, train_envs, test_envs=None, epoch: int = 300, episode_per_collect: int = 20,
               step_per_epoch: int = 10000, repeat_per_collect: int = 4, buffer_size: int = 100000,

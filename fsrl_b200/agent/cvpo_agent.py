@@ -12,7 +12,6 @@ from torch.distributions import Independent, Normal
 from ..nets import ActorProb, DoubleCritic, Net, SingleCritic
 from ..policy import CVPO
 from ..policy.base_policy import ActorCritic
-from ..utils.exp_util import seed_all
 from ..utils.logger import BaseLogger, DummyLogger
 from .base_agent import OffpolicyAgent
 
@@ -35,14 +34,8 @@ class CVPOAgent(OffpolicyAgent):
                  deterministic_eval: bool = True, action_scaling: bool = True, action_bound_method: str = "clip",
                  lr_scheduler: Optional[torch.optim.lr_scheduler.LambdaLR] = None) -> None:
         super().__init__()
-        self.logger, self.cost_limit = logger, cost_limit
+        device = self._prologue(logger, cost_limit, seed, thread, device)
         cost_dim = 1 if np.isscalar(cost_limit) else len(cost_limit)
-        seed_all(seed)
-        torch.set_num_threads(thread)
-        if device == "cpu":
-            import warnings
-            warnings.warn("fsrl_b200 runs on CUDA devices only: device='cpu' is mapped to 'cuda'", RuntimeWarning, stacklevel=2)
-            device = "cuda"
         state_shape, action_shape = env.observation_space.shape, env.action_space.shape
         max_action = float(env.action_space.high[0])
         assert hasattr(env.spec, "max_episode_steps"), \
@@ -71,7 +64,7 @@ class CVPOAgent(OffpolicyAgent):
                 if isinstance(m, torch.nn.Linear):
                     torch.nn.init.zeros_(m.bias)
                     m.weight.data.copy_(0.01 * m.weight.data)
-        self.policy = CVPO(
+        self._adopt_policy(CVPO(
             actor=actor, critics=critics, actor_optim=actor_optim, critic_optim=critic_optim, logger=logger,
             action_space=env.action_space, dist_fn=_dist, max_episode_steps=env.spec.max_episode_steps,
             cost_limit=cost_limit, tau=tau, gamma=gamma, n_step=n_step, estep_iter_num=estep_iter_num,
@@ -79,7 +72,5 @@ class CVPOAgent(OffpolicyAgent):
             sample_act_num=sample_act_num, mstep_iter_num=mstep_iter_num, mstep_kl_mu=mstep_kl_mu,
             mstep_kl_std=mstep_kl_std, mstep_dual_max=mstep_dual_max, mstep_dual_lr=mstep_dual_lr,
             deterministic_eval=deterministic_eval, action_scaling=action_scaling,
-            action_bound_method=action_bound_method, lr_scheduler=lr_scheduler)
-        self.policy.arena
-        self.policy.set_action_seed(seed)
+            action_bound_method=action_bound_method, lr_scheduler=lr_scheduler), seed)
         self.policy.set_update_seed(seed + 1)

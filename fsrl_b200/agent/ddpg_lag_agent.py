@@ -4,12 +4,10 @@ from __future__ import annotations
 from typing import Tuple
 
 import numpy as np
-import torch
 
 from ..nets import Actor, Critic, Net
 from ..optim import FusedAdam
 from ..policy import DDPGLagrangian, GaussianNoise
-from ..utils.exp_util import seed_all
 from ..utils.logger import BaseLogger, DummyLogger
 from .base_agent import OffpolicyAgent
 from .ppo_lag_agent import init_actor_critic
@@ -26,15 +24,8 @@ class DDPGLagAgent(OffpolicyAgent):
                  deterministic_eval: bool = True, action_scaling: bool = True,
                  action_bound_method: str = "clip", lr_scheduler=None) -> None:
         super().__init__()
-        self.logger, self.cost_limit = logger, cost_limit
+        device = self._prologue(logger, cost_limit, seed, thread, device)
         cost_dim = 1 if np.isscalar(cost_limit) else len(cost_limit)
-        seed_all(seed)
-        torch.set_num_threads(thread)
-        if device == "cpu":
-            # the reference's default device; this engine has a GPU path only -- say so instead of remapping silently
-            import warnings
-            warnings.warn("fsrl_b200 runs on CUDA devices only: device='cpu' is mapped to 'cuda'", RuntimeWarning, stacklevel=2)
-            device = "cuda"
         state_shape, action_shape = env.observation_space.shape, env.action_space.shape
         max_action = float(env.action_space.high[0])
         actor = Actor(Net(state_shape, hidden_sizes=hidden_sizes, device=device), action_shape,
@@ -42,14 +33,12 @@ class DDPGLagAgent(OffpolicyAgent):
         critics = [Critic(Net(state_shape, action_shape, hidden_sizes=hidden_sizes, concat=True, device=device),
                           device=device) for _ in range(cost_dim + 1)]
         init_actor_critic(actor, critics)
-        self.policy = DDPGLagrangian(
+        self._adopt_policy(DDPGLagrangian(
             actor=actor, critics=critics, actor_optim=FusedAdam(lr=actor_lr), critic_optim=FusedAdam(lr=critic_lr),
             logger=logger, tau=tau, exploration_noise=GaussianNoise(sigma=exploration_noise), n_step=n_step,
             use_lagrangian=use_lagrangian, lagrangian_pid=lagrangian_pid, cost_limit=cost_limit,
             rescaling=rescaling, gamma=gamma, reward_normalization=False,
             deterministic_eval=deterministic_eval, action_scaling=action_scaling,
             action_bound_method=action_bound_method, observation_space=env.observation_space,
-            action_space=env.action_space, lr_scheduler=lr_scheduler)
-        self.policy.arena
-        self.policy.set_action_seed(seed)
+            action_space=env.action_space, lr_scheduler=lr_scheduler), seed)
         self.policy.set_update_seed(seed + 1)

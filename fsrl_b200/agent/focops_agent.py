@@ -11,7 +11,6 @@ from torch.distributions import Independent, Normal
 from ..nets import ActorProb, Critic, Net
 from ..optim import FusedAdam
 from ..policy.focops import FOCOPS
-from ..utils.exp_util import seed_all
 from ..utils.logger import BaseLogger, DummyLogger
 from .base_agent import OnpolicyAgent
 from .ppo_lag_agent import init_actor_critic
@@ -31,14 +30,7 @@ class FOCOPSAgent(OnpolicyAgent):
                  deterministic_eval: bool = True, action_scaling: bool = True,
                  action_bound_method: str = "clip", lr_scheduler=None) -> None:
         super().__init__()
-        self.logger, self.cost_limit = logger, cost_limit
-        seed_all(seed)
-        torch.set_num_threads(thread)
-        if device == "cpu":
-            # the reference's default device; this engine has a GPU path only -- say so instead of remapping silently
-            import warnings
-            warnings.warn("fsrl_b200 runs on CUDA devices only: device='cpu' is mapped to 'cuda'", RuntimeWarning, stacklevel=2)
-            device = "cuda"
+        device = self._prologue(logger, cost_limit, seed, thread, device)
         state_shape, action_shape = env.observation_space.shape, env.action_space.shape
         max_action = float(env.action_space.high[0])
         actor = ActorProb(Net(state_shape, hidden_sizes=hidden_sizes, device=device), action_shape,
@@ -49,7 +41,7 @@ class FOCOPSAgent(OnpolicyAgent):
         init_actor_critic(actor, critics, last_layer_scale)
         if auto_nu:                       # the reference starts the multiplier at 0 in auto mode (:168-170)
             nu = (nu_max, nu_lr, 0.0)
-        self.policy = FOCOPS(
+        self._adopt_policy(FOCOPS(
             actor, critics, FusedAdam(lr=actor_lr), FusedAdam(lr=critic_lr),
             lambda *l: Independent(Normal(*l), 1), logger=logger, cost_limit=cost_limit, nu=nu, l2_reg=l2_reg,
             delta=delta, eta=eta, tem_lambda=tem_lambda, gae_lambda=gae_lambda, max_grad_norm=max_grad_norm,
@@ -57,6 +49,4 @@ class FOCOPSAgent(OnpolicyAgent):
             gamma=gamma, max_batchsize=max_batchsize, reward_normalization=reward_normalization,
             deterministic_eval=deterministic_eval, action_scaling=action_scaling,
             action_bound_method=action_bound_method, observation_space=env.observation_space,
-            action_space=env.action_space, lr_scheduler=lr_scheduler)
-        self.policy.arena
-        self.policy.set_action_seed(seed)
+            action_space=env.action_space, lr_scheduler=lr_scheduler), seed)

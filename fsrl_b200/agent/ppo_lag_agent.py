@@ -12,7 +12,6 @@ from torch.distributions import Independent, Normal
 from ..nets import ActorProb, Critic, Net
 from ..optim import FusedAdam
 from ..policy import PPOLagrangian
-from ..utils.exp_util import seed_all
 from ..utils.logger import BaseLogger, DummyLogger
 from .base_agent import OnpolicyAgent
 
@@ -47,16 +46,8 @@ class PPOLagAgent(OnpolicyAgent):
                  action_scaling: bool = True, action_bound_method: str = "clip",
                  lr_scheduler=None) -> None:
         super().__init__()
-        self.logger = logger
-        self.cost_limit = cost_limit
+        device = self._prologue(logger, cost_limit, seed, thread, device)
         cost_dim = 1 if np.isscalar(cost_limit) else len(cost_limit)
-        seed_all(seed)
-        torch.set_num_threads(thread)
-        if device == "cpu":
-            # the reference's default device; this engine has a GPU path only -- say so instead of remapping silently
-            import warnings
-            warnings.warn("fsrl_b200 runs on CUDA devices only: device='cpu' is mapped to 'cuda'", RuntimeWarning, stacklevel=2)
-            device = "cuda"
         state_shape = env.observation_space.shape
         action_shape = env.action_space.shape
         max_action = float(env.action_space.high[0])
@@ -71,7 +62,7 @@ class PPOLagAgent(OnpolicyAgent):
         def dist(*logits):
             return Independent(Normal(*logits), 1)
 
-        self.policy = PPOLagrangian(
+        self._adopt_policy(PPOLagrangian(
             actor, critics, optim, dist, logger=logger, target_kl=target_kl, vf_coef=vf_coef,
             max_grad_norm=max_grad_norm, gae_lambda=gae_lambda, eps_clip=eps_clip,
             dual_clip=dual_clip, value_clip=value_clip,
@@ -81,6 +72,4 @@ class PPOLagAgent(OnpolicyAgent):
             max_batchsize=max_batchsize, reward_normalization=reward_normalization,
             deterministic_eval=deterministic_eval, action_scaling=action_scaling,
             action_bound_method=action_bound_method, observation_space=env.observation_space,
-            action_space=env.action_space, lr_scheduler=lr_scheduler)
-        self.policy.arena            # move the networks into the device arena
-        self.policy.set_action_seed(seed)
+            action_space=env.action_space, lr_scheduler=lr_scheduler), seed)

@@ -9,7 +9,6 @@ import torch
 from ..nets import ActorProb, DoubleCritic, Net
 from ..optim import FusedAdam
 from ..policy import SACLagrangian
-from ..utils.exp_util import seed_all
 from ..utils.logger import BaseLogger, DummyLogger
 from .base_agent import OffpolicyAgent
 from .ppo_lag_agent import init_actor_critic
@@ -28,15 +27,8 @@ class SACLagAgent(OffpolicyAgent):
                  deterministic_eval: bool = False, action_scaling: bool = True,
                  action_bound_method: str = "clip", lr_scheduler=None) -> None:
         super().__init__()
-        self.logger, self.cost_limit = logger, cost_limit
+        device = self._prologue(logger, cost_limit, seed, thread, device)
         cost_dim = 1 if np.isscalar(cost_limit) else len(cost_limit)
-        seed_all(seed)
-        torch.set_num_threads(thread)
-        if device == "cpu":
-            # the reference's default device; this engine has a GPU path only -- say so instead of remapping silently
-            import warnings
-            warnings.warn("fsrl_b200 runs on CUDA devices only: device='cpu' is mapped to 'cuda'", RuntimeWarning, stacklevel=2)
-            device = "cuda"
         state_shape, action_shape = env.observation_space.shape, env.action_space.shape
         max_action = float(env.action_space.high[0])
         actor = ActorProb(Net(state_shape, hidden_sizes=hidden_sizes, device=device), action_shape,
@@ -50,14 +42,12 @@ class SACLagAgent(OffpolicyAgent):
         if auto_alpha:
             target_entropy = -float(np.prod(env.action_space.shape))
             a = (target_entropy, torch.zeros(1), FusedAdam(lr=alpha_lr))
-        self.policy = SACLagrangian(
+        self._adopt_policy(SACLagrangian(
             actor=actor, critics=critics, actor_optim=FusedAdam(lr=actor_lr), critic_optim=FusedAdam(lr=critic_lr),
             logger=logger, alpha=a, tau=tau, gamma=gamma, exploration_noise=None, n_step=n_step,
             use_lagrangian=use_lagrangian, lagrangian_pid=lagrangian_pid, cost_limit=cost_limit,
             rescaling=rescaling, reward_normalization=False, deterministic_eval=deterministic_eval,
             action_scaling=action_scaling, action_bound_method=action_bound_method,
             observation_space=env.observation_space, action_space=env.action_space,
-            lr_scheduler=lr_scheduler)
-        self.policy.arena
-        self.policy.set_action_seed(seed)
+            lr_scheduler=lr_scheduler), seed)
         self.policy.set_update_seed(seed + 1)

@@ -85,7 +85,7 @@ class EngineCtx:
         return x
 
     # ---- thin wrappers -----------------------------------------------------------------------------
-    def _s(self):
+    def _stream(self):
         return torch.cuda.current_stream().cuda_stream
 
     def sync_mirror(self, slots):
@@ -93,24 +93,24 @@ class EngineCtx:
         with torch.cuda.device(self.arena.device):
             for k in range(0, len(slots), 8):
                 nl = self.netlist(slots[k:k + 8])
-                _lib.check(_lib.lib.fsrl_engine_sync_mirror(ctypes.byref(e), ctypes.byref(nl), self._s()))
+                _lib.check(_lib.lib.fsrl_engine_sync_mirror(ctypes.byref(e), ctypes.byref(nl), self._stream()))
 
     def forward(self, slots, inp, B, save=False):
         e, nl = self.engine(), self.netlist(slots)
         with torch.cuda.device(self.arena.device):
-            _lib.check(_lib.lib.fsrl_engine_forward(ctypes.byref(e), ctypes.byref(nl), ctypes.byref(inp), B, int(save), self._s()))
+            _lib.check(_lib.lib.fsrl_engine_forward(ctypes.byref(e), ctypes.byref(nl), ctypes.byref(inp), B, int(save), self._stream()))
 
     def backward(self, slots, B, want_dx=False):
         e, nl = self.engine(), self.netlist(slots)
         with torch.cuda.device(self.arena.device):
-            _lib.check(_lib.lib.fsrl_engine_backward(ctypes.byref(e), ctypes.byref(nl), B, int(want_dx), self._s()))
+            _lib.check(_lib.lib.fsrl_engine_backward(ctypes.byref(e), ctypes.byref(nl), B, int(want_dx), self._stream()))
 
     def wgrad(self, slots, inp, B, accumulate=False, norm_sq: Optional[torch.Tensor] = None):
         e, nl = self.engine(), self.netlist(slots)
         with torch.cuda.device(self.arena.device):
             _lib.check(_lib.lib.fsrl_engine_wgrad(ctypes.byref(e), ctypes.byref(nl), ctypes.byref(inp), B,
                                                   int(accumulate), None if norm_sq is None else norm_sq.data_ptr(),
-                                                  self._s()))
+                                                  self._stream()))
 
     def adam(self, slots, lr, step, betas=(0.9, 0.999), eps=1e-8, grad_scale=1.0, l2_reg=0.0,
              norm_sq: Optional[torch.Tensor] = None, max_grad_norm=0.0):
@@ -119,9 +119,9 @@ class EngineCtx:
             _lib.check(_lib.lib.fsrl_engine_adam(ctypes.byref(e), ctypes.byref(nl), lr, betas[0], betas[1], eps,
                                                  int(step), grad_scale, l2_reg,
                                                  None if norm_sq is None else norm_sq.data_ptr(),
-                                                 float(max_grad_norm or 0.0), self._s()))
+                                                 float(max_grad_norm or 0.0), self._stream()))
 
     def polyak(self, dst, src, tau):
         e, d, s = self.engine(), self.netlist(dst), self.netlist(src)
         with torch.cuda.device(self.arena.device):
-            _lib.check(_lib.lib.fsrl_engine_polyak(ctypes.byref(e), ctypes.byref(d), ctypes.byref(s), float(tau), self._s()))
+            _lib.check(_lib.lib.fsrl_engine_polyak(ctypes.byref(e), ctypes.byref(d), ctypes.byref(s), float(tau), self._stream()))

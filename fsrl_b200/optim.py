@@ -14,6 +14,16 @@ class FusedAdam:
         self.m = None
         self.v = None
 
+    @classmethod
+    def from_optimizer(cls, opt) -> "FusedAdam":
+        """``opt`` itself if it is a FusedAdam; otherwise a FusedAdam with the lr, betas and eps of its first
+        parameter group, so that a ``torch.optim.Adam`` built by reference-style agent code keeps its
+        hyper-parameters while the update runs in the fused kernel."""
+        if isinstance(opt, FusedAdam):
+            return opt
+        g = opt.param_groups[0]
+        return cls(lr=g["lr"], betas=g.get("betas", (0.9, 0.999)), eps=g.get("eps", 1e-8))
+
     @property
     def lr(self):
         return self.param_groups[0]["lr"]

@@ -95,6 +95,7 @@ class BasePolicy(ABC, nn.Module):
         self.action_bound_method = action_bound_method
         self.lr_scheduler = lr_scheduler
         self.gradient_steps = 0
+        self.last_stats: Dict[str, Any] = {}
         self._arena: Optional[Arena] = None
 
     # ---- arena ------------------------------------------------------------------------------------
@@ -207,6 +208,27 @@ class BasePolicy(ABC, nn.Module):
     def set_action_seed(self, seed: int) -> None:
         """Key of the Philox action-noise stream (documented RNG; oracle/philox.py)."""
         self._act_seed = int(seed)
+
+    # ---- learner plumbing ----------------------------------------------------------------------------
+    def _expand_cost_limit(self, cost_limit) -> list:
+        """One limit per cost critic: a scalar applies to every cost stream."""
+        return [cost_limit] * (self.critics_num - 1) if np.isscalar(cost_limit) else cost_limit
+
+    def _record(self, stats: Dict[str, float]) -> None:
+        """One gradient step's ``tab/key`` scalars: appended to ``last_stats`` and stored in the logger, in
+        the dict's order."""
+        for k, v in stats.items():
+            self.last_stats.setdefault(k, []).append(v)
+            tab, key = k.split("/", 1)
+            self.logger.store(tab, **{key: v})
+
+    def _record_many(self, out: Dict[str, np.ndarray]) -> None:
+        """Columns of per-step ``tab/key`` values from one device->host copy: they become ``last_stats`` and are
+        stored in the logger, in the dict's order."""
+        self.last_stats = out
+        for k, v in out.items():
+            tab, key = k.split("/", 1)
+            self.logger.store_many(tab, key, v)
 
     # ---- reference hooks -----------------------------------------------------------------------------
     def forward(self, batch: Batch, state=None, **kwargs: Any) -> Batch:

@@ -38,10 +38,7 @@ class CPO(TrustRegionMixin, BasePolicy):
         super().__init__(actor, critics, dist_fn, logger, gamma, max_batchsize, reward_normalization,
                          deterministic_eval, action_scaling, action_bound_method, observation_space,
                          action_space, lr_scheduler)
-        if not isinstance(optim, FusedAdam):
-            g = optim.param_groups[0]
-            optim = FusedAdam(lr=g["lr"], betas=g.get("betas", (0.9, 0.999)), eps=g.get("eps", 1e-8))
-        self.optim = optim
+        self.optim = FusedAdam.from_optimizer(optim)
         self._cost_limit = cost_limit
         self._lambda = gae_lambda
         self._norm_adv = advantage_normalization
@@ -57,30 +54,26 @@ class CPO(TrustRegionMixin, BasePolicy):
         self._eng: Optional[EngineCtx] = None
         self._critic_t = 0
         self._ave_cost_return = 0.0
-        self.last_stats: Dict[str, list] = {}
 
     def pre_update_fn(self, stats_train: Dict, **kwarg) -> Any:
         self._ave_cost_return = stats_train["cost"]
 
     def update_cost_limit(self, cost_limit: float) -> None:
         # reference quirk (SURVEY.md App. A.12): writes `cost_limit`, the algorithm reads `_cost_limit`
-        self.cost_limit = [cost_limit] * (self.critics_num - 1) if np.isscalar(cost_limit) else cost_limit
+        self.cost_limit = self._expand_cost_limit(cost_limit)
 
     def process_fn(self, batch, buffer, indices) -> DeviceBatch:
         batch = self.compute_gae_returns(batch, buffer, indices, self._lambda)          # :126
         if self._norm_adv:                                                             # :127-131
             for c in range(self.critics_num):
                 self._standardize(batch.adv[c], batch.n)
-        # old distribution (:133-144): mean from one actor pass; std is state independent
-        z = self.net_forward(0, batch.obs)
-        mu = self.actor._max * torch.tanh(z) if not self.actor._unbounded else z
-        batch.mean_old = mu.contiguous()
-        batch.std_old = self.actor.sigma_param.detach().view(1, -1).exp().expand_as(mu).contiguous()
+        mu, std = self._old_dist(batch.obs)                                             # :133-144
+        batch.mean_old, batch.std_old = mu.contiguous(), std.contiguous()
         return batch
 
     # ---- policy step (:234-351) ----------------------------------------------------------------------------------
     def policy_loss(self, batch: DeviceBatch, perm: Optional[torch.Tensor], n: int) -> dict:
-        eng, lib, s = self._eng, _lib.lib, self._s()
+        eng, lib, s = self._eng, _lib.lib, self._stream()
         a = self.arena.slots[0]
         P = a.size
         v = self._vec
@@ -103,7 +96,7 @@ class CPO(TrustRegionMixin, BasePolicy):
             return sm
 
         # entropy of the state-independent Gaussian BEFORE the step (:239)
-        ent = float((0.5 + 0.5 * np.log(2 * np.pi) + self.actor.sigma_param.detach().flatten()).sum().item())
+        ent = self._entropy()
         eng.forward([a], inp, n, save=True)
         sm = grad_into(1, v["g"])                                                   # :252
         adv_c = batch.adv[1] if perm is None else batch.adv[1][perm.long()]
@@ -196,24 +189,12 @@ class CPO(TrustRegionMixin, BasePolicy):
         self.last_stats = {}
         with torch.cuda.device(self.device):
             for _ in range(repeat):
-                # Batch.split(batch_size, shuffle=True, merge_last=True): np.random.permutation
-                perm_all = np.random.permutation(n_all)
-                merge_last = n_all % batch_size > 0
-                chunks = []
-                for i in range(0, n_all, batch_size):
-                    if merge_last and i + 2 * batch_size >= n_all:
-                        chunks.append(perm_all[i:]); break
-                    chunks.append(perm_all[i:i + batch_size])
-                self._dp_same_count(len(chunks), "minibatch count")
-                for ch in chunks:
-                    perm = torch.as_tensor(ch.astype(np.int32), device=self.device)
-                    n = len(ch)
+                minibatches = self._minibatches(n_all, batch_size)
+                self._dp_same_count(len(minibatches), "minibatch count")
+                for perm, n in minibatches:
                     for _ in range(self._optim_critic_iters):                        # :360-361
                         stats_critic = self.critics_loss(batch, perm, n)
                     stats_actor = self.policy_loss(batch, perm, n)                   # :364
                     self.gradient_steps += 1
-                    for k, val in {**stats_actor, **stats_critic}.items():
-                        self.last_stats.setdefault(k, []).append(val)
-                        tab, key = k.split("/", 1)
-                        self.logger.store(tab, **{key: val})
+                    self._record({**stats_actor, **stats_critic})
         self.logger.store(gradient_steps=self.gradient_steps, tab="update")

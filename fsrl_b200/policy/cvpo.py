@@ -144,7 +144,7 @@ class CVPO(OffPolicyEngine):
         return {"lr": self._mstep_dual_lr, "exp_avg": ms[2:4], "exp_avg_sq": ms[4:6], "step": ms[6:7]}
 
     def update_cost_limit(self, cost_limit) -> None:
-        self.cost_limit = [cost_limit] * (self.critics_num - 1) if np.isscalar(cost_limit) else cost_limit
+        self.cost_limit = self._expand_cost_limit(cost_limit)
         T = self.max_episode_steps
         self.qc_thres = [c * (1 - self._gamma ** T) / (1 - self._gamma) / T for c in self.cost_limit]
 
@@ -230,7 +230,4 @@ class CVPO(OffPolicyEngine):
         for k, col in (("mstep_kl_mu", 7), ("mstep_kl_std", 8), ("mstep_loss_kl", 9), ("mstep_loss_mle", 10),
                        ("mstep_loss_total", 11), ("mstep_dual_mu", 12), ("mstep_dual_std", 13), ("entropy", 14)):
             out["mstep/" + k] = st[:, col]
-        self.last_stats = out
-        for k, v in out.items():
-            tab, key = k.split("/", 1)
-            self.logger.store_many(tab, key, v)
+        self._record_many(out)

@@ -3,7 +3,7 @@
 
 process_fn (:135-155): dual GAE + the old log-prob / mean / std of the collecting policy.
 learn (:217-251): one dual step on nu (:157-162), then per repeat and per minibatch of
-``Batch.split(batch_size, merge_last=True)`` a critic regression step (MSE + L2 over the critic
+tianshou's ``Batch.split`` a critic regression step (MSE + L2 over the critic
 parameters, :164-180) and an actor step (:182-215) on
 
     mean( (KL(new || old) - ratio (A_r - nu A_c) / lambda) * 1[KL <= eta] )
@@ -28,13 +28,6 @@ from .base_policy import BasePolicy, DeviceBatch
 from .trust_region import TrustRegionMixin
 
 
-def _fused(optim) -> FusedAdam:
-    if isinstance(optim, FusedAdam):
-        return optim
-    g = optim.param_groups[0]
-    return FusedAdam(lr=g["lr"], betas=g.get("betas", (0.9, 0.999)), eps=g.get("eps", 1e-8))
-
-
 class FOCOPS(TrustRegionMixin, BasePolicy):
     def __init__(self, actor, critics, actor_optim, critic_optim, dist_fn=None,
                  logger: BaseLogger = DummyLogger(), cost_limit: float = 10,
@@ -48,8 +41,8 @@ class FOCOPS(TrustRegionMixin, BasePolicy):
         super().__init__(actor, critics, dist_fn, logger, gamma, max_batchsize, reward_normalization,
                          deterministic_eval, action_scaling, action_bound_method, observation_space,
                          action_space, lr_scheduler)
-        self.actor_optim = _fused(actor_optim)
-        self.critics_optim = _fused(critic_optim)
+        self.actor_optim = FusedAdam.from_optimizer(actor_optim)
+        self.critics_optim = FusedAdam.from_optimizer(critic_optim)
         self.optim = self.critics_optim              # TrustRegionMixin.critics_loss steps this one
         self.cost_limit = cost_limit
         self._gae_lambda = gae_lambda
@@ -72,22 +65,19 @@ class FOCOPS(TrustRegionMixin, BasePolicy):
         self._actor_t = 0
         self._ave_cost_return = 0.0
         self._norm_sq: Optional[torch.Tensor] = None
-        self.last_stats: Dict[str, list] = {}
 
     def pre_update_fn(self, stats_train: Dict, **kwarg) -> Any:
         self._ave_cost_return = stats_train["cost"]
 
     def update_cost_limit(self, cost_limit: float) -> None:
-        self.cost_limit = [cost_limit] * (self.critics_num - 1) if np.isscalar(cost_limit) else cost_limit
+        self.cost_limit = self._expand_cost_limit(cost_limit)
 
     def process_fn(self, batch, buffer, indices) -> DeviceBatch:
         if self._recompute_adv:
             self._buffer, self._indices = buffer, indices
         batch = self.compute_gae_returns(batch, buffer, indices, self._gae_lambda)       # :143
-        z = self.net_forward(0, batch.obs)                                              # :146-152
-        mu = self.actor._max * torch.tanh(z) if not self.actor._unbounded else z
-        batch.mean_old = mu.contiguous()
-        batch.std_old = self.actor.sigma_param.detach().view(1, -1).exp().expand_as(mu).contiguous()
+        mu, std = self._old_dist(batch.obs)                                             # :146-152
+        batch.mean_old, batch.std_old = mu.contiguous(), std.contiguous()
         return batch
 
     def nu_loss(self) -> dict:
@@ -111,9 +101,9 @@ class FOCOPS(TrustRegionMixin, BasePolicy):
         return self._adv_n
 
     def policy_loss(self, batch: DeviceBatch, perm: torch.Tensor, n: int) -> dict:
-        eng, lib, s = self._eng, _lib.lib, self._s()
+        eng, lib, s = self._eng, _lib.lib, self._stream()
         a = self.arena.slots[0]
-        ent = float((0.5 + 0.5 * np.log(2 * np.pi) + self.actor.sigma_param.detach().flatten()).sum().item())
+        ent = self._entropy()
         adv_n = self._normalised_adv(batch, perm)
         d = self._descriptor(batch, perm, n)
         d.adv = adv_n.data_ptr()
@@ -144,26 +134,14 @@ class FOCOPS(TrustRegionMixin, BasePolicy):
             for step in range(repeat):
                 if self._recompute_adv and step > 0:                                    # :224-227
                     batch = self.compute_gae_returns(batch, self._buffer, self._indices, self._gae_lambda)
-                perm_all = np.random.permutation(n_all)       # Batch.split(batch_size, merge_last=True)
-                merge_last = n_all % batch_size > 0
-                chunks = []
-                for i in range(0, n_all, batch_size):
-                    if merge_last and i + 2 * batch_size >= n_all:
-                        chunks.append(perm_all[i:]); break
-                    chunks.append(perm_all[i:i + batch_size])
                 iter_counts, approx_kl = 0, 0.0
-                for ch in chunks:
-                    perm = torch.as_tensor(ch.astype(np.int32), device=self.device)
-                    n = len(ch)
+                for perm, n in self._minibatches(n_all, batch_size):
                     stats_critic = self.critics_loss(batch, perm, n)                    # :231
                     stats_actor = self.policy_loss(batch, perm, n)                      # :234
                     approx_kl += stats_actor["loss/kl"]
                     iter_counts += 1
                     self.gradient_steps += 1
-                    for k, val in {**stats_nu, **stats_actor, **stats_critic}.items():
-                        self.last_stats.setdefault(k, []).append(val)
-                        tab, key = k.split("/", 1)
-                        self.logger.store(tab, **{key: val})
+                    self._record({**stats_nu, **stats_actor, **stats_critic})
                 approx_kl /= iter_counts + 1e-7                                         # :246
                 if approx_kl > self._delta:
                     self.logger.print("Early stop at step %d due to reaching max kl." % step)

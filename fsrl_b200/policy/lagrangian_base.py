@@ -27,7 +27,7 @@ class LagrangianPolicy(BasePolicy):
                          action_bound_method, observation_space, action_space, lr_scheduler)
         self.rescaling = rescaling
         self.use_lagrangian = use_lagrangian
-        self.cost_limit = [cost_limit] * (self.critics_num - 1) if np.isscalar(cost_limit) else cost_limit
+        self.cost_limit = self._expand_cost_limit(cost_limit)
         if self.use_lagrangian:
             assert len(self.cost_limit) == (self.critics_num - 1), \
                 "cost_limit must has equal len of critics_num"
@@ -39,7 +39,7 @@ class LagrangianPolicy(BasePolicy):
         self.update_lagrangian(stats_train["cost"])
 
     def update_cost_limit(self, cost_limit: float) -> None:
-        self.cost_limit = [cost_limit] * (self.critics_num - 1) if np.isscalar(cost_limit) else cost_limit
+        self.cost_limit = self._expand_cost_limit(cost_limit)
 
     def update_lagrangian(self, cost_values: Union[List, float]) -> None:
         if np.isscalar(cost_values):

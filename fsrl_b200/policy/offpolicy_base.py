@@ -11,7 +11,7 @@ from __future__ import annotations
 
 import ctypes
 from copy import deepcopy
-from typing import Any, Dict, List, Optional
+from typing import Any, List, Optional
 
 import numpy as np
 import torch
@@ -37,7 +37,6 @@ class OffPolicyEngine(BasePolicy):
         self._actor_t = 0
         self._noise_t = 0
         self._upd_seed = 0
-        self.last_stats: Dict[str, np.ndarray] = {}
 
     def set_update_seed(self, seed: int) -> None:
         self._upd_seed = int(seed) & 0xFFFFFFFF
@@ -256,10 +255,7 @@ class OffPolicyLagrangian(OffPolicyEngine, LagrangianPolicy):
             out["loss/lagrangian"] = np.full(len(st), self.lagrangians()[0])
             out["loss/actor_safety"] = st[:, 3]
         self._extra_stats(out, st)
-        self.last_stats = out
-        for k, v in out.items():
-            tab, key = k.split("/", 1)
-            self.logger.store_many(tab, key, v)
+        self._record_many(out)
 
     def _extra_stats(self, out, st):
         pass

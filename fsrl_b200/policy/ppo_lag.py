@@ -40,12 +40,7 @@ class PPOLagrangian(LagrangianPolicy):
                          cost_limit, rescaling, gamma, max_batchsize, reward_normalization,
                          deterministic_eval, action_scaling, action_bound_method,
                          observation_space, action_space, lr_scheduler)
-        if not isinstance(optim, FusedAdam):
-            # accept a torch.optim.Adam built by reference-style agent code: keep its
-            # hyper-parameters, run the update with the fused kernel
-            g = optim.param_groups[0]
-            optim = FusedAdam(lr=g["lr"], betas=g.get("betas", (0.9, 0.999)), eps=g.get("eps", 1e-8))
-        self.optim = optim
+        self.optim = FusedAdam.from_optimizer(optim)
         self._lambda = gae_lambda
         self._weight_vf = vf_coef
         self._grad_norm = max_grad_norm
@@ -66,7 +61,6 @@ class PPOLagrangian(LagrangianPolicy):
         self._scratch = None
         self._bmax = 0
         self._stats_dev = None
-        self.last_stats: Dict[str, np.ndarray] = {}
 
     # -----------------------------------------------------------------------------------------------
     def _ensure_update_state(self, batch_size: int, n_total: int, repeat: int):
@@ -321,7 +315,4 @@ class PPOLagrangian(LagrangianPolicy):
         if self.use_lagrangian and self.critics_num > 1:
             out["loss/lagrangian"] = np.full(len(st), float(u.lagrangian))
             out["loss/actor_safety"] = actor_saf
-        self.last_stats = out
-        for k, v in out.items():
-            tab, key = k.split("/", 1)
-            self.logger.store_many(tab, key, v)
+        self._record_many(out)

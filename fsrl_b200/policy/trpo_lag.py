@@ -34,10 +34,7 @@ class TRPOLagrangian(TrustRegionMixin, LagrangianPolicy):
         super().__init__(actor, critics, dist_fn, logger, use_lagrangian, lagrangian_pid, cost_limit,
                          rescaling, gamma, max_batchsize, reward_normalization, deterministic_eval,
                          action_scaling, action_bound_method, observation_space, action_space, lr_scheduler)
-        if not isinstance(optim, FusedAdam):
-            g = optim.param_groups[0]
-            optim = FusedAdam(lr=g["lr"], betas=g.get("betas", (0.9, 0.999)), eps=g.get("eps", 1e-8))
-        self.optim = optim
+        self.optim = FusedAdam.from_optimizer(optim)
         self._lambda = gae_lambda
         self._norm_adv = advantage_normalization
         self._max_backtracks = max_backtracks
@@ -49,7 +46,6 @@ class TRPOLagrangian(TrustRegionMixin, LagrangianPolicy):
         if not isinstance(actor, ActorProb) or actor._c_sigma:
             raise TypeError("TRPOLagrangian needs a state-independent-sigma ActorProb")
         assert self.critics_num == 2
-        self.last_stats: Dict[str, list] = {}
 
     def process_fn(self, batch, buffer, indices) -> DeviceBatch:
         batch = self.compute_gae_returns(batch, buffer, indices, self._lambda)
@@ -62,10 +58,9 @@ class TRPOLagrangian(TrustRegionMixin, LagrangianPolicy):
 
     def _refresh_old_dist(self, batch: DeviceBatch) -> None:
         """old_dist = self(minibatch).dist under no_grad at the CURRENT parameters (:189-190)."""
-        z = self.net_forward(0, batch.obs)
-        mu = self.actor._max * torch.tanh(z) if not self.actor._unbounded else z
+        mu, std = self._old_dist(batch.obs)
         batch.mean_old.copy_(mu)
-        batch.std_old.copy_(self.actor.sigma_param.detach().view(1, -1).exp().expand_as(mu))
+        batch.std_old.copy_(std)
 
     def learn(self, batch: DeviceBatch, batch_size: int, repeat: int, **kwargs: Any) -> Dict[str, List[float]]:
         n_all = batch.n
@@ -76,19 +71,11 @@ class TRPOLagrangian(TrustRegionMixin, LagrangianPolicy):
         self.last_stats = {}
         theta_a = self.arena.theta[a.offset:a.offset + P]
         with torch.cuda.device(self.device):
-            s = self._s()
+            s = self._stream()
             for _ in range(repeat):
-                perm_all = np.random.permutation(n_all)
-                merge_last = n_all % batch_size > 0
-                chunks = []
-                for i in range(0, n_all, batch_size):
-                    if merge_last and i + 2 * batch_size >= n_all:
-                        chunks.append(perm_all[i:]); break
-                    chunks.append(perm_all[i:i + batch_size])
-                self._dp_same_count(len(chunks), "minibatch count")
-                for ch in chunks:
-                    perm = torch.as_tensor(ch.astype(np.int32), device=self.device)
-                    n = len(ch)
+                minibatches = self._minibatches(n_all, batch_size)
+                self._dp_same_count(len(minibatches), "minibatch count")
+                for perm, n in minibatches:
                     lag = self.lagrangians()[0] if (self.use_lagrangian and self.lag_optims) else 0.0
                     resc = self.rescaling_factor() if self.use_lagrangian else 1.0
                     self._refresh_old_dist(batch)
@@ -144,15 +131,11 @@ class TRPOLagrangian(TrustRegionMixin, LagrangianPolicy):
                     for _ in range(self._optim_critic_iters):                 # :233-238
                         stats_critic = self.critics_loss(batch, perm, n)
                         self.gradient_steps += 1
-                    ent = float((0.5 + 0.5 * np.log(2 * np.pi) + self.actor.sigma_param.detach().flatten()).sum().item())
                     stats = {"loss/actor_rew": float(-(sm[0] / n_g)), "loss/actor_total": float(loss_actor),
                              "loss/rescaling": resc, "loss/kl": kl, "loss/step_size": step_size,
-                             "loss/entropy": ent, **stats_critic}
+                             "loss/entropy": self._entropy(), **stats_critic}
                     if self.use_lagrangian:
                         stats["loss/lagrangian"] = lag
                         stats["loss/actor_safety"] = float(lag * sm[1] / n_g)
-                    for k, val in stats.items():
-                        self.last_stats.setdefault(k, []).append(val)
-                        tab, key = k.split("/", 1)
-                        self.logger.store(tab, **{key: val})
+                    self._record(stats)
         self.logger.store(gradient_steps=self.gradient_steps, tab="update")

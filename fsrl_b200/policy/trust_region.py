@@ -4,7 +4,7 @@ engine context, head-gradient / Hessian-vector-product calls (csrc/cpo.cu), conj
 from __future__ import annotations
 
 import ctypes
-from typing import Optional
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -83,12 +83,34 @@ class TrustRegionMixin:
                 raise RuntimeError(f"data-parallel {what}: ranks disagree ({int(-lo_hi[1])}..{int(lo_hi[0])}); "
                                    "use batch_size >= the per-rank collect size")
 
-    # ---- device helpers -----------------------------------------------------------------------------------
-    def _s(self):
-        return torch.cuda.current_stream().cuda_stream
+    # ---- minibatches and the state-independent Gaussian ------------------------------------------------------
+    def _minibatches(self, n_all: int, batch_size: int) -> List[Tuple[torch.Tensor, int]]:
+        """tianshou's ``Batch.split(batch_size, shuffle=True, merge_last=True)`` over n_all rows: one
+        ``np.random.permutation`` drawn from NumPy's global stream, cut into chunks of batch_size rows, the last
+        full chunk absorbing a short tail.  Each chunk as (device int32 row indices, row count)."""
+        perm_all = np.random.permutation(n_all)
+        merge_last = n_all % batch_size > 0
+        chunks = []
+        for i in range(0, n_all, batch_size):
+            if merge_last and i + 2 * batch_size >= n_all:
+                chunks.append(perm_all[i:]); break
+            chunks.append(perm_all[i:i + batch_size])
+        return [(torch.as_tensor(ch.astype(np.int32), device=self.device), len(ch)) for ch in chunks]
 
+    def _old_dist(self, obs: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(mean, std) of the actor's Gaussian at the current parameters: the mean from one actor pass, squashed
+        to max_action * tanh unless unbounded; the state-independent std broadcast over the rows."""
+        z = self.net_forward(0, obs)
+        mu = self.actor._max * torch.tanh(z) if not self.actor._unbounded else z
+        return mu, self.actor.sigma_param.detach().view(1, -1).exp().expand_as(mu)
+
+    def _entropy(self) -> float:
+        """Entropy of the state-independent Gaussian: sum over actions of 1/2 + log(2 pi)/2 + log sigma."""
+        return float((0.5 + 0.5 * np.log(2 * np.pi) + self.actor.sigma_param.detach().flatten()).sum().item())
+
+    # ---- device helpers -----------------------------------------------------------------------------------
     def _dotp(self, a, b) -> float:
-        _lib.check(_lib.lib.fsrl_vec_dot(a.data_ptr(), b.data_ptr(), a.numel(), self._dot.data_ptr(), self._s()))
+        _lib.check(_lib.lib.fsrl_vec_dot(a.data_ptr(), b.data_ptr(), a.numel(), self._dot.data_ptr(), self._stream()))
         return float(self._dot.item())
 
     def _descriptor(self, batch: DeviceBatch, perm: Optional[torch.Tensor], n: int) -> "_lib.Cpo":
@@ -111,11 +133,11 @@ class TrustRegionMixin:
         return d
 
     def _head(self, d, mode: int):
-        _lib.check(_lib.lib.fsrl_cpo_head(ctypes.byref(d), mode, self._sums.data_ptr(), self._s()))
+        _lib.check(_lib.lib.fsrl_cpo_head(ctypes.byref(d), mode, self._sums.data_ptr(), self._stream()))
 
     def _hvp(self, d, v, out):
         _lib.check(_lib.lib.fsrl_cpo_hvp(ctypes.byref(d), v.data_ptr(), self._v_w2n.data_ptr(), out.data_ptr(),
-                                         float(self._damping_coeff), self._s()))
+                                         float(self._damping_coeff), self._stream()))
         self._gvec(out)      # H = sum_r w_r H_r (the damping term carries through: sum_r w_r = 1)
 
     def _cg(self, d, rhs: torch.Tensor, out: torch.Tensor, nsteps: int = 10, residual_tol: float = 1e-8):
@@ -130,12 +152,12 @@ class TrustRegionMixin:
                 self._cg_state = torch.zeros(8, dtype=torch.float64, device=rhs.device)
             _lib.check(_lib.lib.fsrl_cg_solve(ctypes.byref(d), rhs.data_ptr(), out.data_ptr(), self._cg_work.data_ptr(),
                                               self._v_w2n.data_ptr(), self._cg_state.data_ptr(), n, int(nsteps),
-                                              float(residual_tol), float(self._damping_coeff), self._s()))
+                                              float(residual_tol), float(self._damping_coeff), self._stream()))
             return
         x, r, p, z = v["x"], v["r"], v["p"], v["z"]
         x.zero_(); r.copy_(rhs); p.copy_(rhs)
         rs_old = self._dotp(r, r)
-        lib, s, n = _lib.lib, self._s(), rhs.numel()
+        lib, s, n = _lib.lib, self._stream(), rhs.numel()
         for _ in range(nsteps):
             self._hvp(d, p, z)
             alpha = rs_old / self._dotp(p, z)
@@ -160,7 +182,7 @@ class TrustRegionMixin:
             self._sums.zero_()
             _lib.check(_lib.lib.fsrl_mse_head(eng.slot_view(s, "out").data_ptr(), batch.ret[i].data_ptr(),
                                               None if perm is None else perm.data_ptr(), n,
-                                              eng.slot_view(s, "dout").data_ptr(), self._sums.data_ptr(), self._s()))
+                                              eng.slot_view(s, "dout").data_ptr(), self._sums.data_ptr(), self._stream()))
             th = self.arena.theta[s.offset:s.offset + s.size]
             reg = (self._dotp(th, th) * self._l2_reg) if self._l2_reg else 0.0
             stats["loss/vf" + str(i)] = self._gscalar(float(self._sums[0].item())) / n_g + reg
