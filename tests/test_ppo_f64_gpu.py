@@ -19,6 +19,9 @@ The persistent launch (csrc/ppo_persist.cu) writes no scratch: its gradient, sta
 against the float64 update of the whole minibatch.  With Adam's betas at 0 the first moment after any step is that
 step's (clipped) gradient and v = m^2, so theta before the last step follows from theta, m and v after it.
 
+Long launches (thousands of steps, on both paths) run at lr = 0, which keeps theta fixed, so that every step is the
+float64 update of its own minibatch at theta0 (section 6).
+
 Every bound is a tolerance times a measured scale: the same expression evaluated on the magnitudes of its terms.
 The synthetic batches put the ratio exp(logp - logp_old) on both sides of the clip range and of the dual clip, and the
 stored values on both sides of the value clip, each a clear margin away from the kink; the head stage asserts that
@@ -27,6 +30,7 @@ misplaced row moves the weight gradient far past its bound."""
 import copy
 import ctypes
 import math
+import time
 
 import numpy as np
 import pytest
@@ -46,12 +50,15 @@ FWD_TOL = 7e-6       # h1, h2 against float64 with device masks, relative to the
 DOUT_TOL = 3e-5      # head dout, relative to the element's magnitude: 2.4e-6
 BWD_TOL = 3e-5       # dz2, dz1 from the device's dout / dz2, relative to the magnitude of the product: 3.2e-6
 GRAD_TOL = 9e-6      # weight gradients from the device's activations, relative to |X|^T |G|: 8.6e-7
-NORM_TOL = 6e-6      # loss/grad_norm, relative to the norm of |X|^T |G| (chain) or to itself (persistent): 6.2e-7
+NORM_TOL = 6e-6      # loss/grad_norm, relative to the norm of |X|^T |G| (chain) or to itself (persistent): 6.2e-7,
+                     # 1.3e-6 over the 16384 steps of the long launch at D = 40
 STAT_TOL = 8e-6      # statistics, relative to the sum of the magnitudes of their terms: 7.8e-7
 PGRAD_TOL = 3e-6     # persistent launch: max |g - g64| / max |X|^T |G| per parameter group, natural masks: 2.2e-7
 ULP_TOL = 32.0       # Adam's theta and v in fp32 ulps of their scale: 3.2
 GAE_TOL = 5e-7       # recomputed advantages / returns, relative to the largest value, return and reward: 4.5e-8
 KINK = 1e-3          # the float64 ratio / value offset is at least this far from every kink it can meet
+M_TOL = 6e-7         # long launches: Adam's m, relative to the recurrence run on the per-group gradient scales: 6.3e-8
+V_TOL = 9e-7         # long launches: Adam's v, likewise on the squared scales: 9.4e-8
 
 
 class _BoxEnv:
@@ -63,7 +70,7 @@ class _BoxEnv:
         self.action_space = Box(-high, high, (A,), np.float32)
 
 
-def _policy(D, A, H, C=2, high=1.0, bounded=True, lag=0.7, betas=None, persist=False, seed=3, **kw):
+def _policy(D, A, H, C=2, high=1.0, bounded=True, lag=0.7, betas=None, lr=LR, persist=False, seed=3, **kw):
     if C == 2:
         from fsrl_b200.agent import PPOLagAgent
         p = PPOLagAgent(_BoxEnv(D, A, high), seed=seed, hidden_sizes=(H, H), unbounded=not bounded, lr=LR,
@@ -86,9 +93,9 @@ def _policy(D, A, H, C=2, high=1.0, bounded=True, lag=0.7, betas=None, persist=F
         p = PPOLagrangian(actor, critics, FusedAdam(lr=LR), lambda *l: Independent(Normal(*l), 1),
                           observation_space=env.observation_space, action_space=env.action_space, **kw)
         p.arena
-    if betas is not None:
+    if betas is not None or lr != LR:
         from fsrl_b200.optim import FusedAdam
-        p.optim = FusedAdam(lr=LR, betas=betas)
+        p.optim = FusedAdam(lr=lr, betas=betas or p.optim.param_groups[0]["betas"])
     p._persist_off = not persist
     p._target_kl = 1e9
     assert p.actor._max == high and p.actor._unbounded == (not bounded)
@@ -133,10 +140,30 @@ def _bands(bands, n, g):
     return lo + (hi - lo) * torch.rand(n, generator=g, device="cuda", dtype=torch.float64)
 
 
-def _batch(p, n, seed, trap_rows=()):
+ROW_CHUNK = 1 << 17     # rows per float64 pass over a whole batch
+
+
+def _relu_clearance(nets, x):
+    """per row, the least |z| / (its magnitude chain) over the layer-1 and layer-2 pre-activations of every net"""
+    out = []
+    for xc in x.split(ROW_CHUNK):
+        c = torch.full(xc.shape[:1], math.inf, dtype=torch.float64, device="cuda")
+        for P in nets:
+            z1, z2, _, _, _ = ppo64.forward(P, xc)
+            one = torch.ones_like(z1)
+            m1 = ppo64.forward_mag(P, xc, (one, one))[0]
+            m2 = ppo64.forward_mag(P, xc, ((z1 > 0).double(), one))[1]
+            c = torch.minimum(c, torch.minimum((z1.abs() / m1).amin(1), (z2.abs() / m2).amin(1)))
+        out.append(c)
+    return torch.cat(out)
+
+
+def _batch(p, n, seed, trap_rows=(), relu_margin=0.0):
     """A DeviceBatch of n synthetic rows at the policy's current parameters: actions drawn from the policy, logp_old
     set so that the ratios fall in RATIO_BANDS, stored values VOFF_BANDS away from the critics, and advantages of
-    40 / -30 on the batch rows trap_rows."""
+    40 / -30 on the batch rows trap_rows.  With relu_margin, the observations of every row with a hidden
+    pre-activation closer to zero than relu_margin (_relu_clearance) are redrawn until none is; b.redrawn counts
+    those rows and b.clearance is the least clearance left."""
     from fsrl_b200.policy.base_policy import DeviceBatch
     s0 = p.arena.slots[0]
     D, A, C = s0.D, s0.out, p.critics_num
@@ -144,7 +171,15 @@ def _batch(p, n, seed, trap_rows=()):
     g = torch.Generator(device="cuda").manual_seed(seed)
     obs = torch.randn(n, D, generator=g, device="cuda")
     nets = _split(p, _d(p.arena.theta))
-    outs = [ppo64.forward(P, _d(obs))[4] for P in nets]
+    redrawn = torch.zeros(n, dtype=torch.bool, device="cuda")
+    while relu_margin:
+        clearance = _relu_clearance(nets, _d(obs))
+        bad = clearance < relu_margin
+        if not bad.any():
+            break
+        redrawn |= bad
+        obs[bad] = torch.randn(int(bad.sum()), D, generator=g, device="cuda")
+    outs = [torch.cat([ppo64.forward(P, xc)[4] for xc in _d(obs).split(ROW_CHUNK)]) for P in nets]
     mu = o.max_action * torch.tanh(outs[0]) if o.bounded else outs[0]
     ls = nets[0]["ls"]
     act = (mu + ls.exp() * torch.randn(n, A, generator=g, device="cuda", dtype=torch.float64)).float()
@@ -163,6 +198,9 @@ def _batch(p, n, seed, trap_rows=()):
         if C > 1:
             b.adv[1, r] = -30.0
     b.values, b.rets, b.advs = b.v.t(), b.ret.t(), b.adv.t()
+    b.redrawn = int(redrawn.sum())
+    if relu_margin:
+        b.clearance = float(clearance.min())
     return b
 
 
@@ -172,8 +210,14 @@ def _learn(p, batch, bs, seed, repeat=1):
     return {k: np.asarray(v, dtype=np.float64) for k, v in p.last_stats.items()}
 
 
+def _perms(seed, n, repeat):
+    """the minibatch permutations of the first `repeat` repeats of a learn after np.random.seed(seed)"""
+    rs = np.random.RandomState(seed)
+    return [torch.from_numpy(rs.permutation(n)).cuda() for _ in range(repeat)]
+
+
 def _perm(seed, n):
-    return torch.from_numpy(np.random.RandomState(seed).permutation(n)).cuda()
+    return _perms(seed, n, 1)[0]
 
 
 def _scratch(p, net, B):
@@ -198,8 +242,10 @@ def _theta_before_beta0(p):
 
 
 def _rows(batch, idx):
-    return ppo64.Rows(act=_d(batch.act[idx]), lpo=_d(batch.logp_old[idx]), adv=_d(batch.adv[:, idx]),
-                      ret=_d(batch.ret[:, idx]), values=_d(batch.v[:, idx]))
+    """the batch rows idx [B], or M minibatches of them [M][B], in the layout of ppo64.Rows"""
+    cols = lambda t: _d(t[:, idx]).movedim(0, -2)
+    return ppo64.Rows(act=_d(batch.act[idx]), lpo=_d(batch.logp_old[idx]), adv=cols(batch.adv), ret=cols(batch.ret),
+                      values=cols(batch.v))
 
 
 def _err(got, ref, scale, floor=0.0):
@@ -217,16 +263,19 @@ def _kinks(o, stats, R, v_dev):
     out = float(d.min())
     if o.value_clip:
         for i, v in enumerate(v_dev):
-            off = v - R.values[i]
+            off = v - R.values[..., i, :]
             out = min(out, float(torch.minimum((off - o.eps_clip).abs(), (off + o.eps_clip).abs()).min()))
     return out
 
 
 def _stat_errs(o, stats, st, row, errs):
+    """the logged statistics of step row (or of the steps row of [M] minibatch statistics); keeps the worst"""
     keys = ["actor_rew", "kl", "entropy", "total"] + ["vf%d" % i for i in range(o.C)] + \
         (["actor_safety"] if o.use_saf else [])
+    f64 = lambda v: torch.as_tensor(v, dtype=torch.float64, device="cuda")
     for k in keys:
-        errs["stat." + k] = abs(float(st["loss/" + k][row]) - stats[k]) / max(stats["s_" + k], FLT_MIN)
+        e = float(((f64(st["loss/" + k][row]) - f64(stats[k])).abs() / f64(stats["s_" + k]).clamp(min=FLT_MIN)).max())
+        errs["stat." + k] = max(errs.get("stat." + k, 0.0), e)
 
 
 def _check_chain(p, batch, theta, idx, mb, g_dev, st, row, clip=None):
@@ -294,7 +343,7 @@ def _check_chain(p, batch, theta, idx, mb, g_dev, st, row, clip=None):
 
 
 TOLS = {"mom": MOM_TOL, "fwd": FWD_TOL, "head": DOUT_TOL, "bwd": BWD_TOL, "wgrad": GRAD_TOL, "norm": NORM_TOL,
-        "stat": STAT_TOL, "pgrad": PGRAD_TOL, "adam": ULP_TOL}
+        "stat": STAT_TOL, "pgrad": PGRAD_TOL, "adam": ULP_TOL, "adam_m": M_TOL, "adam_v": V_TOL}
 
 
 def _report(label, errs):
@@ -427,10 +476,17 @@ def _check_persist(p, batch, theta, idx, g_dev, st, row):
     return errs
 
 
+def _persistent(p, batch, n, bs):
+    """whether a learn of n rows in minibatches of bs takes the persistent launch"""
+    from fsrl_b200 import _lib
+    p._ensure_update_state(bs, n, 1)
+    u = p._descriptor(batch, torch.zeros(batch.n, dtype=torch.int32, device="cuda"))
+    return _lib.lib.fsrl_ppo_persist_active(ctypes.byref(u), n, bs) == 1
+
+
 @pytest.mark.parametrize("name", list(PERSIST))
 def test_persistent_launch(name):
     """One 256-row step, then a 4-step launch whose last step is checked at the recovered parameters."""
-    from fsrl_b200 import _lib
     A, D, kw = PERSIST[name]
     H, bs = 256, 256
     p = _policy(D, A, H, betas=(0.0, 0.0), persist=True, **kw)
@@ -438,9 +494,7 @@ def test_persistent_launch(name):
         seed = 31 + n + A + D
         perm = _perm(seed, n)
         batch = _batch(p, n, seed, trap_rows=[int(perm[n - 1])])
-        p._ensure_update_state(bs, n, 1)
-        u = p._descriptor(batch, torch.zeros(n, dtype=torch.int32, device="cuda"))
-        assert _lib.lib.fsrl_ppo_persist_active(ctypes.byref(u), n, bs) == 1
+        assert _persistent(p, batch, n, bs)
         theta0 = _d(p.arena.theta).clone()
         st = _learn(p, batch, bs, seed)
         k = n // bs
@@ -517,3 +571,156 @@ def test_observation_wider_than_the_engine_is_refused():
     with pytest.raises(ValueError, match="observation width %d" % D):
         p = _policy(D, 2, 64)
         _learn(p, _batch(p, 64, 1), 64, 1)
+
+
+# ---- 6. long launches ------------------------------------------------------------------------------------------
+# At lr = 0 theta stays theta0 bit for bit while every step still runs its whole Adam path (the step is -(0 / bc1)
+# times the moment ratio), so step k of repeat r is the float64 update of the rows perm_r[256 k : 256 (k + 1)] at
+# theta0.  Each step's statistics are checked against their own float64 values, and Adam's m and v after the learn
+# against the float64 recurrence over every step's clipped gradient (v remembers about the last 1000 steps): every
+# gradient element of every step, every minibatch index, statistics slot and operand image of the launch is tied to a
+# check.  The rows keep every hidden pre-activation of every net RELU_MARGIN clear of zero at theta0, so the float64
+# ReLU masks are the device's at every step; the ratios and value offsets stay KINK clear of the loss's kinks.
+MAX_MB = 16384       # minibatches of one persistent launch (pp::MAX_MB in csrc/ppo_persist.cu)
+RELU_MARGIN = 1e-5   # least |z| / magnitude chain of a hidden pre-activation: over 10x the forward error (6.5e-7)
+# name: (D, A, H, n, repeat, persistent, policy options); batch_size 256, max_grad_norm 0.5
+LONG = {
+    "c2": (8, 2, 256, 2048 * 300, 4, True, {}),
+    "c2-chain": (8, 2, 256, 2048 * 300, 4, False, {}),
+    "c5-chain": (34, 8, 512, 1024 * 500, 1, False, {}),
+    "gate-top": (40, 8, 256, MAX_MB * 256, 1, True, {}),
+    "one-critic": (8, 3, 256, 64 * 256, 2, True, dict(C=1, bounded=False, value_clip=True, dual_clip=1.5,
+                                                     reward_normalization=True)),
+}
+
+
+def _check_long(p, batch, theta0, perms, st):
+    """every step of a learn at lr = 0 that started from zero Adam moments, against float64: each step's statistics
+    and gradient norm, and m, v after the last step against the recurrence over every step's clipped gradient.
+    A group's m (v) is measured against the same recurrence run on the group's gradient scale (squared)."""
+    o = _opts(p)
+    nets = _split(p, theta0)
+    b1, b2 = p.optim.param_groups[0]["betas"]
+    bs, H = 256, p.arena.slots[0].H
+    n_mb = batch.n // bs
+    T = len(perms) * n_mb
+    assert len(st["loss/kl"]) == T
+    f64 = lambda v: torch.as_tensor(v, dtype=torch.float64, device="cuda")
+    m64 = [{k: torch.zeros_like(v) for k, v in P.items()} for P in nets]
+    v64 = [{k: torch.zeros_like(v) for k, v in P.items()} for P in nets]
+    mmag = [dict.fromkeys(P, 0.0) for P in nets]
+    vmag = [dict.fromkeys(P, 0.0) for P in nets]
+    errs, margin, clip = {"norm": 0.0}, math.inf, p._grad_norm
+    chunk = 65536 // H                                 # minibatches per float64 evaluation
+    for r, perm in enumerate(perms):
+        for k0 in range(0, n_mb, chunk):
+            M = min(chunk, n_mb - k0)
+            idx = perm[k0 * bs:(k0 + M) * bs].view(M, bs)
+            steps = r * n_mb + k0 + np.arange(M)
+            R = _rows(batch, idx)
+            stats, gref, gmag = ppo64.gradients(o, nets, _d(batch.obs[idx]), R)
+            margin = min(margin, _kinks(o, stats, R, stats["v"]))
+            gn = sum((g ** 2).flatten(1).sum(1) for G in gref for g in G.values()).sqrt()
+            scale = (clip / (gn + 1e-6)).clamp(max=1.0) if clip else torch.ones_like(gn)
+            errs["norm"] = max(errs["norm"], float(((f64(st["loss/grad_norm"][steps]) - gn).abs() / gn).max()))
+            _stat_errs(o, stats, st, steps, errs)
+            j = f64(steps)
+            w1, w2 = (1 - b1) * b1 ** (T - 1 - j), (1 - b2) * b2 ** (T - 1 - j)
+            for i, G in enumerate(gref):
+                for key, g in G.items():
+                    sg = scale.view(-1, *[1] * (g.dim() - 1)) * g
+                    smax = scale * gmag[i][key].flatten(1).amax(1)
+                    m64[i][key] += torch.tensordot(w1, sg, dims=1)
+                    v64[i][key] += torch.tensordot(w2, sg * sg, dims=1)
+                    mmag[i][key] += float((w1 * smax).sum())
+                    vmag[i][key] += float((w2 * smax ** 2).sum())
+    md, vd = _split(p, _d(p.optim.m)), _split(p, _d(p.optim.v))
+    for i in range(len(nets)):
+        for key in nets[i]:
+            errs["adam_m.%d.%s" % (i, key)] = float((md[i][key] - m64[i][key]).abs().max()) / mmag[i][key]
+            errs["adam_v.%d.%s" % (i, key)] = float((vd[i][key] - v64[i][key]).abs().max()) / vmag[i][key]
+    return errs, margin
+
+
+@pytest.mark.parametrize("name", list(LONG))
+def test_long_launch_every_step(name):
+    """Every step of a long learn at lr = 0 against float64; on the c2 shape, Adam's step at t = 4 x 2400 + 1."""
+    D, A, H, n, repeat, persist, kw = LONG[name]
+    bs, seed = 256, 41
+    t_start = time.perf_counter()
+    p = _policy(D, A, H, lr=0.0, betas=(0.9, 0.999), persist=persist, max_grad_norm=0.5, **kw)
+    batch = _batch(p, n, seed, relu_margin=RELU_MARGIN)
+    assert batch.clearance >= RELU_MARGIN
+    theta0 = p.arena.theta.detach().clone()
+    assert _persistent(p, batch, n, bs) == persist
+    st = _learn(p, batch, bs, seed, repeat)
+    assert torch.equal(p.arena.theta, theta0)               # lr = 0: the parameters never move
+    assert p.optim.step_count == repeat * (n // bs)
+    errs, margin = _check_long(p, batch, _d(theta0), _perms(seed, n, repeat), st)
+    assert margin > KINK, margin
+    if name.startswith("c2"):
+        # one more 256-row learn at lr 5e-4: Adam at a large t, from the device's own m and v
+        p.optim.param_groups[0]["lr"] = LR
+        one = _batch(p, bs, seed + 1)
+        assert _persistent(p, one, bs, bs) == persist
+        t = p.optim.step_count + 1
+        _learn(p, one, bs, seed)
+        assert p.optim.step_count == t
+        b1, b2 = p.optim.param_groups[0]["betas"]
+        m, v = _d(p.optim.m), _d(p.optim.v)
+        pr = _d(theta0) - LR / (1 - b1 ** t) * m / (v.sqrt() / math.sqrt(1 - b2 ** t) + p.optim.param_groups[0]["eps"])
+        errs["adam.theta"] = _ulps(_d(p.arena.theta), pr, pr.abs() + LR)
+    T = repeat * (n // bs)
+    _report(f"long {name} {'persistent' if persist else 'chain'} D={D} A={A} H={H} n={n} repeat={repeat}: {T} steps, "
+            f"{batch.redrawn} rows redrawn for the ReLU margin (clearance {batch.clearance:.1e}), kink margin "
+            f"{margin:.2e}, {time.perf_counter() - t_start:.1f} s", errs)
+
+
+def test_persistent_launch_is_deterministic():
+    """A c2-shaped learn (4 repeats of 2400 steps, lr 5e-4, betas (0.9, 0.999)) twice from the same state: theta, m
+    and v bit for bit, so that every step read the parameters the step before it published; the statistics, summed
+    with atomics, to a relative 1e-6 of each statistic's largest value."""
+    n, bs, seed = 2048 * 300, 256, 43
+    p = _policy(8, 2, 256, betas=(0.9, 0.999), persist=True, max_grad_norm=0.5)
+    batch = _batch(p, n, seed)
+    assert _persistent(p, batch, n, bs)
+    start = [t.detach().clone() for t in (p.arena.theta, p.optim.m, p.optim.v)]
+    runs = []
+    for _ in range(2):
+        for t, s in zip((p.arena.theta, p.optim.m, p.optim.v), start):
+            t.data.copy_(s)
+        p.optim.step_count = 0
+        p._mirror_dirty = True
+        st = _learn(p, batch, bs, seed, repeat=4)
+        runs.append(([t.detach().clone() for t in (p.arena.theta, p.optim.m, p.optim.v)], st))
+    (s0, st0), (s1, st1) = runs
+    assert len(st0["loss/kl"]) == 4 * n // bs
+    assert float((s0[0] - start[0]).abs().max()) > 100 * LR        # the parameters moved
+    for name, a, b in zip(("theta", "m", "v"), s0, s1):
+        assert torch.equal(a, b), (name, float((a - b).abs().max()))
+    worst = max(float(np.abs(st0[k] - st1[k]).max() / max(np.abs(st0[k]).max(), FLT_MIN)) for k in st0)
+    print(f"\ndeterminism: theta, m, v bit-identical; statistics {worst:.1e}/1e-06", end="")
+    assert worst <= 1e-6
+
+
+# (D, A, H, C, n, batch_size, persistent)
+GATE = {
+    "c2": (8, 2, 256, 2, 2048 * 300, 256, True),
+    "top": (40, 8, 256, 2, MAX_MB * 256, 256, True),
+    "one-critic": (8, 3, 256, 1, 64 * 256, 256, True),
+    "max-mb+1": (40, 8, 256, 2, (MAX_MB + 1) * 256, 256, False),
+    "merged-tail": (8, 2, 256, 2, 2048 * 300 + 128, 256, False),
+    "bs128": (8, 2, 256, 2, 2048 * 300, 128, False),
+    "bs512": (8, 2, 256, 2, 2048 * 300, 512, False),
+    "h128": (8, 2, 128, 2, 2048 * 300, 256, False),
+    "h512": (8, 2, 512, 2, 2048 * 300, 256, False),
+    "D41": (41, 2, 256, 2, 2048 * 300, 256, False),
+}
+
+
+@pytest.mark.parametrize("name", list(GATE))
+def test_persistent_gate(name):
+    """which learns the persistent launch takes, the rest going to the chain"""
+    D, A, H, C, n, bs, want = GATE[name]
+    p = _policy(D, A, H, C=C, persist=True)
+    assert _persistent(p, _batch(p, 256, 1), n, bs) == want
